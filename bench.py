@@ -1,11 +1,11 @@
 #!/usr/bin/env python3
-"""bench.py — queries/sec and GB/s of the VectorBase top-k lookup on B200.
+"""bench.py — queries/sec and GB/s of the VectorBase top-k lookup on an H100.
 
 One "step" = one pass of the hot path over one batch of synthetic queries:
 the whole corpus is scored against B queries and the k best rows per query are returned.
 
 Default workload (BASELINE.json `metric`: "top-k cosine on 10M x 768"): configs[2] =
-10M x 768 bf16 corpus, batch 256, top-100, on one B200.  With --gpus N (launched by
+10M x 768 bf16 corpus, batch 256, top-100, on one H100.  With --gpus N (launched by
 torch.distributed.run, one rank per GPU) the SAME corpus is row-sharded over the N GPUs
 (strong scaling): every rank searches its rows, per-rank candidates are exchanged and merged on
 every rank.
@@ -18,13 +18,16 @@ Output: ONE JSON line (rank 0).
   roofline   the dominant kernel's algorithmic bytes / its event-timed duration — events recorded
              by libtavec around that kernel INSIDE the timed region of `value` (same pass, so
              kernel_ms_per_step <= ms_per_step by construction) — against MEASURED_PEAKS.json;
-             `sustained` repeats it over >= 2 s of back-to-back steps (the power-capped figure);
+             `sustained` repeats it over >= 2 s of back-to-back steps (the figure under the card's
+             power limit);
   cpu_baseline  the reference's own VectorBase (unmodified file, vendored under oracle/_ref by
              build(); else the numpy restatement) on this box's host cores over the FULL corpus;
   parity_checked  4 queries of the final step compared with the blocked numpy oracle over the
              device corpus at the contract tolerances;
   secondary  the other single-GPU BASELINE configs (c1, c2, c5; c4 at 8 GPUs), each with its own
-             value / e2e / roofline / cpu_baseline.
+             value / e2e / roofline / cpu_baseline, timed over the same --steps.
+`--dump-outputs DIR` writes what the last timed step of the main workload returned to DIR/<name>.npy;
+inputs are seeded, so two builds run with the same arguments can be compared output for output.
 `--impl reference` times the reference's CPU path alone (same metric / config strings, so the
 driver can divide).
 """
@@ -86,6 +89,8 @@ def parse_args():
     p.add_argument("--no-parity", action="store_true", help="skip the blocked-oracle check of the final step")
     p.add_argument("--sustain-seconds", type=float, default=2.0, help="0 disables the sustained roofline run")
     p.add_argument("--cpu-queries", type=int, default=8, help="timed single-query lookups of the cpu_baseline leg")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write the outputs of the last timed step of the main workload as DIR/<name>.npy")
     return p.parse_args()
 
 
@@ -100,20 +105,6 @@ def algorithmic_bytes(rows, dim, storage, batch, k):
     return rows * dim * ELEM[storage] + batch * dim * 4 + batch * k * 12
 
 
-def load_ncu_traffic(workload, path, world, rows):
-    """dram bytes per launch of the dominant kernel from the committed ncu capture, or None."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            table = json.load(f)
-    except Exception:
-        return None
-    key = f"{workload}/{path}/{world}"
-    if rows != WORKLOADS[workload]["rows"]:
-        key = f"{workload}-shard-{rows}/{path}/{world}"
-    entry = table.get(key)
-    return entry["bytes"] if entry else None
-
-
 def load_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
@@ -121,7 +112,8 @@ def load_peaks():
             p = json.load(f)
         return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p.get("bf16_tflops"),
                 "bf16_tflops_sustained": p.get("bf16_tflops_sustained"), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA's H100 SXM data sheet (700 W): HBM3 bandwidth and dense BF16 tensor rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": None, "source": "fallback"}
 
 
 def workload_config(w, n_gpus):
@@ -129,7 +121,7 @@ def workload_config(w, n_gpus):
         "workload": w["desc"], "rows": w["rows"], "dim": w["dim"], "storage": w["storage"],
         "batch": w["batch"], "k": w["k"], "min_score": w["min_score"],
         "parallelism": f"row-sharded x{n_gpus}, candidate exchange + merge on every rank" if n_gpus > 1 else "single GPU",
-        "l2": "corpus shard >> 126 MB L2, no flush needed" if w["rows"] * w["dim"] * ELEM[w["storage"]] / n_gpus > 4e8
+        "l2": "corpus shard >> 50 MB L2, no flush needed" if w["rows"] * w["dim"] * ELEM[w["storage"]] / n_gpus > 4e8
               else "corpus fits L2: L2 flushed (256 MB write) between timed steps",
     }
 
@@ -428,7 +420,8 @@ class Bench:
             self.dist.destroy_process_group()
 
 
-def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, parity=True, cpu=True, cpu_queries=8):
+def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, parity=True, cpu=True, cpu_queries=8,
+            dump_dir=None):
     """One workload on the GPUs of this run -> the result dict (rank 0) or None (other ranks)."""
     import typeagent_py_b200 as tab
     from typeagent_py_b200.sharded import ShardedVectorBase, shard_bounds
@@ -477,6 +470,7 @@ def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, par
         return sharded.search_tensors(q_dev, k, w["min_score"], defer_check=True)
 
     fallbacks = [0]
+    last = [None]   # (items, scores, counts) of the most recent resident step
 
     def finish_resident():
         # exact fallbacks are legitimate (probability ~1e-7 per query) and their cost stays in the
@@ -523,7 +517,7 @@ def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, par
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for i in range(n_steps):
-                step_resident()
+                last[0] = step_resident()
                 if (i & 7) == 7:
                     finish_resident()      # at most 8 (sharded) / 64 searches may be outstanding
             finish_resident()
@@ -535,7 +529,7 @@ def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, par
             bn.barrier()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            step_resident()
+            last[0] = step_resident()
             finish_resident()
             e1.record()
             bn.barrier()
@@ -552,6 +546,8 @@ def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, par
     sampler = ClockSampler(bn.local_rank) if rank == 0 else None
     ms_resident = bn.max_over_ranks(timed_resident(steps))
     hist = history(steps)                       # the SAME pass as ms_resident
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, *last[0])
     # rank-to-rank spread of the local search (a sharded step ends when the SLOWEST rank has published)
     per_rank = None
     if world > 1:
@@ -639,7 +635,7 @@ def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, par
     algo_launch_bytes = (hi - lo) * dim * ELEM[storage] * passes + batch * dim * 4 + batch * k * 12
     achieved = algo_bytes / (kernel_ms / 1e3) / 1e9
     flops = 2.0 * batch * (hi - lo) * dim
-    tensor_bound = path in ("mma", "mma_split") and flops / (peaks["bf16_tflops"] or 1.6e3) / 1e12 > \
+    tensor_bound = path in ("mma", "mma_split") and flops / (peaks["bf16_tflops"] or 989.0) / 1e12 > \
         algo_bytes / peaks["hbm_gbs"] / 1e9 * 1.25
     out = {
         "metric": metric_string(w),
@@ -663,7 +659,7 @@ def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, par
         "roofline": {
             "bound": "hbm", "kernel": "scan_rows_kernel" if path == "scan" else "mma_topk_kernel (" + path + ")",
             "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"],
-            "of": peaks["source"], "traffic": load_ncu_traffic(name, path, world, rows),
+            "of": peaks["source"],
             "kernel_ms_per_step": kernel_ms,
             "search_ms_per_step_same_pass": statistics.fmean(hist["search_total"]) if hist["search_total"] else None,
             "per_step_ms_by_kernel_kind": breakdown,
@@ -672,7 +668,7 @@ def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, par
             "algorithmic_bytes_per_step": algo_bytes,
             "bytes_actually_requested_per_step": algo_launch_bytes,
             "note": "achieved = algorithmic bytes (corpus shard read once per batch) / duration of the dominant "
-                    "kernel (the MAIN launch of the tcgen05 kernel, or the row-scan kernel), CUDA events recorded by "
+                    "kernel (the MAIN launch of the tensor-core kernel, or the row-scan kernel), CUDA events recorded by "
                     "libtavec around it inside the timed region of `value` (same pass)" + ("" if passes == 1 else
                     f"; the row-scan path re-reads the corpus once per 8 queries ({passes} passes)"),
         },
@@ -698,7 +694,7 @@ def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, par
             **sustained, "achieved": s_ach, "frac": s_ach / peaks["hbm_gbs"] if s_ach else None,
             "value": batch / (sustained["ms_per_step"] / 1e3),
             "note": "same measurement over >= 2 s of back-to-back steps (kernel_ms = mean of the last 64): the "
-                    "figure under the 1 kW power cap"}
+                    "figure under the card's power limit"}
         if peaks.get("bf16_tflops_sustained") and sustained["kernel_ms"]:
             out["roofline"]["sustained"]["tensor_frac_of_sustained"] = \
                 flops / (sustained["kernel_ms"] / 1e3) / 1e12 / peaks["bf16_tflops_sustained"]
@@ -706,6 +702,14 @@ def measure(bn: Bench, name, w, steps, warmup, *, force=None, sustain_s=0.0, par
         leg = cpu_reference_leg(w, warmup=3, timed=cpu_queries, want_batched=True)
         out["cpu_baseline"] = cpu_baseline_block(leg)
     return out
+
+
+def dump_outputs(dump_dir, items, scores, counts):
+    """The arrays a caller of the timed path receives, as float32 / float64 .npy files."""
+    os.makedirs(dump_dir, exist_ok=True)
+    np.save(os.path.join(dump_dir, "items.npy"), items.cpu().numpy().astype(np.float64))
+    np.save(os.path.join(dump_dir, "scores.npy"), scores.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(dump_dir, "counts.npy"), counts.cpu().numpy().astype(np.float64))
 
 
 def check_parity(bn, corpus, lo, qn, items, scores, counts, k, min_score, storage):
@@ -738,14 +742,15 @@ def run_b200(args, w):
     bn = Bench(args)
     force = None if args.path == "auto" else args.path
     out = measure(bn, args.workload, w, args.steps, args.warmup, force=force, sustain_s=args.sustain_seconds,
-                  parity=not args.no_parity, cpu=not args.no_cpu_baseline, cpu_queries=args.cpu_queries)
+                  parity=not args.no_parity, cpu=not args.no_cpu_baseline, cpu_queries=args.cpu_queries,
+                  dump_dir=args.dump_outputs)
     # the other BASELINE configs ride along so that the driver's records carry them
     secondary = {}
     if not args.no_secondary and args.workload == "c3" and args.rows is None:
         names = ["c1", "c2", "c5"] if bn.world == 1 else (["c4"] if bn.world == 8 else [])
         for name in names:
             sw = dict(WORKLOADS[name])
-            res = measure(bn, name, sw, steps=max(args.steps, 10), warmup=max(args.warmup, 3), sustain_s=0.0,
+            res = measure(bn, name, sw, steps=args.steps, warmup=max(args.warmup, 3), sustain_s=0.0,
                           parity=not args.no_parity, cpu=not args.no_cpu_baseline, cpu_queries=args.cpu_queries)
             if res is not None:
                 keep = ("metric", "value", "unit", "ms_per_step", "path", "e2e", "roofline", "cpu_baseline",

@@ -1,5 +1,5 @@
 /*
- * tavec.h — C ABI of libtavec.so, the B200 (sm_100a) engine behind typeagent's
+ * tavec.h — C ABI of libtavec.so, the H100 (sm_90a) engine behind typeagent's
  * VectorBase top-k lookup.
  *
  * This is the drop-in boundary for ONE path of microsoft/typeagent-py:
@@ -63,7 +63,7 @@ enum tav_search_flags {
     TAV_QUERIES_ON_DEVICE = 1, /* `queries` is a device pointer (float32 [n_queries, dim]) */
     TAV_OUTPUTS_ON_DEVICE = 2, /* out_* are device pointers; no synchronisation */
     TAV_FORCE_SCAN = 4,        /* use the CUDA-core row-scan kernels whatever the shape */
-    TAV_FORCE_MMA = 8,         /* use the tcgen05 tensor-core kernel (needs dim % 8 == 0, no subset) */
+    TAV_FORCE_MMA = 8,         /* use the wgmma tensor-core kernel (needs dim % 8 == 0, no subset) */
     /* Fully asynchronous tensor-core search (needs both ..._ON_DEVICE flags): the check whether
      * some query must be redone by the exact row scan — a host synchronisation — is left to
      * tav_finish_search.  Until then the outputs of such (rare) queries are not final. */
@@ -78,10 +78,7 @@ enum tav_search_flags {
     /* Do not use the single-launch form of the row scan (one host query, host outputs: the query
      * rides in the kernel parameters and the last CTA merges); tests use it to reach the two-kernel
      * form with one query. */
-    TAV_NO_FUSED_SCAN = 128,
-    /* Tensor-core path: keep the query block in shared memory (re-fetched per corpus tile) instead of
-     * parking it in tensor memory; diagnostic / test switch for the Q-stationary form. */
-    TAV_NO_TMEM_QUERIES = 256
+    TAV_NO_FUSED_SCAN = 128
 };
 
 int tav_abi_version(void);
@@ -219,9 +216,9 @@ int tav_set_timing(tav_index* ix, int enabled);
 
 /* Device time of the last tav_search on this index, measured with CUDA events on the
  * search's stream: `scan_ms` = the dominant kernel (row-scan kernel, or the MAIN launch of the
- * tcgen05 kernel; summed over query chunks), `total_ms` = first launch to last result byte on
+ * tensor-core kernel; summed over query chunks), `total_ms` = first launch to last result byte on
  * device (both -1 when timing is off); `launches` = kernels launched; `path` = 1 row-scan
- * kernels, 2 tcgen05 kernel on bf16/fp16 rows, 3 tcgen05 kernel on a float32 index through
+ * kernels, 2 tensor-core kernel on bf16/fp16 rows, 3 tensor-core kernel on a float32 index through
  * its two fp16 planes (x = hi + lo/2048, ~2^-22 relative).  Synchronises when timing is on. */
 int tav_last_timing(tav_index* ix, float* scan_ms, float* total_ms, int* launches, int* path);
 

@@ -1,6 +1,6 @@
 """Shared pytest configuration.
 
-Markers: ``gpu`` — needs a CUDA device (run on the B200 box with ``-m gpu``);
+Markers: ``gpu`` — needs a CUDA device (an H100; run with ``-m gpu``);
 everything else must pass on a CPU-only container (``-m "not gpu"``).
 """
 
@@ -17,7 +17,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (B200)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (H100)")
 
 
 def _cuda_available() -> bool:

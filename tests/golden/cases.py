@@ -10,6 +10,7 @@ benchmark does (tools/benchmark_vectorbase.py:80-94).
 
 from __future__ import annotations
 
+import json
 import os
 
 import numpy as np
@@ -17,10 +18,22 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 EPISODE53_FILE = os.path.join(HERE, "episode53_excerpt.npy")
 GOLDEN_FILE = os.path.join(HERE, "golden_cases.json")
+EPISODE53_GOLDEN_FILE = os.path.join(HERE, "golden_episode53.json")
 
 # rows of tests/testdata/Episode_53_AdrianTchaikovsky_index_embeddings.bin kept in the
-# excerpt: the first 300 related-term rows and all 106 message-chunk rows (1188..1293)
-EPISODE53_ROWS = list(range(300)) + list(range(1188, 1294))
+# excerpt (kept under 1 MB): the first 100 related-term rows and the first 50 message-chunk rows
+# (1188..1237)
+EPISODE53_ROWS = list(range(100)) + list(range(1188, 1238))
+
+
+def load_golden() -> dict:
+    """The recorded reference outputs: ``golden_cases.json``, with the Episode-53 case taken from its
+    own file, recorded over the excerpt as stored now."""
+    with open(GOLDEN_FILE) as f:
+        golden = json.load(f)
+    with open(EPISODE53_GOLDEN_FILE) as f:
+        golden["cases"]["episode53"] = json.load(f)
+    return golden
 
 
 def unit_rows(rng, n, d):
@@ -52,7 +65,7 @@ def episode53():
     # queries: a few term rows and a few message rows, slightly perturbed so that the
     # best hit is not a trivial exact duplicate with score 1.0 only
     rng = np.random.default_rng(53)
-    picks = [0, 7, 123, 299, 300, 350, 405]
+    picks = [0, 7, 63, 99, 100, 125, 149]
     q = v[picks] + 0.05 * unit_rows(rng, len(picks), v.shape[1])
     q /= np.linalg.norm(q, axis=1, keepdims=True)
     return v, q.astype(np.float32)
@@ -104,7 +117,7 @@ CASES: list[dict] = [
          lookups=[("lookup", dict(max_hits=50, min_score=0.85)),
                   ("lookup", dict(max_hits=10, min_score=0.7)),
                   ("lookup", dict(max_hits=25, min_score=0.0)),
-                  ("subset", dict(subset=("range", 300, 406), max_hits=25, min_score=0.7))]),
+                  ("subset", dict(subset=("range", 100, 150), max_hits=25, min_score=0.7))]),
 ]
 
 

@@ -5,8 +5,8 @@ Run in the build container only (needs /root/reference):
 
     python tests/golden/make_golden.py
 
-Writes ``golden_cases.json`` (reference outputs: items + float32 scores as Python
-floats, which round-trip exactly through JSON) and ``episode53_excerpt.npy`` (406 of
+Writes ``golden_cases.json`` and ``golden_episode53.json`` (reference outputs: items + float32 scores as Python
+floats, which round-trip exactly through JSON) and ``episode53_excerpt.npy`` (150 of
 the 1294 real embedding rows of the reference's Episode-53 test fixture).  Also records
 the reference's own known-answer tests as literal cases.
 """
@@ -67,6 +67,8 @@ def main() -> None:
     assert kat == {"items": [0, 1, 2], "scores": [1.0, 0.5, 0.0]}, kat
     out["known_answer_score_scale"] = kat
 
+    with open(C.EPISODE53_GOLDEN_FILE, "w") as f:
+        json.dump(out["cases"].pop("episode53"), f)
     with open(C.GOLDEN_FILE, "w") as f:
         json.dump(out, f)
     print("wrote", C.GOLDEN_FILE, os.path.getsize(C.GOLDEN_FILE), "bytes")

@@ -5,7 +5,7 @@ real batch of 1024, config 5):
     (the reference's np.dot / clip / flatnonzero / argpartition, tests/parity.blocked_oracle_lookup)
     ranks a handful of the batch's queries — including a planted one — at the contract tolerances
     (scores 1e-4, ties 2e-6; aitools/vectorbase.py:163-190, tools/benchmark_vectorbase.py:80-94);
-  * two independent CUDA paths agree: the tcgen05 kernel vs the exact row-scan kernel, on the
+  * two independent CUDA paths agree: the tensor-core kernel vs the exact row-scan kernel, on the
     same device-resident corpus, for a handful of the batch's queries (identical index sets up
     to float32 summation-order ties, scores within 2e-6);
   * planted rows: exact copies of some queries overwrite known rows and must come back first

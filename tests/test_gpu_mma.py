@@ -1,4 +1,4 @@
-"""The tcgen05 tensor-core path (bf16 / fp16 storage, batched queries) against the oracle.
+"""The wgmma tensor-core path (bf16 / fp16 storage, batched queries) against the oracle.
 
 Inputs are rounded to the storage dtype first ("identical fp32 inputs": the oracle gets the
 rounded values upcast to float32), so products are exact in float32 and only the summation
@@ -302,31 +302,33 @@ def test_split_values_beyond_fp16_range_fall_back_to_the_exact_scan():
         assert_hits_match(got, O.lookup(O.make_corpus(8000, 64, seed=4)[0], qq, 10, 0.0))
 
 
-# ------------------------------------------------------------------ Q-stationary form (queries in tensor memory)
+# ------------------------------------------------------------------ many query chunks against the exact row scan
 @pytest.mark.parametrize("storage,n,d,b,k,ms", [
-    ("bfloat16", 30000, 768, 256, 100, 0.0),     # N = 64 tiles (384 TMEM columns of queries), the config-3 shape
-    ("float16", 50000, 384, 1000, 5, 0.0),       # N = 128 tiles, four query chunks (config 5)
+    ("bfloat16", 30000, 768, 256, 100, 0.0),     # the config-3 shape, two query chunks
+    ("float16", 50000, 384, 1000, 5, 0.0),       # eight query chunks (config 5)
     ("bfloat16", 20011, 136, 130, 10, 0.0),      # ragged K (136 = 2 slices + 8) and a ragged last tile
     ("float16", 777, 512, 200, 30, 0.0),         # small corpus: no sampling, most units idle
     ("bfloat16", 40000, 64, 300, 8, 0.55),       # one K slice; threshold from min_score
-    ("bfloat16", 33000, 640, 129, 64, 0.0),      # 320 query columns -> N = 64
+    ("bfloat16", 33000, 640, 129, 64, 0.0),      # one query past a full chunk
 ])
 def test_queries_in_tensor_memory_form(storage, n, d, b, k, ms):
-    """More than 128 queries on 16-bit storage with D <= 768 run MAIN with the query block parked in
-    TMEM (A operand from tensor memory); it must agree with the smem-operand form and the oracle."""
+    """More than 128 queries on 16-bit storage spread over several query chunks of the tensor-core
+    kernel; it must agree with the exact row-scan kernels and the oracle, also under a row mask.
+    (The name dates from a kernel form that parked the query block in tensor memory; the shapes
+    that covered it are kept under the same test ids.)"""
     v, q = O.make_corpus(n, d, seed=n + d + b, n_queries=b)
     vr, qr = O.round_to_storage(v, storage), O.round_to_storage(q, storage)
     ts = make_base(v, storage, "mma")
-    ss = make_base(v, storage, "mma_smem")
+    ss = make_base(v, storage, "scan")
     a = ts.search_arrays(qr, k, ms)
     c = ss.search_arrays(qr, k, ms)
-    assert ts.last_timing()["path"] == ss.last_timing()["path"] == "mma"
+    assert ts.last_timing()["path"] == "mma" and ss.last_timing()["path"] == "scan"
     np.testing.assert_array_equal(a[2], c[2])
     for i in list(range(0, b, max(1, b // 16))) + [b - 1]:
         got = {"items": a[0][i, : a[2][i]].tolist(), "scores": a[1][i, : a[2][i]].tolist()}
         other = {"items": c[0][i, : c[2][i]].tolist(), "scores": c[1][i, : c[2][i]].tolist()}
-        assert_hits_match(got, other, score_tol=2e-6, min_score=ms, what=f"tmem vs smem q{i}")
-        assert_hits_match(got, O.lookup(vr, qr[i], k, ms), min_score=ms, what=f"tmem vs oracle q{i}")
+        assert_hits_match(got, other, score_tol=2e-6, min_score=ms, what=f"mma vs scan q{i}")
+        assert_hits_match(got, O.lookup(vr, qr[i], k, ms), min_score=ms, what=f"mma vs oracle q{i}")
     allowed = np.random.default_rng(1).random(n) < 0.5
     m = ts.search_arrays(qr[:200], k, ms, allowed=allowed)
     for i in (0, 57, min(b, 200) - 1):

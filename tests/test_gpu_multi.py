@@ -1,9 +1,9 @@
-"""Multi-GPU parity as a driver-run test: when at least two GPUs are visible, launch
+"""Multi-GPU parity: when at least two GPUs are visible, launch
 ``tools/multi_gpu_check.py`` (one rank per GPU, NCCL rendezvous on 127.0.0.1) on two of them.  It checks
 that the row-sharded lookup — local search, libtavec's peer-memory candidate exchange (and the NCCL
 form), merge — is bit-identical to the single-GPU lookup and agrees with the oracle, including the
 float32 split form, the five-query-chunk batch of BASELINE configs[3] and the exact fallback through
-``finish()``.  Skipped on single-GPU boxes (the host logic is covered on CPU by test_sharded_gloo.py)."""
+``finish()``.  Skipped on single-GPU machines (the host logic is covered on CPU by test_sharded_gloo.py)."""
 
 from __future__ import annotations
 

@@ -13,7 +13,6 @@ from __future__ import annotations
 
 import asyncio
 import ctypes as C
-import json
 
 import numpy as np
 import pytest
@@ -26,8 +25,7 @@ from typeagent_py_b200 import _capi
 
 pytestmark = pytest.mark.gpu
 
-with open(GC.GOLDEN_FILE) as _f:
-    GOLDEN = json.load(_f)
+GOLDEN = GC.load_golden()
 
 
 def gpu_base(vectors=None, **kw):

@@ -138,9 +138,9 @@ def _assert_terms_match(got, want, tie=2e-6):
 
 
 def _vocabularies():
-    ep, epq = C.episode53()                      # real data: 406 x 1536 (terms 0..299, message chunks 300..405)
-    yield "episode53", ep[:300], epq, 50, 0.85
-    yield "episode53-lowfloor", ep[:300], epq, 10, 0.0
+    ep, epq = C.episode53()                      # real data: 150 x 1536 (terms 0..99, message chunks 100..149)
+    yield "episode53", ep[:100], epq, 50, 0.85
+    yield "episode53-lowfloor", ep[:100], epq, 10, 0.0
     v, q = O.make_corpus(6000, 384, seed=61, n_queries=64)   # >= 4096 rows, >= 16 queries: tensor cores
     yield "synthetic-6000x384", v, q, 5, 0.0
 
@@ -218,14 +218,14 @@ def test_embedding_file_pair_loads_into_a_search(tmp_path):
     from typeagent_py_b200 import formats
 
     ep, epq = C.episode53()
-    related, messages = ep[:300], ep[300:]
+    related, messages = ep[:100], ep[100:]
     prefix = str(tmp_path / "Episode_53_excerpt_index")
     formats.write_embedding_file(prefix, related, messages)
     raw = np.fromfile(prefix + "_embeddings.bin", dtype=np.float32).reshape(-1, ep.shape[1])   # podcasts/podcast.py:147-168
     np.testing.assert_array_equal(raw, ep)
     settings = tab.TextEmbeddingIndexSettings(O.FakeEmbeddingModel())
     rel_base, msg_base = formats.load_embedding_file(prefix, settings)
-    assert len(rel_base) == 300 and len(msg_base) == 106
+    assert len(rel_base) == 100 and len(msg_base) == 50
     ref_rel = ref_loader.make_reference_vectorbase(related)
     ref_msg = ref_loader.make_reference_vectorbase(messages)
     for q in epq:

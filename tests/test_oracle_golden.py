@@ -8,7 +8,6 @@
 
 from __future__ import annotations
 
-import json
 
 import numpy as np
 import pytest
@@ -18,8 +17,7 @@ from oracle.ref_loader import make_reference_vectorbase, reference_available
 from tests.golden import cases as C
 from tests.parity import assert_hits_match
 
-with open(C.GOLDEN_FILE) as _f:
-    GOLDEN = json.load(_f)
+GOLDEN = C.load_golden()
 
 
 def run_oracle_lookup(vectors, q, kind, kw):

@@ -91,7 +91,7 @@ def main() -> None:
         if len(got) != 10 or [h.item for h in got] != [h.item for h in want]:
             raise SystemExit(f"{label}: GPU and CPU disagree: {got} vs {want}")
         results[label] = {
-            "gpu": report(f"[B200] {label}", run(lambda: call(gpu), args.rounds, args.warmup_rounds)),
+            "gpu": report(f"[GPU] {label}", run(lambda: call(gpu), args.rounds, args.warmup_rounds)),
             "cpu": report(f"[CPU numpy, {os.cpu_count()} cores] {label}",
                           run(lambda: call(cpu), args.rounds, args.warmup_rounds)),
         }

@@ -1,8 +1,8 @@
-"""typeagent-py_b200 — B200-native engine for typeagent's VectorBase top-k lookup.
+"""typeagent-py_b200 — H100-native engine for typeagent's VectorBase top-k lookup.
 
 Drop-in for ONE path of microsoft/typeagent-py: ``typeagent.aitools.vectorbase.VectorBase``
 (and its thin wrapper ``typeagent.knowpro.fuzzyindex.EmbeddingIndex``), executed by
-hand-written sm_100a CUDA kernels behind the C ABI in ``include/tavec.h``.  There is no CPU
+hand-written sm_90a CUDA kernels behind the C ABI in ``include/tavec.h``.  There is no CPU
 fallback: lookups raise ``RuntimeError`` when the CUDA library or a device is missing.
 """
 

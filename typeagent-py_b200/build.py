@@ -1,4 +1,4 @@
-"""Build libtavec.so (the C-ABI CUDA library) in-tree for sm_100a.
+"""Build libtavec.so (the C-ABI CUDA library) in-tree for sm_90a (H100).
 
     python typeagent-py_b200/build.py [--force]
 
@@ -22,7 +22,7 @@ STAMP = os.path.join(HERE, ".libtavec.stamp")
 SOURCES = ["tav_api.cu", "tav_scan.cu", "tav_mma.cu", "tav_group.cu"]
 HEADERS = ["tav_common.cuh", "tav_internal.h", "tav_ptx.cuh", "../../include/tavec.h"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xptxas=-v",
     "-Xcompiler", "-fPIC,-O3,-Wall",

@@ -1,5 +1,5 @@
 // tav_api.cu — the C ABI of libtavec (include/tavec.h): index lifecycle, append / adopt,
-// the search dispatcher (row-scan path or tcgen05 path) and the shard-merge entry point.
+// the search dispatcher (row-scan path or wgmma tensor-core path) and the shard-merge entry point.
 //
 // Reference surface this stands in for (src/typeagent/aitools/vectorbase.py):
 //   add_embedding(s) :115-148 -> tav_append          clear :253-256        -> tav_clear
@@ -559,7 +559,7 @@ static int scan_search(tav_index* ix, TimedSearch* ts, bool timing, const float*
     // CTAs and writes the hits (no select launch) — the device-query twin of the single-launch latency form
     const bool fuse = allow_fuse && n_pass == 1 && pass_k <= 64 &&
                       static_cast<size_t>(n_scan) * ix->dim * dtype_size(ix->dtype) <= kFusedScanMaxBytes &&
-                      static_cast<int64_t>(std::min(grid, 148)) * std::max(pass_k, 32) <= kFusedSelectMax;
+                      static_cast<int64_t>(std::min(grid, 132)) * std::max(pass_k, 32) <= kFusedSelectMax;
     if (fuse) grid = std::min(grid, kFusedSelectMax / std::max(pass_k, 32));
     const int cand_stride = grid * (fuse ? std::max(pass_k, 32) : pass_k);
     TAV_CUDA(ix->cand_keys.ensure(static_cast<size_t>(qb) * cand_stride * sizeof(uint64_t)));
@@ -1089,7 +1089,6 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             m.retry_total_host = static_cast<int32_t*>(ix->retry_host.p) + 2 * slot;
             m.split_overflow_host = use_split ? static_cast<int*>(ix->retry_host.p) + 2 * slot + 1 : nullptr;
             m.row_mask = d_mask;
-            m.no_ts = (flags & TAV_NO_TMEM_QUERIES) ? 1 : 0;
             int ev_used = 0;
             const bool slab_timed = timing && q0 == 0;
             m.ev = slab_timed ? ts->ev : nullptr;
@@ -1189,7 +1188,6 @@ int tav_mma_scores(tav_index* ix, const float* queries, int n_queries, int flags
     m.queries = d_queries;
     m.nq = n_queries;
     m.k = 1;
-    m.no_ts = 1;
     const size_t ws = mma_workspace_bytes(m);
     if (ws > ix->mma_ws.bytes) {
         TAV_CUDA(cudaStreamSynchronize(s));

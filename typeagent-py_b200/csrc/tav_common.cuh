@@ -1,4 +1,4 @@
-// tav_common.cuh — shared device/host helpers of libtavec (sm_100a).
+// tav_common.cuh — shared device/host helpers of libtavec (sm_90a).
 //
 // Candidate keys.  Every (row, score) candidate travels as one 64-bit key
 //     key = (float_bits(score) << 32) | position

@@ -333,7 +333,7 @@ int tav_sharded_search(tav_index* ix, tav_group* g, const float* queries_device,
     packed_offsets(n_queries, k, &off_scores, &off_counts, &bytes);
     char* mine = g->region + g->off_slots + (static_cast<size_t>(slot) * g->world + g->rank) * g->slot_bytes;
     // local search straight into this rank's slot (global ordinals through item_offset)
-    const int sflags = (flags & (TAV_FORCE_SCAN | TAV_FORCE_MMA | TAV_USE_ROW_MASK | TAV_NO_TMEM_QUERIES)) | TAV_QUERIES_ON_DEVICE |
+    const int sflags = (flags & (TAV_FORCE_SCAN | TAV_FORCE_MMA | TAV_USE_ROW_MASK)) | TAV_QUERIES_ON_DEVICE |
                        TAV_OUTPUTS_ON_DEVICE | TAV_DEFER_RETRY;
     if (tav_size(ix) == 0) {
         TAVG_CUDA(cudaMemsetAsync(mine + off_counts, 0, static_cast<size_t>(n_queries) * 4, s));

@@ -120,14 +120,13 @@ struct MmaArgs {
     int32_t* retry_total_host;  // the same counter in mapped pinned memory (read by the host without a copy), or nullptr
     int* split_overflow_host;   // split only: mapped pinned twin of split_overflow, or nullptr
     const uint32_t* row_mask;  // optional device bitmask over corpus rows (bit set = row may be returned)
-    int no_ts;             // 1: never use the Q-stationary (queries in tensor memory) form
     cudaEvent_t (*ev)[2];  // optional event pairs, one recorded around every kernel launched
     int* ev_kind;          //   kind per pair: 0 = dominant (MAIN) kernel, 1 = sample pass, 2 = auxiliary
     int ev_max;
     int* ev_used;
     int ev_main_only;      // 1: record events only around the dominant (MAIN) kernel
 };
-constexpr int kMmaMaxQueries = 32768;  // queries per launch_mma_search call (512 chunks of >= 128 ... callers slab)
+constexpr int kMmaMaxQueries = 32768;  // queries per launch_mma_search call (256 chunks of 128; callers slab)
 size_t mma_workspace_bytes(const MmaArgs& a);
 cudaError_t launch_mma_search(const MmaArgs& a, void* workspace, size_t workspace_bytes,
                               cudaStream_t s, int* launches);

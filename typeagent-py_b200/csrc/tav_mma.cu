@@ -1,46 +1,42 @@
 // tav_mma.cu — the tensor-core path of libtavec: batched query x corpus similarity as a dense
-// bf16/fp16 contraction on tcgen05 (fp32 accumulators in TMEM) fed by TMA tiles from HBM, with
-// the score threshold and top-k candidate selection fused into the TMEM epilogue.
+// bf16/fp16 contraction on Hopper warpgroup MMAs (wgmma, fp32 accumulators in registers) fed by
+// TMA tiles from HBM, with the score threshold and top-k candidate selection fused into the
+// epilogue that reads the accumulators.
 //
 // Reference semantics (aitools/vectorbase.py:163-190, per query): x = dot(row, q) in float32;
 // score = clip((x+1)/2, 0, 1); keep score >= min_score; k best by score.  Products of bf16/fp16
 // values are exact in float32, so on storage-rounded inputs only the summation order differs
 // from the reference's sgemv.
 //
-// Shape of one CTA (persistent, one per SM, 320 threads; see the template comment below for the
-// CTA-pair and split-precision forms):
-//   warp 0     TMA producer: per (corpus tile, query chunk, 64-wide K slice) loads the query
-//              slice [128 x 64] and this CTA's corpus slice ([128 x 64] in a pair, [256 x 64]
-//              alone) into a smem ring (6 x 32 KB / 4 x 48 KB, 128-byte swizzle), completing on
-//              an mbarrier.
-//   warp 1     MMA issuer: one elected thread (of the pair's leader CTA) issues tcgen05.mma
-//              .kind::f16 M=256 (pair) or 128, N=256, K=16 — 4 per stage — into one of two
-//              256-column TMEM accumulator stages; tcgen05.commit frees the smem slot (in both
-//              CTAs) and publishes the accumulator.
-//   warps 2-9  epilogue: tcgen05.ld 32 lanes x 32 columns, double-buffered in registers — a
-//              thread owns ONE query (its TMEM lane) and half of the tile's 256 rows.  Per
-//              32-row chunk: the maximum of each group of 8 dots against the query's admission
-//              threshold; only a group that holds an admitted row runs its 8 predicated
-//              compare-and-append steps, (dot, row) keys going to the thread's PRIVATE segment
-//              of the query's candidate buffer (register counter, no atomics; admit_chunk).
-//              Runs concurrently with the next tile's MMAs (two TMEM stages).
-// For embedding sizes up to 768 and more than 128 queries the MAIN pass runs in the Q-stationary
-// form instead (mma_ts_main_kernel below): the query block lives in tensor memory.
+// Shape of one CTA (persistent, one per SM, 288 threads):
+//   warps 0-7  two consumer warpgroups.  Warpgroup g owns queries [64g, 64g+64) of the unit's
+//              128-query chunk: per 64-wide K slice it issues four wgmma m64nNk16 (N = 256 corpus
+//              rows, or 128 in the split form) on the query slice and the corpus slice in shared
+//              memory, keeping one group in flight while it releases the previous slot.  After the
+//              last K slice of a tile its accumulators are screened in registers: a thread holds two
+//              queries (rows r and r+8 of its warp's 16) and, of every 8 corpus rows, two neighbours.
+//              Per 32 rows of a query: the maximum of its 8 dots against the query's admission
+//              threshold; only a group that holds an admitted row runs its 8 predicated compare-and-
+//              append steps, (dot, row) keys going to the thread's PRIVATE segment of the query's
+//              candidate buffer (register counter, no atomics; admit_group).
+//   warp 8     TMA producer: per (corpus tile, query chunk, 64-wide K slice) loads the query slice
+//              [128 x 64] and the corpus slice [N x 64] into a smem ring (4 x 48 KB, or 3 x 64 KB in
+//              the split form; 128-byte swizzle), completing on an mbarrier.
 //
-// Work items are (corpus tile, query chunk) pairs — a chunk is 128 queries (single CTA) or 256
-// (CTA pair) — so ANY number of queries is served by ONE launch per pass: a unit serves one chunk
-// and every n-th tile, the chunks of a tile are visited by neighbouring units at the same time
-// and share the tile through L2, i.e. HBM is read once per search, not once per 256 queries.
+// Work items are (corpus tile, query chunk of 128) pairs, so ANY number of queries is served by ONE
+// launch per pass: a unit serves one chunk and every n-th tile, the chunks of a tile are visited by
+// neighbouring units at the same time and share the tile through L2, i.e. HBM is read once per
+// search, not once per 128 queries.
 //
 // Admission thresholds.  A first launch of the same kernel in SAMPLE mode scores a strided sample
-// of corpus tiles; its epilogue is branch-free: every thread only keeps the maxima of blocks of
-// the dots it sees (128 rows = a tile half for large corpora; 32 or 8 rows when the target is a
-// larger share of the corpus) and stores them.  The unit that finishes a query chunk's last
-// sample tile then derives, per query, the 8th largest block maximum — at least 8 distinct
-// rows reach it — lowers it to the bottom of its float32 score class, never below the caller's
-// min_score, and publishes it as the admission threshold (expected to admit `target` rows of the
-// corpus, see make_plan).  The MAIN launch then streams the whole corpus once; a finalize kernel
-// maps the admitted dots to scores and selects the top k with the library's total order.
+// of corpus tiles; its epilogue is branch-free: it only keeps the maxima of blocks of the dots of a
+// query (128 rows for large corpora; 32 or 8 rows when the target is a larger share of the corpus)
+// and stores them.  The unit that finishes a query chunk's last sample tile then derives, per query,
+// the 8th largest block maximum — at least 8 distinct rows reach it — lowers it to the bottom of its
+// float32 score class, never below the caller's min_score, and publishes it as the admission
+// threshold (expected to admit `target` rows of the corpus, see make_plan).  The MAIN launch then
+// streams the whole corpus once; a finalize kernel maps the admitted dots to scores and selects the
+// top k with the library's total order.
 // Exactness: every row not admitted scores strictly below every admitted row, so if at least k
 // rows were admitted (or the threshold is the caller's min_score itself) the result is the exact
 // top-k.  For k <= 8 that always holds (the 8 block maxima are themselves admitted); otherwise a
@@ -68,24 +64,21 @@ namespace tav {
 
 namespace {
 
-constexpr int kBM = 128;   // queries per accumulator  (TMEM lanes)
-constexpr int kBN = 256;   // corpus rows per tile     (TMEM columns per accumulator)
+constexpr int kBM = 128;   // queries per chunk (two warpgroups of 64)
 constexpr int kBK = 64;    // 16-bit elements per K slice = one 128-byte swizzle row
-constexpr int kUmmaK = 16;
 constexpr int kABytes = kBM * kBK * 2;              // 16 KB
-constexpr int kBBytes = kBN * kBK * 2;              // 32 KB
-constexpr int kStageBytes = kABytes + kBBytes;      // 48 KB
-constexpr int kEpiWarps = 8;                        // 4 TMEM lane quadrants x 2 column halves
-constexpr int kMmaThreads = 64 + 32 * kEpiWarps;    // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
-constexpr int kEpiCols = kBN / 2;                   // columns per epilogue warp
+constexpr int kConsumerWarps = 8;                   // two warpgroups
+constexpr int kMmaThreads = 32 * kConsumerWarps + 32;  // + the TMA producer warp
 constexpr int kSampleTop = 8;                       // the threshold is the 8th largest block maximum
-constexpr int kTmemCols = 512;
-constexpr int kMaxChunks = 512;                      // query chunks per launch (tav_search slabs larger batches)
+constexpr int kMaxChunks = 512;                     // query chunks per launch (tav_search slabs larger batches)
 constexpr int kFinalizeFast = 8192;                 // finalize sorts up to this many candidates in one go
-constexpr int kMaxSegments = 320;                   // candidate segments per query (2 per unit of its chunk)
-// both forms: 192 KB of tiles + barriers + a small scratch used by the sampler's tail
-constexpr size_t kScratchBytes = 2 * 128 * kSampleTop * sizeof(float);  // the sampler tail's exchange of partial top-8 lists
-constexpr size_t kSmemBytes = 1024 + static_cast<size_t>(4) * kStageBytes + 256 + kScratchBytes;
+constexpr int kSegPerUnit = 4;                      // candidate segments per query per unit (the 4 threads of a quad)
+constexpr int kMaxSegments = kSegPerUnit * 160;     // candidate segments per query
+constexpr int kTileRows = 256;                      // corpus rows per tile (128 in the split form)
+constexpr int kTileRowsSplit = 128;
+constexpr size_t kTileSmem = 192 * 1024;            // the stage ring: 4 x (16 + 32) KB, or 3 x 2 x (16 + 16) KB
+constexpr size_t kScratchBytes = 2 * kBM * kSampleTop * sizeof(float);  // the sampler tail's exchange of partial top-8 lists
+constexpr size_t kSmemBytes = 1024 + kTileSmem + 256 + kScratchBytes;
 
 enum Mode { kSample = 0, kMain = 1, kDump = 2 };
 
@@ -96,16 +89,16 @@ struct KernelArgs {
     int64_t tile_div;
     int kb_count;          // ceil(dim / 64)
     int nq;                // valid queries (all chunks)
-    int nqc;               // query chunks of 128 * CG queries
-    int nq_pad;            // nqc * 128 * CG
-    int n_seg;             // MAIN: candidate segments per query = 2 * (units per chunk)
+    int nqc;               // query chunks of 128 queries
+    int nq_pad;            // nqc * 128
+    int n_seg;             // MAIN: candidate segments per query = 4 * (units per chunk)
     float* thr;            // [nq_pad] admission threshold (raw dot) per query: SAMPLE writes, MAIN reads
     float* floor_x;        // SAMPLE: [nq_pad] the caller's min_score as a dot floor
-    float* sample_max;     // SAMPLE: [n_tiles_work * 2 * sample_gph, nq_pad] block maxima
-    int sample_gph;        // SAMPLE: blocks per thread per tile: 1 (128 rows each), 4 (32 rows) or 16 (8 rows)
+    float* sample_max;     // SAMPLE: [n_tiles_work * blocks per tile, nq_pad] block maxima
+    int sample_gph;        // SAMPLE: blocks per 128 rows: 1 (128 rows each), 4 (32 rows) or 16 (8 rows)
     int sample_use;        // SAMPLE: blocks the threshold is derived from ...
     int sample_stride;     //         ... every sample_stride-th of the stored ones
-    uint32_t* sample_done; // SAMPLE: [nqc * CG] finished-unit counters (self-resetting)
+    uint32_t* sample_done; // SAMPLE: [nqc] finished-unit counters (self-resetting)
     int32_t* retry;        // SAMPLE: [nq] per-query "redo exactly" flags, cleared here
     float floor_score;     // SAMPLE: (float)min_score
     uint64_t* cand;        // MAIN: [nq_pad, n_seg, cap_seg]  (dot bits << 32 | row)
@@ -125,29 +118,32 @@ __device__ __forceinline__ void insert_top(float (&top)[kSampleTop], float x) {
     }
 }
 
+// accumulator d[4j + 2h + e] of a thread: query row h (0: r, 1: r + 8), corpus column 8j + 2 (lane % 4) + e
+__device__ __forceinline__ int acc_index(int j, int h, int e) { return 4 * j + 2 * h + e; }
 
-// MAIN epilogue of one 32-row chunk: this thread's 32 dots of ITS query against its admission threshold.
-// Two-level screen, all in registers: the maximum of each group of 8 dots (FMNMX3 trees) is tested first;
-// only a group that holds an admitted row runs the 8 predicated compare-and-store steps, appending
-// (dot, row) keys to the thread's PRIVATE candidate segment (one writer, a register counter).
-// Why this shape (profiles/README.md, "epilogue"): a shared per-query counter cost ~1 us of L2 round trip
-// per atomicAdd; a branch-free 32-bit mask + 32 predicated stores cost ~300 instructions whenever ANY of
-// the warp's 32 queries admitted a row (93 % of the chunks at 50k rows); a warp-cooperative walk over the
-// hit lanes was latency-bound on its shuffle / ballot / shared-memory chains (~2000 cycles per chunk).
+// MAIN epilogue of one group of 32 corpus rows for ONE query of this thread (h): its 8 dots of those rows
+// (columns 32g + 8jj + 2 (lane % 4) + e) against the query's admission threshold.  The maximum of the 8 is
+// tested first; only a group that holds an admitted row runs the 8 predicated compare-and-store steps,
+// appending (dot, row) keys to the thread's PRIVATE candidate segment (one writer, a register counter).
 // `amask`: bit i set = row rbase + i exists and passes the row mask (warp-uniform).
-__device__ __forceinline__ void admit_chunk(const uint32_t (&v)[32], float tau, uint32_t rbase, uint32_t amask,
-                                            uint64_t* my_cand, uint32_t& n_admitted, uint32_t cap_seg) {
+template <int NACC>
+__device__ __forceinline__ void admit_group(const float (&d)[NACC], int g, int h, int t4, float tau, uint32_t rbase,
+                                            uint32_t amask, uint64_t* my_cand, uint32_t& n_admitted,
+                                            uint32_t cap_seg) {
+    float m = -INFINITY;
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-        float m = fmaxf(__uint_as_float(v[8 * g]), __uint_as_float(v[8 * g + 1]));
+    for (int jj = 0; jj < 4; ++jj)
+        m = fmaxf(m, fmaxf(d[acc_index(4 * g + jj, h, 0)], d[acc_index(4 * g + jj, h, 1)]));
+    if (m >= tau) {
 #pragma unroll
-        for (int j = 2; j < 8; ++j) m = fmaxf(m, __uint_as_float(v[8 * g + j]));
-        if (m >= tau) {
+        for (int jj = 0; jj < 4; ++jj) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int i = 8 * g + j;
-                if (__uint_as_float(v[i]) >= tau && ((amask >> i) & 1u)) {
-                    if (n_admitted < cap_seg) my_cand[n_admitted] = (static_cast<uint64_t>(v[i]) << 32) | (rbase + i);
+            for (int e = 0; e < 2; ++e) {
+                const float x = d[acc_index(4 * g + jj, h, e)];
+                const int i = 8 * jj + 2 * t4 + e;
+                if (x >= tau && ((amask >> i) & 1u)) {
+                    if (n_admitted < cap_seg)
+                        my_cand[n_admitted] = (static_cast<uint64_t>(__float_as_uint(x)) << 32) | (rbase + i);
                     ++n_admitted;
                 }
             }
@@ -155,10 +151,38 @@ __device__ __forceinline__ void admit_chunk(const uint32_t (&v)[32], float tau, 
     }
 }
 
-// Work distribution: unit u (a CTA, or a CTA pair) serves ONE query chunk, c = u % nqc, and every
-// (n_units / nqc)-th tile of the launch, starting at u / nqc — so the nqc units that share a tile run
-// side by side (the tile is fetched from HBM once and served to the others by L2) and an epilogue
-// thread keeps the same query for the whole launch (its candidate counter lives in a register).
+// maximum over the 4 threads of a quad (which together hold every column of a query's 8-row group)
+__device__ __forceinline__ float quad_max(float x) {
+    x = fmaxf(x, __shfl_xor_sync(0xFFFFFFFFu, x, 1));
+    return fmaxf(x, __shfl_xor_sync(0xFFFFFFFFu, x, 2));
+}
+
+// SAMPLE epilogue of one tile for one query of this thread (h): maxima of blocks of JPB * 8 rows, the
+// masked-out rows ignored, stored to dst[block * nq_pad] by one thread of the quad.
+template <int JPB, int NACC>
+__device__ __forceinline__ void sample_blocks(const float (&d)[NACC], int h, int t4, const uint32_t* row_mask,
+                                              int64_t row0, float* dst, int nq_pad) {
+    constexpr int kJ = NACC / 4;  // 8-row groups in the tile
+#pragma unroll
+    for (int b = 0; b < kJ / JPB; ++b) {
+        float m = -INFINITY;
+#pragma unroll
+        for (int jj = 0; jj < JPB; ++jj) {
+            const int j = b * JPB + jj;
+            const uint32_t bits = row_mask ? row_mask[(row0 >> 5) + (j >> 2)] : 0xFFFFFFFFu;
+            const int i = 8 * (j & 3) + 2 * t4;
+            m = fmaxf(m, ((bits >> i) & 1u) ? d[acc_index(j, h, 0)] : -INFINITY);
+            m = fmaxf(m, ((bits >> (i + 1)) & 1u) ? d[acc_index(j, h, 1)] : -INFINITY);
+        }
+        m = quad_max(m);
+        if (t4 == (b & 3)) dst[static_cast<size_t>(b) * nq_pad] = m;
+    }
+}
+
+// Work distribution: unit u (a CTA) serves ONE query chunk, c = u % nqc, and every (n_units / nqc)-th
+// tile of the launch, starting at u / nqc — so the nqc units that share a tile run side by side (the tile
+// is fetched from HBM once and served to the others by L2) and an epilogue thread keeps the same queries
+// for the whole launch (its candidate counters live in registers).
 // Item i of unit `unit` -> (visited tile t, query chunk c); false when the unit has no such item.
 __device__ __forceinline__ bool get_item(const KernelArgs& a, int unit, int n_units, int i, int& t, int& c) {
     const int upc = n_units / a.nqc;  // units per chunk (the launcher makes n_units a multiple of nqc)
@@ -190,56 +214,55 @@ __device__ float dot_floor_for_score(float s) {
     return ord_to_float(lo);
 }
 
-// CG = 1: one CTA per item, 128 queries per chunk.
-// CG = 2: a CTA pair (cluster of 2, tcgen05 cta_group::2) per item, 256 queries per chunk: CTA r
-//         owns query block r (its 128 TMEM lanes) and stages rows [128r, 128r+128) of the corpus
-//         tile; every MMA is M=256 x N=256 across the pair, so each CTA's shared memory sees half
-//         of the operand traffic of the single-CTA form — the single-CTA form is smem-bandwidth
-//         bound at ~55 % of the tensor pipe (profiles/README.md).
-// SPLIT: float32 data carried as two fp16 planes, x = hi + lo / 2048 (22 significant bits;
-//         products of fp16 values are exact in the fp32 accumulator).  Three MMAs per K step:
-//         hi.hi' into the MAIN accumulator, hi.lo' + lo.hi' into the CROSS accumulator; the
-//         epilogue combines main + cross / 2048 (the lo.lo' term, <= 2^-22 relative, is dropped).
-//         Both accumulators of a tile fill TMEM (2 x 256 columns), so tiles are not
-//         double-buffered in this form.
-template <int MODE, int CG, bool SPLIT>
+template <int N, bool BF16>
+__device__ __forceinline__ void wgmma_step(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+    if constexpr (N == 256) {
+        if constexpr (BF16) ptx::wgmma_m64n256_bf16(d, da, db, scale_d);
+        else ptx::wgmma_m64n256_f16(d, da, db, scale_d);
+    } else {
+        static_assert(N == 128 && !BF16, "the split form is fp16, N = 128");
+        ptx::wgmma_m64n128_f16(d, da, db, scale_d);
+    }
+}
+
+// BF16: operand format (bf16 or fp16).
+// SPLIT: float32 data carried as two fp16 planes, x = hi + lo / 2048 (22 significant bits; products of
+//        fp16 values are exact in the fp32 accumulator).  Three MMAs per K step: hi.hi' into the MAIN
+//        accumulator, hi.lo' + lo.hi' into the CROSS accumulator; the epilogue combines main + cross /
+//        2048 (the lo.lo' term, <= 2^-22 relative, is dropped).  Two accumulators of 64 x 128 take the
+//        registers one of 64 x 256 does, so tiles are 128 corpus rows in this form.
+template <int MODE, bool BF16, bool SPLIT>
 __global__ void __launch_bounds__(kMmaThreads, 1)
 mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c,
                 const __grid_constant__ CUtensorMap map_q_lo, const __grid_constant__ CUtensorMap map_c_lo,
-                const KernelArgs a, const uint32_t idesc) {
-    constexpr int kRowsB = kBN / CG;                         // corpus rows staged per CTA per tile
-    constexpr int kBBytesCta = kRowsB * kBK * 2;
+                const KernelArgs a) {
+    constexpr int kTileN = SPLIT ? kTileRowsSplit : kTileRows;  // corpus rows per tile
+    constexpr int kNacc = kTileN / 2;                          // accumulator registers per thread
+    constexpr int kBBytes = kTileN * kBK * 2;
     constexpr int kPlanes = SPLIT ? 2 : 1;
-    constexpr int kStageBytesCta = kPlanes * (kABytes + kBBytesCta);  // [A | B | A_lo | B_lo]
-    constexpr int kNumStages = (CG == 2 ? 6 : 4) / kPlanes;  // 192 KB of tiles in every form
-    constexpr int kAccStages = SPLIT ? 1 : 2;                // TMEM accumulator stages
-    constexpr int kChunk = kBM * CG;                         // queries per chunk
+    constexpr int kStageBytes = kPlanes * (kABytes + kBBytes);  // [A | B | A_lo | B_lo]
+    constexpr int kNumStages = static_cast<int>(kTileSmem / kStageBytes);
+    static_assert(kNumStages * kStageBytes == static_cast<int>(kTileSmem), "stage ring");
     extern __shared__ uint8_t smem_dyn[];
     // SWIZZLE_128B tiles need 1024-byte alignment
     uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + static_cast<size_t>(kNumStages) * kStageBytesCta);
-    uint64_t* full = bars;                    // [stages] TMA -> MMA      (the leader's copy is used)
-    uint64_t* empty = bars + kNumStages;      // [stages] MMA -> TMA      (each CTA its own)
-    uint64_t* tfull = bars + 2 * kNumStages;  // [2] MMA -> epilogue      (each CTA its own)
-    uint64_t* tempty = tfull + 2;             // [2] epilogue -> MMA      (the leader's copy is used)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + kTileSmem);
+    uint64_t* full = bars;                    // [stages] TMA -> MMA
+    uint64_t* empty = bars + kNumStages;      // [stages] MMA -> TMA (one arrive per consumer warp)
     float* scratch = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);  // sampler tail
     __shared__ int s_last;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t cta_rank = CG == 2 ? ptx::cluster_ctarank() : 0;
-    const int unit = blockIdx.x / CG, n_units = gridDim.x / CG;  // a unit = CTA or CTA pair
+    const int unit = blockIdx.x, n_units = gridDim.x;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < kNumStages; ++s) {
-            ptx::mbar_init(&full[s], 1);      // the leader's producer arrives once with the unit's bytes
-            ptx::mbar_init(&empty[s], 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            ptx::mbar_init(&tfull[s], 1);
-            ptx::mbar_init(&tempty[s], kEpiWarps * CG);  // one arrive per epilogue warp of the unit
+            ptx::mbar_init(&full[s], 1);  // the producer arrives once with the stage's bytes
+            ptx::mbar_init(&empty[s], kConsumerWarps);
         }
         ptx::fence_mbar_init();
+    }
+    if (warp == kConsumerWarps && lane == 0) {
         ptx::prefetch_tensormap(&map_q);
         ptx::prefetch_tensormap(&map_c);
         if (SPLIT) {
@@ -247,238 +270,154 @@ mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
             ptx::prefetch_tensormap(&map_c_lo);
         }
     }
-    if (warp == 1) {
-        if (CG == 2) ptx::tmem_alloc_pair(tmem_slot, kTmemCols);
-        else ptx::tmem_alloc(tmem_slot, kTmemCols);
-    }
-    ptx::tc_fence_before();
-    if (CG == 2) ptx::cluster_sync_all();
-    else __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
 
-    if (warp == 0) {
-        // ================= TMA producer (every CTA) =================
-        if (ptx::elect_one()) {
+    if (warp == kConsumerWarps) {
+        // ================= TMA producer =================
+        if (lane == 0) {
             uint32_t stage = 0, phase = 0;
             int t, c;
             for (int i = 0; get_item(a, unit, n_units, i, t, c); ++i) {
                 const int64_t tile = (static_cast<int64_t>(t) * a.tile_mul) / a.tile_div;
-                const int32_t row0 = static_cast<int32_t>(tile * kBN + cta_rank * kRowsB);
-                const int32_t qrow = c * kChunk + static_cast<int32_t>(cta_rank) * kBM;
+                const int32_t row0 = static_cast<int32_t>(tile * kTileN);
+                const int32_t qrow = c * kBM;
                 for (int kb = 0; kb < a.kb_count; ++kb) {
                     ptx::mbar_wait(&empty[stage], phase ^ 1);
-                    uint8_t* sa = tiles + static_cast<size_t>(stage) * kStageBytesCta;
-                    if (CG == 2) {
-                        // Both CTAs' loads complete on the LEADER's barrier; only the leader arms it,
-                        // with the bytes of both (a peer load landing first just drives the pending
-                        // byte count negative until the leader's expect_tx; the peer cannot run a phase
-                        // ahead because its slot is released by the same multicast commit).
-                        const uint32_t lead_full = ptx::map_to_cta(ptx::smem_u32(&full[stage]), 0);
-                        if (cta_rank == 0) ptx::mbar_expect_tx(&full[stage], 2 * kStageBytesCta);
-                        ptx::tma_load_2d_pair(sa, &map_q, lead_full, kb * kBK, qrow, ptx::kEvictLast);
-                        ptx::tma_load_2d_pair(sa + kABytes, &map_c, lead_full, kb * kBK, row0, ptx::kEvictFirst);
-                        if (SPLIT) {
-                            uint8_t* sl = sa + kABytes + kBBytesCta;
-                            ptx::tma_load_2d_pair(sl, &map_q_lo, lead_full, kb * kBK, qrow, ptx::kEvictLast);
-                            ptx::tma_load_2d_pair(sl + kABytes, &map_c_lo, lead_full, kb * kBK, row0, ptx::kEvictFirst);
-                        }
-                    } else {
-                        ptx::mbar_expect_tx(&full[stage], kStageBytesCta);
-                        ptx::tma_load_2d(sa, &map_q, &full[stage], kb * kBK, qrow, ptx::kEvictLast);
-                        ptx::tma_load_2d(sa + kABytes, &map_c, &full[stage], kb * kBK, row0, ptx::kEvictFirst);
-                        if (SPLIT) {
-                            uint8_t* sl = sa + kABytes + kBBytesCta;
-                            ptx::tma_load_2d(sl, &map_q_lo, &full[stage], kb * kBK, qrow, ptx::kEvictLast);
-                            ptx::tma_load_2d(sl + kABytes, &map_c_lo, &full[stage], kb * kBK, row0, ptx::kEvictFirst);
-                        }
+                    uint8_t* sa = tiles + static_cast<size_t>(stage) * kStageBytes;
+                    ptx::mbar_expect_tx(&full[stage], kStageBytes);
+                    ptx::tma_load_2d(sa, &map_q, &full[stage], kb * kBK, qrow, ptx::kEvictLast);
+                    ptx::tma_load_2d(sa + kABytes, &map_c, &full[stage], kb * kBK, row0, ptx::kEvictFirst);
+                    if (SPLIT) {
+                        uint8_t* sl = sa + kABytes + kBBytes;
+                        ptx::tma_load_2d(sl, &map_q_lo, &full[stage], kb * kBK, qrow, ptx::kEvictLast);
+                        ptx::tma_load_2d(sl + kABytes, &map_c_lo, &full[stage], kb * kBK, row0, ptx::kEvictFirst);
                     }
                     if (++stage == kNumStages) {
                         stage = 0;
                         phase ^= 1;
                     }
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ================= MMA issuer (leader CTA of the unit) =================
-        if (cta_rank == 0 && ptx::elect_one()) {
-            uint32_t stage = 0, phase = 0;
-            int t, c;
-            for (int i = 0; get_item(a, unit, n_units, i, t, c); ++i) {
-                const uint32_t item = static_cast<uint32_t>(i);
-                const uint32_t as = item % kAccStages, aphase = (item / kAccStages) & 1;
-                ptx::mbar_wait(&tempty[as], aphase ^ 1);  // epilogue(s) drained this accumulator
-                ptx::tc_fence_after();
-                const uint32_t d_tmem = tmem_base + as * kBN;
-                const uint32_t d_cross = tmem_base + kBN;  // SPLIT only
-                for (int kb = 0; kb < a.kb_count; ++kb) {
-                    ptx::mbar_wait(&full[stage], phase);
-                    ptx::tc_fence_after();
-                    const uint32_t sa = ptx::smem_u32(tiles + static_cast<size_t>(stage) * kStageBytesCta);
-                    const uint64_t da = ptx::make_kmajor_sw128_desc(sa);
-                    const uint64_t db = ptx::make_kmajor_sw128_desc(sa + kABytes);
-#pragma unroll
-                    for (int k = 0; k < kBK / kUmmaK; ++k) {
-                        // advance 16 elements = 32 bytes along K inside the swizzle atom
-                        const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-                        const uint32_t acc = (kb | k) != 0 ? 1u : 0u;
-                        if (CG == 2) ptx::umma_f16_pair(d_tmem, da + koff, db + koff, idesc, acc);
-                        else ptx::umma_f16(d_tmem, da + koff, db + koff, idesc, acc);
-                        if (SPLIT) {
-                            const uint64_t da_lo = ptx::make_kmajor_sw128_desc(sa + kABytes + kBBytesCta) + koff;
-                            const uint64_t db_lo = ptx::make_kmajor_sw128_desc(sa + 2 * kABytes + kBBytesCta) + koff;
-                            if (CG == 2) {
-                                ptx::umma_f16_pair(d_cross, da + koff, db_lo, idesc, acc);  // hi . lo'
-                                ptx::umma_f16_pair(d_cross, da_lo, db + koff, idesc, 1u);   // lo . hi'
-                            } else {
-                                ptx::umma_f16(d_cross, da + koff, db_lo, idesc, acc);
-                                ptx::umma_f16(d_cross, da_lo, db + koff, idesc, 1u);
-                            }
-                        }
-                    }
-                    // smem slot reusable (in both CTAs) once these MMAs retire
-                    if (CG == 2) ptx::umma_commit_pair(&empty[stage], 3);
-                    else ptx::umma_commit(&empty[stage]);
-                    if (++stage == kNumStages) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-                if (CG == 2) ptx::umma_commit_pair(&tfull[as], 3);  // accumulator complete (both CTAs)
-                else ptx::umma_commit(&tfull[as]);
             }
         }
     } else {
-        // ================= epilogue: one thread = one query (TMEM lane) x half the columns =====
-        const int quad = warp & 3;            // TMEM lane quadrant this warp may read
-        const int half = (warp - 2) >> 2;     // which 128 of the tile's 256 columns
-        const int lane_q = static_cast<int>(cta_rank) * kBM + quad * 32 + lane;  // query inside the chunk
-        const uint32_t lead_tempty0 = CG == 2 ? ptx::map_to_cta(ptx::smem_u32(&tempty[0]), 0) : 0;
-        // MAIN: this thread's private candidate segment (no atomics: one writer per segment)
-        const int seg = (unit / a.nqc) * 2 + half;
-        const int my_q = (unit % a.nqc) * kChunk + lane_q;
-        uint64_t* const my_cand = a.cand + (static_cast<size_t>(my_q) * a.n_seg + seg) * a.cap_seg;
-        uint32_t n_admitted = 0;
+        // ================= consumer warpgroups: MMAs, then the epilogue on the accumulators =====
+        const int wg = warp >> 2;                    // which 64 queries of the chunk
+        const int t4 = lane & 3;                     // column pair inside every 8-row group
+        const int c_unit = unit % a.nqc;
+        const int q_local = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // + 8 for the second query (h = 1)
+        const int my_q[2] = {c_unit * kBM + q_local, c_unit * kBM + q_local + 8};
+        // MAIN: this thread's private candidate segments (no atomics: one writer per segment)
+        const int seg = (unit / a.nqc) * kSegPerUnit + t4;
+        uint64_t* my_cand[2];
+        uint32_t n_admitted[2] = {0u, 0u};
+        float tau[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            my_cand[h] = a.cand + (static_cast<size_t>(my_q[h]) * a.n_seg + seg) * a.cap_seg;
+            tau[h] = (MODE == kMain && my_q[h] < a.nq) ? a.thr[my_q[h]] : INFINITY;
+        }
+        // A: this warpgroup's 64 query rows (8 swizzle groups of 1024 B in); B: the corpus slice
+        const uint32_t a_off = static_cast<uint32_t>(wg) * 64 * 128;
+        float acc[kNacc];
+        float accx[SPLIT ? kNacc : 1];
+#pragma unroll
+        for (int i = 0; i < kNacc; ++i) acc[i] = 0.0f;
+#pragma unroll
+        for (int i = 0; i < (SPLIT ? kNacc : 1); ++i) accx[i] = 0.0f;
+        uint32_t stage = 0, phase = 0;
         int t, c;
         for (int i = 0; get_item(a, unit, n_units, i, t, c); ++i) {
-            const uint32_t item = static_cast<uint32_t>(i);
             const int64_t tile = (static_cast<int64_t>(t) * a.tile_mul) / a.tile_div;
-            const int64_t row0 = tile * kBN + half * kEpiCols;
-            // columns of this warp's half that are real corpus rows (warp-uniform)
+            const int64_t row0 = tile * kTileN;
+            uint32_t prev = 0;
+            for (int kb = 0; kb < a.kb_count; ++kb) {
+                ptx::mbar_wait(&full[stage], phase);
+                const uint32_t sa = ptx::smem_u32(tiles + static_cast<size_t>(stage) * kStageBytes);
+                const uint64_t da = ptx::make_kmajor_sw128_desc(sa + a_off);
+                const uint64_t db = ptx::make_kmajor_sw128_desc(sa + kABytes);
+                ptx::wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kBK / 16; ++k) {
+                    const uint32_t accumulate = (kb | k) != 0 ? 1u : 0u;
+                    wgmma_step<kTileN, BF16>(acc, da + 2 * k, db + 2 * k, accumulate);
+                    if constexpr (SPLIT) {
+                        const uint64_t da_lo = ptx::make_kmajor_sw128_desc(sa + kABytes + kBBytes + a_off) + 2 * k;
+                        const uint64_t db_lo = ptx::make_kmajor_sw128_desc(sa + 2 * kABytes + kBBytes) + 2 * k;
+                        wgmma_step<kTileN, false>(accx, da + 2 * k, db_lo, accumulate);  // hi . lo'
+                        wgmma_step<kTileN, false>(accx, da_lo, db + 2 * k, 1u);          // lo . hi'
+                    }
+                }
+                ptx::wgmma_commit();
+                // the previous slice's MMAs have retired: its slot may be refilled
+                if (kb > 0) {
+                    ptx::wgmma_wait<1>();
+                    if (lane == 0) ptx::mbar_arrive(&empty[prev]);
+                }
+                prev = stage;
+                if (++stage == static_cast<uint32_t>(kNumStages)) {
+                    stage = 0;
+                    phase ^= 1;
+                }
+            }
+            ptx::wgmma_wait<0>();
+            if (lane == 0) ptx::mbar_arrive(&empty[prev]);
+            if constexpr (SPLIT) {
+                // x = main + cross / 2048
+#pragma unroll
+                for (int r = 0; r < kNacc; ++r) acc[r] = fmaf(accx[r], 1.0f / 2048.0f, acc[r]);
+            }
+
+            // columns of the tile that are real corpus rows (uniform)
             const int ncols = static_cast<int>(max(static_cast<int64_t>(0),
-                                                   min(static_cast<int64_t>(kEpiCols), a.n_rows - row0)));
-            const uint32_t as = item % kAccStages, aphase = (item / kAccStages) & 1;
-            const int q = c * kChunk + lane_q;  // global query index
-            float tau = INFINITY;
-            if (MODE == kMain && q < a.nq) tau = a.thr[q];
-            float bmax = -INFINITY;             // SAMPLE: best dot of this thread's 128 rows of the tile
-            ptx::mbar_wait(&tfull[as], aphase);
-            ptx::tc_fence_after();
-            const uint32_t taddr =
-                tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + as * kBN + half * kEpiCols;
-
-            auto process = [&](const uint32_t (&v)[32], int c0) {
-                const int nvalid = min(32, ncols - c0);  // >= 1 here
-                const uint32_t rbase = static_cast<uint32_t>(row0 + c0);  // a multiple of 32
-                if (MODE == kDump) {
-                    if (q < a.nq) {
+                                                   min(static_cast<int64_t>(kTileN), a.n_rows - row0)));
+            if (MODE == kDump) {
 #pragma unroll
-                        for (int i2 = 0; i2 < 32; ++i2)
-                            if (i2 < nvalid)
-                                a.dump[static_cast<size_t>(q) * a.n_rows + row0 + c0 + i2] = __uint_as_float(v[i2]);
-                    }
-                    return;
-                }
-                if (MODE == kSample) {
-                    // branch-free: sample tiles are full tiles, every column is a real row.  Maxima of the
-                    // four groups of 8 rows, then — by the block size the planner chose — stored per group
-                    // (blocks of 8 rows), per chunk (32) or folded into the tile maximum (128).
-                    const uint32_t bits = a.row_mask ? a.row_mask[rbase >> 5] : 0xFFFFFFFFu;
-                    float g4[4];
+                for (int h = 0; h < 2; ++h) {
+                    if (my_q[h] >= a.nq) continue;
+                    float* out = a.dump + static_cast<size_t>(my_q[h]) * a.n_rows + row0;
 #pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        float m = -INFINITY;
+                    for (int j = 0; j < kNacc / 4; ++j)
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const int i2 = 8 * g + j;
-                            m = fmaxf(m, ((bits >> i2) & 1u) ? __uint_as_float(v[i2]) : -INFINITY);
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 8 * j + 2 * t4 + e;
+                            if (col < ncols) out[col] = acc[acc_index(j, h, e)];
                         }
-                        g4[g] = m;
-                    }
-                    const float cm = fmaxf(fmaxf(g4[0], g4[1]), fmaxf(g4[2], g4[3]));
-                    float* dst = a.sample_max + (static_cast<size_t>(t) * 2 + half) * a.sample_gph * a.nq_pad + q;
-                    if (a.sample_gph == 16) {
-#pragma unroll
-                        for (int g = 0; g < 4; ++g) dst[static_cast<size_t>((c0 >> 3) + g) * a.nq_pad] = g4[g];
-                    } else if (a.sample_gph == 4) {
-                        dst[static_cast<size_t>(c0 >> 5) * a.nq_pad] = cm;
-                    } else {
-                        bmax = fmaxf(bmax, cm);
-                    }
-                    return;
                 }
-                // MAIN: group-wise screen and private-segment append (admit_chunk)
-                uint32_t amask = nvalid >= 32 ? 0xFFFFFFFFu : ((1u << nvalid) - 1u);
-                if (a.row_mask) amask &= a.row_mask[rbase >> 5];
-                admit_chunk(v, tau, rbase, amask, my_cand, n_admitted, a.cap_seg);
-            };
-
-            uint32_t va[32], vb[32];
-            if (SPLIT) {
-                // main and cross accumulators of the same 32 columns, combined: x = main + cross / 2048
-#pragma unroll 1
-                for (int c0 = 0; c0 < ncols; c0 += 32) {
-                    ptx::tmem_ld_32x32(taddr + c0, va);
-                    ptx::tmem_ld_32x32(taddr + kBN + c0, vb);
-                    ptx::tmem_ld_wait();
+            } else if (MODE == kSample) {
+                // branch-free: sample tiles are full tiles, every column is a real row
+                const int bpt = (kTileN / 128) * a.sample_gph;  // blocks per tile
 #pragma unroll
-                    for (int i2 = 0; i2 < 32; ++i2)
-                        va[i2] = __float_as_uint(fmaf(__uint_as_float(vb[i2]), 1.0f / 2048.0f, __uint_as_float(va[i2])));
-                    process(va, c0);
+                for (int h = 0; h < 2; ++h) {
+                    float* dst = a.sample_max + static_cast<size_t>(t) * bpt * a.nq_pad + my_q[h];
+                    if (a.sample_gph == 16) sample_blocks<1>(acc, h, t4, a.row_mask, row0, dst, a.nq_pad);
+                    else if (a.sample_gph == 4) sample_blocks<4>(acc, h, t4, a.row_mask, row0, dst, a.nq_pad);
+                    else sample_blocks<16>(acc, h, t4, a.row_mask, row0, dst, a.nq_pad);
                 }
             } else {
-                // two register buffers: the load of chunk c+1 is in flight while chunk c is screened
-                if (ncols > 0) {
-                    ptx::tmem_ld_32x32(taddr, va);
-                    ptx::tmem_ld_wait();
-                }
-#pragma unroll 1
-                for (int c0 = 0; c0 < kEpiCols; c0 += 64) {
-                    if (c0 + 32 < ncols) ptx::tmem_ld_32x32(taddr + c0 + 32, vb);
-                    if (c0 < ncols) process(va, c0);
-                    ptx::tmem_ld_wait();
-                    if (c0 + 64 < ncols) ptx::tmem_ld_32x32(taddr + c0 + 64, va);
-                    if (c0 + 32 < ncols) process(vb, c0 + 32);
-                    ptx::tmem_ld_wait();
+                // MAIN: group-wise screen and private-segment append (admit_group)
+#pragma unroll
+                for (int g = 0; g < kTileN / 32; ++g) {
+                    const int nvalid = min(32, ncols - 32 * g);
+                    if (nvalid <= 0) break;
+                    const uint32_t rbase = static_cast<uint32_t>(row0 + 32 * g);
+                    uint32_t amask = nvalid >= 32 ? 0xFFFFFFFFu : ((1u << nvalid) - 1u);
+                    if (a.row_mask) amask &= a.row_mask[rbase >> 5];
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        admit_group(acc, g, h, t4, tau[h], rbase, amask, my_cand[h], n_admitted[h], a.cap_seg);
                 }
             }
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (CG == 2) ptx::mbar_arrive_cluster(lead_tempty0 + as * 8);
-                else ptx::mbar_arrive(&tempty[as]);
-            }
-            if (MODE == kSample && a.sample_gph == 1)
-                a.sample_max[(static_cast<size_t>(t) * 2 + half) * a.nq_pad + q] = bmax;
         }
         if (MODE == kSample) __threadfence();  // block maxima visible device-wide before the unit signs off
-        if (MODE == kMain && unit / a.nqc < n_units / a.nqc)
-            a.cand_count[static_cast<size_t>(my_q) * a.n_seg + seg] = n_admitted;
-    }
-
-    // teardown: nobody may leave while the peer still reads its smem / signals its barriers
-    ptx::tc_fence_before();
-    if (CG == 2) ptx::cluster_sync_all();
-    else __syncthreads();
-    if (warp == 1) {
-        __syncwarp();
-        if (CG == 2) ptx::tmem_dealloc_pair(tmem_base, kTmemCols);
-        else ptx::tmem_dealloc(tmem_base, kTmemCols);
+        if (MODE == kMain && unit / a.nqc < n_units / a.nqc) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) a.cand_count[static_cast<size_t>(my_q[h]) * a.n_seg + seg] = n_admitted[h];
+        }
     }
 
     if (MODE == kSample) {
         // ---- sampler tail: the last unit of a query chunk turns block maxima into thresholds ----
+        __syncthreads();
         const int upc = n_units / a.nqc;
         const int c = unit % a.nqc;
         const bool has_items = unit / a.nqc < min(upc, a.n_tiles_work);
@@ -487,18 +426,18 @@ mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
             int last = 0;
             if (has_items) {
                 __threadfence();
-                const uint32_t done = atomicAdd(&a.sample_done[c * CG + cta_rank], 1u);
+                const uint32_t done = atomicAdd(&a.sample_done[c], 1u);
                 last = done == static_cast<uint32_t>(n_signing - 1);
-                if (last) a.sample_done[c * CG + cta_rank] = 0;  // ready for the next search
+                if (last) a.sample_done[c] = 0;  // ready for the next search
             }
             s_last = last;
         }
         __syncthreads();
-        if (s_last && warp >= 2) {
+        if (s_last && warp < kConsumerWarps) {
             __threadfence();
-            const int te = threadIdx.x - 64;          // 0..255
+            const int te = threadIdx.x;  // 0..255
             const int ql = te & (kBM - 1), part = te >> 7;
-            const int q = c * kChunk + static_cast<int>(cta_rank) * kBM + ql;
+            const int q = c * kBM + ql;
             const int n_blocks = a.sample_use;  // blocks j * sample_stride of the stored ones, j < sample_use
             float top[kSampleTop];
 #pragma unroll
@@ -519,7 +458,7 @@ mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
 #pragma unroll
                 for (int i = 0; i < kSampleTop; ++i) scratch[(i * kBM) + ql] = top[i];
             }
-            asm volatile("bar.sync 1, 256;" ::: "memory");  // the 8 epilogue warps
+            asm volatile("bar.sync 1, 256;" ::: "memory");  // the consumer warps
             if (part == 0) {
 #pragma unroll
                 for (int i = 0; i < kSampleTop; ++i) insert_top(top, scratch[(i * kBM) + ql]);
@@ -537,202 +476,6 @@ mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
                 }
             }
         }
-    }
-}
-
-// ---- Q-stationary form of the MAIN pass (A operand in tensor memory) ----------------------------
-// For embedding sizes up to 768 the unit's 256 queries fit in TENSOR MEMORY next to the accumulators
-// (128 lanes x D/2 32-bit columns per CTA: 384 columns at D = 768), so they are loaded ONCE per kernel
-// (tcgen05.st) and every MMA takes its A operand from TMEM: the query block is no longer re-fetched
-// from L2 for every corpus tile (that re-fetch doubled the L2 -> SM traffic of the smem-operand form:
-// 30.7 GB per 15.4 GB corpus pass at 10M x 768, profiles/r01_ncu_c3_main_kernel.txt) and shared memory
-// carries the corpus stream alone — a 4-deep ring of whole-K slabs (48 KB per CTA per tile).
-// What is left of TMEM holds two accumulator stages of N = 64 corpus rows (D > 512) or 128 (D <= 512).
-// CTA pairs only (cta_group::2, M = 256 across the pair); same warp roles, candidate segments and
-// exactness argument as mma_topk_kernel<kMain>.
-struct TsArgs {
-    KernelArgs k;
-    const void* q;        // queries in the storage dtype [nq_pad, dim], rows >= nq zero
-    int dim;
-    int tile_n;           // corpus rows per tile across the pair: 64 or 128
-    int n_stages;         // slabs in the shared-memory ring
-    int a_cols;           // TMEM columns holding the query block = kb_count * 32
-};
-
-__global__ void __launch_bounds__(kMmaThreads, 1)
-mma_ts_main_kernel(const __grid_constant__ CUtensorMap map_c, const TsArgs ta, const uint32_t idesc) {
-    const KernelArgs& a = ta.k;
-    constexpr int CG = 2;
-    constexpr int kChunk = kBM * CG;
-    const int rows_cta = ta.tile_n / CG;                       // corpus rows this CTA stages per tile
-    const int kb_bytes = rows_cta * kBK * 2;                   // one 64-wide K slice of the slab
-    const int slab_bytes = kb_bytes * a.kb_count;              // whole-K slab: [kb][rows][64]
-    extern __shared__ uint8_t smem_dyn[];
-    uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + static_cast<size_t>(ta.n_stages) * slab_bytes);
-    uint64_t* full = bars;                 // [8] TMA -> MMA      (the leader's copy is used)
-    uint64_t* empty = bars + 8;            // [8] MMA -> TMA      (each CTA its own)
-    uint64_t* tfull = bars + 16;           // [2] MMA -> epilogue (each CTA its own)
-    uint64_t* tempty = bars + 18;          // [2] epilogue -> MMA (the leader's copy is used)
-    uint64_t* a_full = bars + 20;          // [1] query block resident in TMEM, both CTAs (leader's copy)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 21);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t cta_rank = ptx::cluster_ctarank();
-    const int unit = blockIdx.x / CG, n_units = gridDim.x / CG;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < ta.n_stages; ++s) {
-            ptx::mbar_init(&full[s], 1);
-            ptx::mbar_init(&empty[s], 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            ptx::mbar_init(&tfull[s], 1);
-            ptx::mbar_init(&tempty[s], kEpiWarps * CG);
-        }
-        ptx::mbar_init(a_full, kEpiWarps * CG);
-        ptx::fence_mbar_init();
-        ptx::prefetch_tensormap(&map_c);
-    }
-    if (warp == 1) ptx::tmem_alloc_pair(tmem_slot, kTmemCols);
-    ptx::tc_fence_before();
-    ptx::cluster_sync_all();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t acc_base = tmem_base + static_cast<uint32_t>(ta.a_cols);
-
-    if (warp == 0) {
-        // ================= TMA producer: one whole-K slab of this CTA's rows per tile ==============
-        if (ptx::elect_one()) {
-            uint32_t stage = 0, phase = 0;
-            int t, c;
-            for (int i = 0; get_item(a, unit, n_units, i, t, c); ++i) {
-                const int32_t row0 = t * ta.tile_n + static_cast<int32_t>(cta_rank) * rows_cta;
-                ptx::mbar_wait(&empty[stage], phase ^ 1);
-                uint8_t* slab = tiles + static_cast<size_t>(stage) * slab_bytes;
-                const uint32_t lead_full = ptx::map_to_cta(ptx::smem_u32(&full[stage]), 0);
-                if (cta_rank == 0) ptx::mbar_expect_tx(&full[stage], 2 * slab_bytes);
-                for (int kb = 0; kb < a.kb_count; ++kb)
-                    ptx::tma_load_2d_pair(slab + static_cast<size_t>(kb) * kb_bytes, &map_c, lead_full, kb * kBK, row0,
-                                          ptx::kEvictFirst);
-                if (++stage == static_cast<uint32_t>(ta.n_stages)) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ================= MMA issuer (leader CTA): A from TMEM, B from the slab ===================
-        if (cta_rank == 0 && ptx::elect_one()) {
-            ptx::mbar_wait(a_full, 0);  // both CTAs' query blocks are in tensor memory
-            ptx::tc_fence_after();
-            uint32_t stage = 0, phase = 0;
-            int t, c;
-            for (int i = 0; get_item(a, unit, n_units, i, t, c); ++i) {
-                const uint32_t as = static_cast<uint32_t>(i) & 1u, aphase = (static_cast<uint32_t>(i) >> 1) & 1u;
-                ptx::mbar_wait(&tempty[as], aphase ^ 1);
-                ptx::mbar_wait(&full[stage], phase);
-                ptx::tc_fence_after();
-                const uint32_t d_tmem = acc_base + as * static_cast<uint32_t>(ta.tile_n);
-                const uint32_t slab = ptx::smem_u32(tiles + static_cast<size_t>(stage) * slab_bytes);
-                // one MMA per 16 K elements: B descriptor + 2 (32 bytes >> 4) inside a 64-wide slice, + one
-                // slice per K block; A = 8 more TMEM columns.  Kept to a handful of instructions per MMA: a
-                // single thread has to issue one every 32 tensor-pipe cycles at N = 64.
-                uint64_t db = ptx::make_kmajor_sw128_desc(slab);
-                const uint64_t db_step = static_cast<uint64_t>(kb_bytes >> 4);
-                uint32_t a_tmem = tmem_base;
-                ptx::umma_ts_f16_pair(d_tmem, a_tmem, db, idesc, 0u);
-                ptx::umma_ts_f16_pair(d_tmem, a_tmem + 8, db + 2, idesc, 1u);
-                ptx::umma_ts_f16_pair(d_tmem, a_tmem + 16, db + 4, idesc, 1u);
-                ptx::umma_ts_f16_pair(d_tmem, a_tmem + 24, db + 6, idesc, 1u);
-#pragma unroll 2
-                for (int kb = 1; kb < a.kb_count; ++kb) {
-                    db += db_step;
-                    a_tmem += 32;
-                    ptx::umma_ts_f16_pair(d_tmem, a_tmem, db, idesc, 1u);
-                    ptx::umma_ts_f16_pair(d_tmem, a_tmem + 8, db + 2, idesc, 1u);
-                    ptx::umma_ts_f16_pair(d_tmem, a_tmem + 16, db + 4, idesc, 1u);
-                    ptx::umma_ts_f16_pair(d_tmem, a_tmem + 24, db + 6, idesc, 1u);
-                }
-                ptx::umma_commit_pair(&empty[stage], 3);  // slab reusable (both CTAs) once these MMAs retire
-                ptx::umma_commit_pair(&tfull[as], 3);     // accumulator complete (both CTAs)
-                if (++stage == static_cast<uint32_t>(ta.n_stages)) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-        }
-    } else {
-        // ================= epilogue warps: first park the query block in TMEM, then screen tiles =====
-        const int quad = warp & 3;
-        const int half = (warp - 2) >> 2;
-        const int lane_q = static_cast<int>(cta_rank) * kBM + quad * 32 + lane;
-        const int my_q = (unit % a.nqc) * kChunk + lane_q;
-        const uint32_t lane_addr = static_cast<uint32_t>(quad * 32) << 16;
-        const uint32_t lead_tempty0 = ptx::map_to_cta(ptx::smem_u32(&tempty[0]), 0);
-        {
-            // this thread's query row: K slices `half`, half + 2, ... (the two column halves share the work);
-            // one 32-bit column = elements (2c, 2c+1), i.e. the row's bytes in order
-            const uint4* qrow = reinterpret_cast<const uint4*>(static_cast<const char*>(ta.q) +
-                                                               static_cast<size_t>(my_q) * ta.dim * 2);
-            const int n_vec = ta.dim / 8;  // 16-byte vectors in a row (dim % 8 == 0)
-            for (int kb = half; kb < a.kb_count; kb += 2) {
-                uint32_t r[32];
-#pragma unroll
-                for (int v = 0; v < 8; ++v) {
-                    const int vi = kb * 8 + v;
-                    uint4 x = make_uint4(0u, 0u, 0u, 0u);
-                    if (vi < n_vec) x = __ldg(qrow + vi);
-                    r[4 * v + 0] = x.x, r[4 * v + 1] = x.y, r[4 * v + 2] = x.z, r[4 * v + 3] = x.w;
-                }
-                ptx::tmem_st_32x32(tmem_base + lane_addr + static_cast<uint32_t>(kb * 32), r);
-            }
-            ptx::tmem_st_wait();
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive_cluster(ptx::map_to_cta(ptx::smem_u32(a_full), 0));
-        }
-        const int seg = (unit / a.nqc) * 2 + half;
-        uint64_t* const my_cand = a.cand + (static_cast<size_t>(my_q) * a.n_seg + seg) * a.cap_seg;
-        uint32_t n_admitted = 0;
-        const float tau = my_q < a.nq ? a.thr[my_q] : INFINITY;
-        const int cols_warp = ta.tile_n / 2;  // 32 or 64 columns per epilogue warp
-        int t, c;
-        for (int i = 0; get_item(a, unit, n_units, i, t, c); ++i) {
-            const uint32_t as = static_cast<uint32_t>(i) & 1u, aphase = (static_cast<uint32_t>(i) >> 1) & 1u;
-            const int64_t row0 = static_cast<int64_t>(t) * ta.tile_n + half * cols_warp;
-            const int ncols = static_cast<int>(max(static_cast<int64_t>(0),
-                                                   min(static_cast<int64_t>(cols_warp), a.n_rows - row0)));
-            ptx::mbar_wait(&tfull[as], aphase);
-            ptx::tc_fence_after();
-            const uint32_t taddr = acc_base + lane_addr + as * static_cast<uint32_t>(ta.tile_n) +
-                                   static_cast<uint32_t>(half * cols_warp);
-            auto process = [&](const uint32_t (&v)[32], int c0) {
-                const int nvalid = min(32, ncols - c0);
-                const uint32_t rbase = static_cast<uint32_t>(row0 + c0);  // a multiple of 32
-                uint32_t amask = nvalid >= 32 ? 0xFFFFFFFFu : ((1u << nvalid) - 1u);
-                if (a.row_mask) amask &= a.row_mask[rbase >> 5];
-                admit_chunk(v, tau, rbase, amask, my_cand, n_admitted, a.cap_seg);
-            };
-            uint32_t va[32], vb[32];
-            if (ncols > 0) ptx::tmem_ld_32x32(taddr, va);
-            if (ncols > 32) ptx::tmem_ld_32x32(taddr + 32, vb);
-            ptx::tmem_ld_wait();
-            // the accumulator is in registers: hand the TMEM stage back before screening
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive_cluster(lead_tempty0 + as * 8);
-            if (ncols > 0) process(va, 0);
-            if (ncols > 32) process(vb, 32);
-        }
-        if (unit / a.nqc < n_units / a.nqc) a.cand_count[static_cast<size_t>(my_q) * a.n_seg + seg] = n_admitted;
-    }
-
-    ptx::tc_fence_before();
-    ptx::cluster_sync_all();
-    if (warp == 1) {
-        __syncwarp();
-        ptx::tmem_dealloc_pair(tmem_base, kTmemCols);
     }
 }
 
@@ -965,58 +708,35 @@ bool encode_map(CUtensorMap* map, int dtype, const void* base, int64_t rows, int
 
 struct Plan {
     int sms;
-    int cg;            // 1: single CTAs (<= 128 queries), 2: CTA pairs
-    int chunk;         // queries per chunk = 128 * cg
-    int nqc;           // query chunks
-    int nq_pad;        // nqc * chunk
+    int nqc;           // query chunks of 128
+    int nq_pad;        // nqc * 128
+    int tile_n;        // corpus rows per tile: 256, or 128 in the split form
     int n_tiles;
     int n_full_tiles;
     int kb_count;
     int n_sample;      // tiles in the sample pass (0 = no sampling)
-    int sample_gph;    // blocks per thread per tile in the sample pass (block = 128 / sample_gph rows)
+    int sample_gph;    // blocks per 128 rows in the sample pass (block = 128 / sample_gph rows)
     int sample_use;    // blocks the threshold uses, every sample_stride-th of the stored ones
     int sample_stride;
     int sample_units;  // a multiple of nqc
     int main_units;    // a multiple of nqc
-    int n_seg;         // candidate segments per query = 2 * main_units / nqc
+    int n_seg;         // candidate segments per query = 4 * main_units / nqc
     uint32_t cap_seg;  // rows a segment holds
-    bool ts;           // MAIN runs in the Q-stationary form (query block in tensor memory)
-    int tile_n;        // corpus rows per MAIN tile: 256, or 64 / 128 in the Q-stationary form
-    int n_main_tiles;
-    int ts_stages;     // slabs in the Q-stationary form's shared-memory ring
-    size_t ts_smem;
     // workspace offsets
     size_t off_q, off_q_lo, off_sample, off_thr, off_floor, off_count, off_done, off_cand, total;
 };
 
-bool ts_enabled() {
-    static const bool on = getenv("TAV_NO_TS") == nullptr;  // diagnostic switch: force the smem-operand form
-    return on;
-}
-
-Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split, bool no_ts = false) {
+Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split) {
     Plan p{};
-    p.sms = 148;
+    p.sms = 132;
     cudaDeviceGetAttribute(&p.sms, cudaDevAttrMultiProcessorCount, device);
-    p.cg = nq > kBM ? 2 : 1;
-    p.chunk = kBM * p.cg;
-    p.nqc = std::max(1, (nq + p.chunk - 1) / p.chunk);
-    p.nq_pad = p.nqc * p.chunk;
-    p.n_tiles = static_cast<int>((n_rows + kBN - 1) / kBN);
-    p.n_full_tiles = static_cast<int>(n_rows / kBN);
+    p.nqc = std::max(1, (nq + kBM - 1) / kBM);
+    p.nq_pad = p.nqc * kBM;
+    p.tile_n = split ? kTileRowsSplit : kTileRows;
+    p.n_tiles = static_cast<int>((n_rows + p.tile_n - 1) / p.tile_n);
+    p.n_full_tiles = static_cast<int>(n_rows / p.tile_n);
     p.kb_count = (dim + kBK - 1) / kBK;
-    // Q-stationary MAIN: CTA pairs, 16-bit storage, query block (kb_count * 32 TMEM columns) + two
-    // accumulator stages within the 512 columns of tensor memory
-    p.ts = p.cg == 2 && !split && !no_ts && p.kb_count * 32 <= 384 && ts_enabled();
-    p.tile_n = !p.ts ? kBN : (p.kb_count * 32 > 256 ? 64 : 128);
-    p.n_main_tiles = static_cast<int>((n_rows + p.tile_n - 1) / p.tile_n);
-    if (p.ts) {
-        const size_t slab = static_cast<size_t>(p.tile_n / 2) * kBK * 2 * p.kb_count;
-        const size_t room = 232448 - 1024 - 256 - kScratchBytes;  // 227 KB per CTA minus alignment, barriers, scratch
-        p.ts_stages = static_cast<int>(std::max<size_t>(2, std::min<size_t>(8, room / slab)));
-        p.ts_smem = 1024 + p.ts_stages * slab + 256 + kScratchBytes;
-    }
-    const int max_units = p.cg == 2 ? std::max(1, p.sms / 2) : p.sms;
+    const int max_units = p.sms;
     // Rows we aim to admit per query (`target`).  The threshold is the m-th largest (m = kSampleTop = 8)
     // block maximum of a uniform sample of L blocks of 128 rows; with p = target / N the chance that a
     // block's maximum clears the p-quantile is q_b = 1 - (1-p)^128, so L = m / q_b blocks put the m-th
@@ -1028,7 +748,7 @@ Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split, b
     // For k <= 8 nothing can starve, so small corpora aim much lower (32 rows: a quarter of the corpus is
     // sampled, with the branch-free epilogue, and MAIN's epilogue then rarely has anything to append).
     static const int64_t small_k_floor = [] {
-        const char* e = getenv("TAV_SMALLK_TARGET");  // tuning knob (profiles/r02_c5_target_sweep.log)
+        const char* e = getenv("TAV_SMALLK_TARGET");  // tuning knob of the small-k admission target
         const int64_t v = e ? atoll(e) : 0;
         return v >= 8 ? v : int64_t(32);
     }();
@@ -1036,21 +756,23 @@ Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split, b
                                ? std::min<int64_t>(2048, std::max<int64_t>(small_k_floor, n_rows / 4096))
                                : std::max<int64_t>(16ll * k, std::min<int64_t>(2048, std::max<int64_t>(128, n_rows / 4096)));
     int64_t admitted = n_rows;  // rows a query is expected to admit
+    const int64_t per_tile = static_cast<int64_t>(p.tile_n / 128);  // 128-row spans per tile (x sample_gph blocks)
     if (n_rows <= 16384 || 8 * target >= n_rows || p.n_full_tiles < 8) {
         p.n_sample = 0;
     } else {
         // Block size: the m-th largest of L block maxima sits at the row quantile p when 1 - (1-p)^b = m / L;
         // for p * b well above 1 every block clears the quantile and the maxima say nothing about it (the
         // threshold would come out too high and queries starve).  So mid-size corpora — where the target is a
-        // larger fraction of the rows — use blocks of 32 or 8 rows instead of a thread's 128.
+        // larger fraction of the rows — use blocks of 32 or 8 rows instead of 128.
         const double prob = static_cast<double>(target) / static_cast<double>(n_rows);
         const int block_rows = prob * 128 <= 0.7 ? 128 : (prob * 32 <= 0.7 ? 32 : 8);
         p.sample_gph = 128 / block_rows;
         const double q_b = 1.0 - pow(1.0 - prob, static_cast<double>(block_rows));
         const int64_t blocks = static_cast<int64_t>(ceil(kSampleTop / q_b));
-        const int64_t per_tile = 2ll * p.sample_gph;
-        p.n_sample = static_cast<int>(std::min<int64_t>(p.n_full_tiles, std::max<int64_t>(4, (blocks + per_tile - 1) / per_tile)));
-        const int64_t stored = static_cast<int64_t>(p.n_sample) * per_tile;
+        const int64_t blocks_per_tile = per_tile * p.sample_gph;
+        p.n_sample = static_cast<int>(std::min<int64_t>(
+            p.n_full_tiles, std::max<int64_t>(4, (blocks + blocks_per_tile - 1) / blocks_per_tile)));
+        const int64_t stored = static_cast<int64_t>(p.n_sample) * blocks_per_tile;
         p.sample_use = static_cast<int>(std::min<int64_t>(blocks, stored));
         p.sample_stride = static_cast<int>(std::max<int64_t>(1, stored / p.sample_use));
         admitted = target;
@@ -1061,15 +783,16 @@ Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split, b
         p.sample_units = per_chunk * p.nqc;  // may exceed max_units when nqc > max_units: extra units queue
     }
     {
-        // every unit of a chunk owns two candidate segments per query (one per epilogue column half):
-        // room for 16x the expected share of a segment, and for every row it can see when nothing is cut
-        const int per_chunk =
-            std::max(1, std::min(std::min(std::max(1, max_units / p.nqc), p.n_main_tiles), kMaxSegments / 2));
+        // every unit of a chunk owns four candidate segments per query (one per thread of the quad that
+        // holds the query): room for 16x the expected share of a segment (at least half a tile's share),
+        // and for every row it can see when nothing is cut
+        const int per_chunk = std::max(
+            1, std::min(std::min(std::max(1, max_units / p.nqc), p.n_tiles), kMaxSegments / kSegPerUnit));
         p.main_units = per_chunk * p.nqc;
-        p.n_seg = 2 * per_chunk;
-        const int64_t tiles_per_unit = (p.n_main_tiles + per_chunk - 1) / per_chunk;
-        const int64_t seen = tiles_per_unit * (p.tile_n / 2);
-        const int64_t want = p.n_sample == 0 ? seen : std::max<int64_t>(64, (16 * admitted + p.n_seg - 1) / p.n_seg);
+        p.n_seg = kSegPerUnit * per_chunk;
+        const int64_t tiles_per_unit = (p.n_tiles + per_chunk - 1) / per_chunk;
+        const int64_t seen = tiles_per_unit * (p.tile_n / kSegPerUnit);
+        const int64_t want = p.n_sample == 0 ? seen : std::max<int64_t>(p.tile_n / (2 * kSegPerUnit), (16 * admitted + p.n_seg - 1) / p.n_seg);
         p.cap_seg = static_cast<uint32_t>(std::min<int64_t>(want, seen));
     }
     auto align = [](size_t v) { return (v + 255) & ~size_t(255); };
@@ -1077,13 +800,14 @@ Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split, b
     // the search: they must read zero at the start of every search and only the kernels ever write them
     size_t off = 0;
     p.off_done = off;
-    off = align(off + static_cast<size_t>(kMaxChunks) * 2 * sizeof(uint32_t));
+    off = align(off + static_cast<size_t>(kMaxChunks) * sizeof(uint32_t));
     p.off_q = off;
     off = align(off + static_cast<size_t>(p.nq_pad) * dim * 2);
     p.off_q_lo = off;  // lo plane of the queries (split form only; reserved always)
     off = align(off + static_cast<size_t>(p.nq_pad) * dim * 2);
-    p.off_sample = off;  // block maxima [n_sample * 2, nq_pad]
-    off = align(off + static_cast<size_t>(std::max(1, p.n_sample)) * 2 * std::max(1, p.sample_gph) * p.nq_pad * sizeof(float));
+    p.off_sample = off;  // block maxima [n_sample * blocks per tile, nq_pad]
+    off = align(off + static_cast<size_t>(std::max(1, p.n_sample)) * per_tile * std::max(1, p.sample_gph) * p.nq_pad *
+                          sizeof(float));
     p.off_thr = off;
     off = align(off + static_cast<size_t>(p.nq_pad) * sizeof(float));
     p.off_floor = off;
@@ -1097,51 +821,34 @@ Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split, b
 }
 
 struct Maps {
-    CUtensorMap q, q_lo;        // queries (hi plane / lo plane when split)
-    CUtensorMap c1, c1_lo;      // corpus, 256-row boxes (single CTA)
-    CUtensorMap c2, c2_lo;      // corpus, 128-row boxes (per CTA of a pair)
+    CUtensorMap q, q_lo;  // queries, 128-row boxes (hi plane / lo plane when split)
+    CUtensorMap c, c_lo;  // corpus, one tile of rows per box
 };
 
-template <int MODE, int CG, bool SPLIT>
-cudaError_t launch_kernel_cg(const Maps& m, const KernelArgs& ka, uint32_t idesc, int units, cudaStream_t s) {
-    auto kern = mma_topk_kernel<MODE, CG, SPLIT>;
+template <int MODE, bool BF16, bool SPLIT>
+cudaError_t launch_kernel_t(const Maps& m, const KernelArgs& ka, int units, cudaStream_t s) {
+    auto kern = mma_topk_kernel<MODE, BF16, SPLIT>;
     static int granted[16] = {};
     cudaError_t e = ensure_dynamic_smem(kern, kSmemBytes, granted);
     if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(units * CG));
-    cfg.blockDim = dim3(kMmaThreads);
-    cfg.dynamicSmemBytes = kSmemBytes;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CG;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (CG == 2) return cudaLaunchKernelEx(&cfg, kern, m.q, m.c2, m.q_lo, m.c2_lo, ka, idesc);
-    return cudaLaunchKernelEx(&cfg, kern, m.q, m.c1, m.q_lo, m.c1_lo, ka, idesc);
+    kern<<<units, kMmaThreads, kSmemBytes, s>>>(m.q, m.c, m.q_lo, m.c_lo, ka);
+    return cudaGetLastError();
 }
 
-// cg == 2 (more than 128 queries): CTA pairs; cg == 1: single CTAs; split: two-plane fp16 (float32 data)
+// split: two-plane fp16 (float32 data)
 template <int MODE>
-cudaError_t launch_kernel(const Maps& m, const KernelArgs& ka, int cg, int dtype, bool split, int units,
-                          cudaStream_t s) {
-    const int fmt = dtype == TAV_BF16 ? 1 : 0;
-    const uint32_t idesc = ptx::make_idesc_f16(cg * kBM, kBN, fmt);
-    if (cg == 2)
-        return split ? launch_kernel_cg<MODE, 2, true>(m, ka, idesc, units, s)
-                     : launch_kernel_cg<MODE, 2, false>(m, ka, idesc, units, s);
-    return split ? launch_kernel_cg<MODE, 1, true>(m, ka, idesc, units, s)
-                 : launch_kernel_cg<MODE, 1, false>(m, ka, idesc, units, s);
+cudaError_t launch_kernel(const Maps& m, const KernelArgs& ka, int dtype, bool split, int units, cudaStream_t s) {
+    if (split) return launch_kernel_t<MODE, false, true>(m, ka, units, s);
+    if (dtype == TAV_BF16) return launch_kernel_t<MODE, true, false>(m, ka, units, s);
+    return launch_kernel_t<MODE, false, false>(m, ka, units, s);
 }
 
 cudaError_t prep_queries(const MmaArgs& a, void* dst, void* dst_lo, int nq_pad, int init_state, float* thr,
                          float* floor_out, cudaStream_t s) {
     const int64_t total = static_cast<int64_t>(nq_pad) * a.dim;
     const int grid = static_cast<int>(std::max<int64_t>(
-        std::min<int64_t>((total + 255) / 256, 148 * 8), init_state ? (a.nq + 255) / 256 : 1));
+        std::min<int64_t>((total + 255) / 256, 132 * 8),
+        init_state ? (a.nq + 255) / 256 : 1));
     if (a.split) {
         split_rows_kernel<<<grid, 256, 0, s>>>(a.queries, static_cast<__half*>(dst), static_cast<__half*>(dst_lo),
                                                a.nq, nq_pad, a.dim, a.split_overflow, a.split_overflow_host, init_state,
@@ -1169,7 +876,7 @@ cudaError_t launch_split_rows(const float* src, void* hi, void* lo, int64_t n, i
                               cudaStream_t s) {
     if (n == 0) return cudaSuccess;
     const int64_t total = n * dim;
-    const int grid = static_cast<int>(std::min<int64_t>((total + 255) / 256, 148 * 16));
+    const int grid = static_cast<int>(std::min<int64_t>((total + 255) / 256, 132 * 16));
     split_rows_kernel<<<grid, 256, 0, s>>>(src, static_cast<__half*>(hi), static_cast<__half*>(lo), n, n, dim, overflow,
                                            nullptr, 0, 0.0f, nullptr, nullptr, nullptr);
     return cudaGetLastError();
@@ -1181,46 +888,41 @@ inline int mma_dtype(const MmaArgs& a) { return a.split ? TAV_F16 : a.dtype; }
 
 bool build_maps_uncached(const MmaArgs& a, const void* d_q, const void* d_q_lo, int nq_pad, Maps& m);
 
-// cuTensorMapEncodeTiled costs 1-2 us a piece and a search needs seven: remember, per device, the maps of
+// cuTensorMapEncodeTiled costs 1-2 us a piece and a search needs four: remember, per device, the maps of
 // the last search (serving loops repeat the same corpus / workspace pointers and shapes)
 struct MapCacheEntry {
     const void *corpus = nullptr, *corpus_lo = nullptr, *q = nullptr, *q_lo = nullptr;
     int64_t n = -1;
-    int dim = 0, dt = -1, nq_pad = 0, ts_rows = 0;
+    int dim = 0, dt = -1, nq_pad = 0;
     Maps maps;
-    CUtensorMap ts;
     bool valid = false;
 };
 std::mutex g_map_mu;
 MapCacheEntry g_map_cache[16];
 
-bool build_maps(const MmaArgs& a, const void* d_q, const void* d_q_lo, int nq_pad, int ts_rows, Maps& m,
-                CUtensorMap* ts_map) {
+bool build_maps(const MmaArgs& a, const void* d_q, const void* d_q_lo, int nq_pad, Maps& m) {
     const int dt = mma_dtype(a);
     std::lock_guard<std::mutex> lock(g_map_mu);
     MapCacheEntry& e = g_map_cache[a.device >= 0 && a.device < 16 ? a.device : 0];
     const void* lo = a.split ? a.corpus_lo : nullptr;
     if (!(e.valid && e.corpus == a.corpus && e.corpus_lo == lo && e.q == d_q && e.q_lo == d_q_lo && e.n == a.n_corpus &&
-          e.dim == a.dim && e.dt == dt && e.nq_pad == nq_pad && e.ts_rows == ts_rows)) {
+          e.dim == a.dim && e.dt == dt && e.nq_pad == nq_pad)) {
         e.valid = false;
         if (!build_maps_uncached(a, d_q, d_q_lo, nq_pad, e.maps)) return false;
-        if (ts_rows > 0 && !encode_map(&e.ts, dt, a.corpus, a.n_corpus, a.dim, ts_rows)) return false;
         e.corpus = a.corpus, e.corpus_lo = lo, e.q = d_q, e.q_lo = d_q_lo, e.n = a.n_corpus;
-        e.dim = a.dim, e.dt = dt, e.nq_pad = nq_pad, e.ts_rows = ts_rows;
+        e.dim = a.dim, e.dt = dt, e.nq_pad = nq_pad;
         e.valid = true;
     }
     m = e.maps;
-    if (ts_map && ts_rows > 0) *ts_map = e.ts;
     return true;
 }
 
 bool build_maps_uncached(const MmaArgs& a, const void* d_q, const void* d_q_lo, int nq_pad, Maps& m) {
     const int dt = mma_dtype(a);
-    if (!encode_map(&m.c1, dt, a.corpus, a.n_corpus, a.dim, kBN)) return false;
-    if (!encode_map(&m.c2, dt, a.corpus, a.n_corpus, a.dim, kBN / 2)) return false;
+    const int tile_n = a.split ? kTileRowsSplit : kTileRows;
+    if (!encode_map(&m.c, dt, a.corpus, a.n_corpus, a.dim, tile_n)) return false;
     const void* lo = a.split ? a.corpus_lo : a.corpus;  // unused maps still need a valid encoding
-    if (!encode_map(&m.c1_lo, dt, lo, a.n_corpus, a.dim, kBN)) return false;
-    if (!encode_map(&m.c2_lo, dt, lo, a.n_corpus, a.dim, kBN / 2)) return false;
+    if (!encode_map(&m.c_lo, dt, lo, a.n_corpus, a.dim, tile_n)) return false;
     if (!encode_map(&m.q, dt, d_q, nq_pad, a.dim, kBM)) return false;
     return encode_map(&m.q_lo, dt, a.split ? d_q_lo : d_q, nq_pad, a.dim, kBM);
 }
@@ -1232,13 +934,13 @@ bool args_ok(const MmaArgs& a) {
 }  // namespace
 
 size_t mma_workspace_bytes(const MmaArgs& a) {
-    return make_plan(a.device, a.n_corpus, a.dim, a.nq, a.k, a.split != 0, a.no_ts != 0).total;
+    return make_plan(a.device, a.n_corpus, a.dim, a.nq, a.k, a.split != 0).total;
 }
 
 cudaError_t launch_mma_search(const MmaArgs& a, void* workspace, size_t workspace_bytes, cudaStream_t s,
                               int* launches) {
     if (!args_ok(a) || a.k > kPassK || a.nq < 1 || a.nq > kMmaMaxQueries) return cudaErrorInvalidValue;
-    const Plan p = make_plan(a.device, a.n_corpus, a.dim, a.nq, a.k, a.split != 0, a.no_ts != 0);
+    const Plan p = make_plan(a.device, a.n_corpus, a.dim, a.nq, a.k, a.split != 0);
     if (workspace_bytes < p.total) return cudaErrorInvalidValue;
     char* ws = static_cast<char*>(workspace);
     void* d_q = ws + p.off_q;
@@ -1267,8 +969,7 @@ cudaError_t launch_mma_search(const MmaArgs& a, void* workspace, size_t workspac
 
     // tensor maps first (host work only), so that the launches below go out back to back
     Maps maps;
-    CUtensorMap map_ts;
-    if (!build_maps(a, d_q, d_q_lo, p.nq_pad, p.ts ? p.tile_n / 2 : 0, maps, &map_ts)) return cudaErrorUnknown;
+    if (!build_maps(a, d_q, d_q_lo, p.nq_pad, maps)) return cudaErrorUnknown;
 
     // queries -> storage dtype; without a sample pass this launch also initialises thresholds / counters
     if ((e = ev_begin_kind(2)) != cudaSuccess) return e;
@@ -1306,45 +1007,17 @@ cudaError_t launch_mma_search(const MmaArgs& a, void* workspace, size_t workspac
         ka.tile_mul = p.n_full_tiles;
         ka.tile_div = p.n_sample;
         if ((e = ev_begin_kind(1)) != cudaSuccess) return e;
-        e = launch_kernel<kSample>(maps, ka, p.cg, kdt, split, p.sample_units, s);
+        e = launch_kernel<kSample>(maps, ka, kdt, split, p.sample_units, s);
         if (e != cudaSuccess) return e;
         if ((e = ev_end(1)) != cudaSuccess) return e;
         ++n_launch;
     }
 
-    ka.n_tiles_work = p.n_main_tiles;
+    ka.n_tiles_work = p.n_tiles;
     ka.tile_mul = 1;
     ka.tile_div = 1;
     if ((e = ev_begin_kind(0)) != cudaSuccess) return e;
-    if (p.ts) {
-        // Q-stationary form: query block in tensor memory, corpus slabs through shared memory
-        TsArgs ta{};
-        ta.k = ka;
-        ta.q = d_q;
-        ta.dim = a.dim;
-        ta.tile_n = p.tile_n;
-        ta.n_stages = p.ts_stages;
-        ta.a_cols = p.kb_count * 32;
-        static int ts_granted[16] = {};
-        e = ensure_dynamic_smem(mma_ts_main_kernel, p.ts_smem, ts_granted);
-        if (e != cudaSuccess) return e;
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(static_cast<unsigned>(p.main_units * 2));
-        cfg.blockDim = dim3(kMmaThreads);
-        cfg.dynamicSmemBytes = p.ts_smem;
-        cfg.stream = s;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        const uint32_t idesc_ts = ptx::make_idesc_f16(2 * kBM, p.tile_n, kdt == TAV_BF16 ? 1 : 0);
-        e = cudaLaunchKernelEx(&cfg, mma_ts_main_kernel, map_ts, ta, idesc_ts);
-    } else {
-        e = launch_kernel<kMain>(maps, ka, p.cg, kdt, split, p.main_units, s);
-    }
+    e = launch_kernel<kMain>(maps, ka, kdt, split, p.main_units, s);
     if (e != cudaSuccess) return e;
     if ((e = ev_end(0)) != cudaSuccess) return e;
     ++n_launch;
@@ -1375,7 +1048,7 @@ cudaError_t launch_mma_search(const MmaArgs& a, void* workspace, size_t workspac
 // Debug / verification entry: all raw dot products of the tensor-core path, out[nq, n_rows] (device).
 cudaError_t launch_mma_dump(const MmaArgs& a, void* workspace, size_t workspace_bytes, float* out, cudaStream_t s) {
     if (!args_ok(a) || a.nq < 1 || a.nq > kMmaMaxQueries) return cudaErrorInvalidValue;
-    Plan p = make_plan(a.device, a.n_corpus, a.dim, a.nq, 1, a.split != 0, true);
+    Plan p = make_plan(a.device, a.n_corpus, a.dim, a.nq, 1, a.split != 0);
     if (workspace_bytes < p.total) return cudaErrorInvalidValue;
     char* ws = static_cast<char*>(workspace);
     void* d_q = ws + p.off_q;
@@ -1383,7 +1056,7 @@ cudaError_t launch_mma_dump(const MmaArgs& a, void* workspace, size_t workspace_
     cudaError_t e = prep_queries(a, d_q, d_q_lo, p.nq_pad, 0, nullptr, nullptr, s);
     if (e != cudaSuccess) return e;
     Maps maps;
-    if (!build_maps(a, d_q, d_q_lo, p.nq_pad, 0, maps, nullptr)) return cudaErrorUnknown;
+    if (!build_maps(a, d_q, d_q_lo, p.nq_pad, maps)) return cudaErrorUnknown;
     KernelArgs ka{};
     ka.n_rows = a.n_corpus;
     ka.kb_count = p.kb_count;
@@ -1394,7 +1067,7 @@ cudaError_t launch_mma_dump(const MmaArgs& a, void* workspace, size_t workspace_
     ka.tile_mul = 1;
     ka.tile_div = 1;
     ka.dump = out;
-    return launch_kernel<kDump>(maps, ka, p.cg, mma_dtype(a), a.split != 0, p.main_units, s);
+    return launch_kernel<kDump>(maps, ka, mma_dtype(a), a.split != 0, p.main_units, s);
 }
 
 }  // namespace tav

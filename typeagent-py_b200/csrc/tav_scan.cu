@@ -409,7 +409,7 @@ scan_rows_kernel(const ScanArgs a, const __grid_constant__ BLOB blob) {
 
 int scan_grid(int device, int dtype, int dim, int nq, int k, int64_t n_scan) {
     (void)dtype;
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     const size_t smem = scan_smem_bytes(nq, dim, k);
     int per_sm = static_cast<int>((200 * 1024) / (smem + 1024));
@@ -463,17 +463,17 @@ bool scan1_fits(int dim, int k, int64_t n_scan, int64_t subset_len, bool has_sub
     if (has_subset && subset_len > kParamSubsetMax) return false;
     // the last CTA sorts every CTA's k survivors at once: a full wave of CTAs must fit its buffer
     const int64_t tiles = (n_scan + kRoundRows - 1) / kRoundRows;
-    return static_cast<int64_t>(k) * std::min<int64_t>(tiles, 148) <= kFusedSelectMax;
+    return static_cast<int64_t>(k) * std::min<int64_t>(tiles, 132) <= kFusedSelectMax;
 }
 
 int scan1_grid(int device, int dim, int k, int64_t n_scan) {
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     int64_t tiles = (n_scan + kRoundRows - 1) / kRoundRows;
     // up to 4 CTAs per SM (the general form's occupancy), one round of rows per CTA while the rows last.  The
-    // last CTA merges grid * k survivors: its buffer bounds the grid, and for the rank-selection merge (k <= 32,
-    // ~2.3 us per 1000 survivors) so does its cost — measured on 10k x 384, k = 10 (profiles/r02_latency_grid_sweep.log):
-    // 2048 survivors (204 CTAs, two rounds each) beats 8192 (313 CTAs, one round) by 4.7 us and 512 by 4.2 us.
+    // last CTA merges grid * k survivors: its buffer bounds the grid, and for the rank-selection merge (k <= 32)
+    // so does its cost, which grows with the survivors; 2048 survivors balance that merge against the rounds of
+    // rows per CTA (TAV_SCAN1_SURVIVORS overrides it).
     int64_t g = std::min<int64_t>(tiles, 4ll * sms);
     static const int64_t survivors_env = [] {
         const char* e = getenv("TAV_SCAN1_SURVIVORS");  // tuning knob for that sweep
@@ -787,7 +787,7 @@ template <typename S>
 static cudaError_t launch_convert_s(const S* src, void* dst, int dst_dtype, int64_t n, int dim,
                                     int normalize, cudaStream_t s) {
     int64_t blocks = (n + 7) / 8;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks < 1) blocks = 1;
     const int g = static_cast<int>(blocks);
     switch (dst_dtype) {

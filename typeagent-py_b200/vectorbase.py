@@ -98,7 +98,7 @@ def _as_f32_scalar(value: float) -> np.float32:
 
 
 class VectorBase:
-    """In-HBM embedding matrix with brute-force top-k lookup on a B200."""
+    """In-HBM embedding matrix with brute-force top-k lookup on an H100."""
 
     def __init__(
         self,
@@ -329,8 +329,6 @@ class VectorBase:
             return _capi.TAV_FORCE_SCAN | _capi.TAV_NO_FUSED_SCAN
         if self.force_path == "mma":
             return _capi.TAV_FORCE_MMA
-        if self.force_path == "mma_smem":   # tensor cores with the query block in shared memory (no TMEM parking)
-            return _capi.TAV_FORCE_MMA | _capi.TAV_NO_TMEM_QUERIES
         return 0
 
     # ------------------------------------------------------------------ row masks
