@@ -19,6 +19,7 @@ import pytest
 
 import typeagent_py_b200 as tab
 from oracle import vectorbase_oracle as O
+from tests.exact import dot_error_bound
 from tests.parity import assert_hits_match
 from typeagent_py_b200 import _capi
 
@@ -46,7 +47,7 @@ def mma_scores(base, q):
 
 @pytest.mark.parametrize("storage", ["bfloat16", "float16"])
 @pytest.mark.parametrize("n,d,b", [(256, 64, 128), (1000, 768, 5), (3001, 136, 130), (700, 1536, 256),
-                                    (513, 8, 300), (40000, 384, 64)])
+                                    (513, 8, 300), (40000, 384, 64), (3001, 72, 1), (2000, 64, 133 * 128 + 5)])
 def test_every_dot_product_of_the_tensor_core_path(storage, n, d, b):
     v, q = O.make_corpus(n, d, seed=n + d, n_queries=b)
     vr, qr = O.round_to_storage(v, storage), O.round_to_storage(q, storage)
@@ -54,7 +55,9 @@ def test_every_dot_product_of_the_tensor_core_path(storage, n, d, b):
     got = mma_scores(base, q)
     want = qr.astype(np.float64) @ vr.astype(np.float64).T
     assert got.shape == want.shape
-    # fp32 accumulation of exact products: error ~ sqrt(d) * 2^-24 * |x|; bound generously
+    # fp32 accumulation of exact products: at most gamma_d * sum |q_i v_i| in any order, typically
+    # ~sqrt(d) * 2^-24 * |x|
+    assert (np.abs(got - want) <= dot_error_bound(qr, vr)).all()
     np.testing.assert_allclose(got, want, atol=2e-6, rtol=0)
 
 
@@ -243,13 +246,15 @@ def test_many_query_chunks_one_pass(storage, n, d, b, k):
 
 
 # ------------------------------------------------------------------ float32 index on tensor cores
-@pytest.mark.parametrize("n,d,b", [(256, 64, 128), (3001, 136, 130), (700, 1536, 256), (40000, 384, 64)])
+@pytest.mark.parametrize("n,d,b", [(256, 64, 128), (3001, 136, 130), (700, 1536, 256), (40000, 384, 64),
+                                   (3001, 72, 1), (2000, 64, 133 * 128 + 5)])
 def test_split_every_dot_product_float32(n, d, b):
     """float32 rows as two fp16 planes (x = hi + lo/2048): every dot vs float64 on the UNROUNDED data."""
     v, q = O.make_corpus(n, d, seed=n + d + 1, n_queries=b)
     base = make_base(v, "float32")
     got = mma_scores(base, q)
     want = q.astype(np.float64) @ v.astype(np.float64).T
+    assert (np.abs(got - want) <= dot_error_bound(q, v, split=True)).all()
     np.testing.assert_allclose(got, want, atol=1e-6, rtol=0)
     assert np.abs(got - want).max() < 5e-7
 

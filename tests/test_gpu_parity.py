@@ -308,16 +308,22 @@ def test_query_shape_errors():
 
 
 # ------------------------------------------------------------------ sharded merge on one GPU
-@pytest.mark.parametrize("world", [2, 3, 8])
-def test_shard_merge_kernel_equals_unsharded(world):
+@pytest.mark.parametrize("world,dyadic", [pytest.param(2, False, id="2"), pytest.param(3, False, id="3"),
+                                          pytest.param(8, False, id="8"), pytest.param(3, True, id="3-dyadic_coarse")])
+def test_shard_merge_kernel_equals_unsharded(world, dyadic):
     """Split the corpus over `world` indexes on this GPU, search each with its row offset,
-    pack as the all-gather would, merge with tav_merge_topk: bit-identical to one index."""
+    pack as the all-gather would, merge with tav_merge_topk: bit-identical to one index
+    (and, on an exact-arithmetic corpus with heavy ties, to tests/exact.py's expectation)."""
     import torch
 
+    from tests.exact import dyadic_corpus, expected_topk, preset
     from typeagent_py_b200.sharded import CudaShardEngine, packed_layout, shard_bounds
 
-    v, q = O.make_corpus(5003, 64, 131, n_queries=9)
-    v = np.concatenate([v, v[:50]])  # exact duplicates across shards -> exact ties
+    if dyadic:
+        v, q, dots = dyadic_corpus(5003, 64, 9, *preset("coarse", 64), seed=131)
+    else:
+        v, q = O.make_corpus(5003, 64, 131, n_queries=9)
+        v = np.concatenate([v, v[:50]])  # exact duplicates across shards -> exact ties
     k, ms = 25, 0.45
     whole = gpu_base(v)
     want_items, want_scores, want_counts = whole.search_arrays(q, k, ms)
@@ -336,6 +342,12 @@ def test_shard_merge_kernel_equals_unsharded(world):
         c = want_counts[b]
         np.testing.assert_array_equal(items[b, :c].cpu().numpy(), want_items[b, :c])
         np.testing.assert_array_equal(scores[b, :c].cpu().numpy(), want_scores[b, :c])
+    if dyadic:
+        e_items, e_scores, e_counts = expected_topk(dots, k, ms)
+        np.testing.assert_array_equal(counts.cpu().numpy(), e_counts)
+        for b, c in enumerate(e_counts):
+            np.testing.assert_array_equal(items[b, :c].cpu().numpy(), e_items[b, :c])
+            np.testing.assert_array_equal(scores[b, :c].cpu().numpy(), e_scores[b, :c])
 
 
 def test_device_tensor_handles_and_timing():
