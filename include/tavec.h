@@ -125,12 +125,38 @@ int tav_read_rows(tav_index* ix, int64_t first, int64_t n, float* out_host, void
  *   out_counts [n_queries]    int32   number of valid entries per query (<= k)
  *
  * k must be >= 1 (the caller turns the reference's "max_hits == 0 means everything",
- * quirk Q2, into k = number of rows).  Any k is accepted; above TAV_PASS_K rows per
- * query the search runs in several passes.
+ * quirk Q2, into k = number of rows).  Any k is accepted.  Routing of large k: with host
+ * outputs, k >= rows searched and more than 4 * TAV_PASS_K (8192) rows, the search is
+ * served by the threshold engine of tav_range_search (one read of the rows) and its
+ * result laid out as above; otherwise, above TAV_PASS_K rows per query, the search runs
+ * in ceil(k / TAV_PASS_K) passes over the rows.  Both give the same result.
  */
 int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float min_score,
                int flags, const int64_t* subset, int64_t subset_len, int64_t item_offset,
                int64_t* out_items, float* out_scores, int32_t* out_counts, void* stream);
+
+/* Threshold (range) search.  Every row whose score >= min_score, per query, in the library's
+ * order: score descending, then row descending (row ascending with TAV_TIES_LOW_FIRST).
+ * Writes CSR offsets out_offsets[n_queries + 1] (host, or device with TAV_OUTPUTS_ON_DEVICE):
+ * query q's hits are [out_offsets[q], out_offsets[q + 1]).  The hits stay in library-owned
+ * device memory until the next search on the index; tav_range_fetch copies them out.
+ * expected_hits is a capacity hint for the whole batch (0 = library default; the previous
+ * search's total is a good one); it never changes the result, only whether queries with more
+ * hits than their share get one more pass.  Flags: QUERIES_ON_DEVICE, OUTPUTS_ON_DEVICE,
+ * FORCE_SCAN, FORCE_MMA, USE_ROW_MASK, TIES_LOW_FIRST.  Path choice as in tav_search: batches
+ * (>= 16 queries, >= 4096 rows, no subset, dim % 8 == 0) or FORCE_MMA on the tensor cores, the row
+ * scan otherwise; a float32 value beyond the fp16 range sends the search to the row scan.  Subset
+ * and row mask as in tav_search.  NaN min_score, an empty corpus or an empty subset give all-zero
+ * offsets; NaN rows are never returned.  Synchronises once: it must learn the total before it can
+ * size the result (a tensor-core re-pass adds a second check of its counts).  TAV_ERR_OOM when
+ * the hits do not fit in device memory (the index stays usable). */
+int tav_range_search(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
+                     const int64_t* subset, int64_t subset_len, int64_t item_offset,
+                     int64_t expected_hits, int64_t* out_offsets, void* stream);
+/* Copy hits [first, first + n) of the last range search (items = row + item_offset, or the
+ * subset ordinal + item_offset; scores float32) to host or device (TAV_OUTPUTS_ON_DEVICE) memory. */
+int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items, float* out_scores,
+                    int flags, void* stream);
 
 /* Completes EVERY outstanding TAV_DEFER_RETRY search of the index: synchronises `stream`, redoes
  * each search's flagged queries exactly into that search's own outputs and reports how many

@@ -172,6 +172,12 @@ struct tav_index {
     // predicate pushdown: one bit per row (tav_set_row_mask)
     DevBuf row_mask;
     int64_t row_mask_rows = 0;   // 0 = no mask set
+    // threshold search (tav_range_search): collect regions, re-pass regions, sort scratch, CSR result
+    DevBuf range_keys, range_keys2, range_counts, range_qgather, range_tmp, range_sortws;
+    DevBuf range_mmaws, range_mmaws2, range_mmaaux;  // tensor-core collection: workspaces, scratch
+    DevBuf range_items, range_scores;
+    int64_t range_total = 0;     // hits of the last range search held in range_items / range_scores
+    cudaEvent_t ev_range = nullptr;  // end of the last range search (tav_range_fetch waits for it)
 
     // timing
     TimedSearch* hist = nullptr; // [kHistory], created by tav_set_timing(1)
@@ -289,8 +295,12 @@ int tav_destroy(tav_index* ix) {
     cudaDeviceSynchronize();  // searches may still be in flight on the caller's streams
     if (ix->rows && !ix->adopted) cudaFree(ix->rows);
     for (DevBuf* b : {&ix->queries, &ix->subset, &ix->cand_keys, &ix->cand_count, &ix->out_pack, &ix->staging,
-                      &ix->mma_ws, &ix->retry, &ix->split_hi, &ix->split_lo, &ix->split_flag, &ix->row_mask})
+                      &ix->mma_ws, &ix->retry, &ix->split_hi, &ix->split_lo, &ix->split_flag, &ix->row_mask,
+                      &ix->range_keys, &ix->range_keys2, &ix->range_counts, &ix->range_qgather, &ix->range_tmp,
+                      &ix->range_sortws, &ix->range_items, &ix->range_scores, &ix->range_mmaws,
+                      &ix->range_mmaws2, &ix->range_mmaaux})
         b->release();
+    if (ix->ev_range) cudaEventDestroy(ix->ev_range);
     ix->pin_in.release();
     ix->pin_out.release();
     ix->retry_host.release();
@@ -723,6 +733,418 @@ static int finish_pending(tav_index* ix, cudaStream_t s, int* redone) {
     return TAV_OK;
 }
 
+// ---- threshold search (tav_range_search; tav_search with k >= rows) ------------------------------------
+constexpr int64_t kRangeDefaultPerQuery = 16384;  // collect region per query when the caller gives no hint
+
+// an allocation of the threshold search: a failure leaves no sticky error behind and the index usable
+static int range_alloc(DevBuf& b, size_t bytes, const char* what) {
+    cudaError_t e = b.ensure(bytes);
+    if (e == cudaSuccess) return TAV_OK;
+    cudaGetLastError();
+    set_error("threshold search: cannot allocate %s (%zu bytes): %s", what, bytes, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? TAV_ERR_OOM : TAV_ERR_CUDA;
+}
+
+// host queries / subset -> device, shared by tav_search and the threshold search: subset ordinals through
+// pinned staging, queries float32 (normalised when the index is TAV_NORMALIZE).  `o_dev`: the call returns
+// without synchronising, so the pinned staging stays busy until the copies are done.
+static int stage_inputs(tav_index* ix, TimedSearch* ts, bool timing, const float* queries, int n_queries, bool q_dev,
+                        bool o_dev, const int64_t* subset, int64_t subset_len, const float** out_queries,
+                        const int64_t** out_subset, cudaStream_t s) {
+    const int64_t* d_subset = nullptr;
+    // subset ordinals -> device
+    if (subset) {
+        const size_t sub_bytes = static_cast<size_t>(subset_len) * sizeof(int64_t);
+        TAV_CUDA(ix->subset.ensure(sub_bytes));
+        const void* src = subset;
+        if (sub_bytes <= kPinnedStageLimit) {
+            TAV_CUDA(pin_in_acquire(ix, ((sub_bytes + 15) & ~size_t(15)) +
+                                            static_cast<size_t>(n_queries) * ix->dim * sizeof(float)));
+            memcpy(ix->pin_in.p, subset, sub_bytes);
+            src = ix->pin_in.p;
+        }
+        TAV_CUDA(cudaMemcpyAsync(ix->subset.p, src, sub_bytes, cudaMemcpyHostToDevice, s));
+        d_subset = static_cast<const int64_t*>(ix->subset.p);
+    }
+
+    if (timing) TAV_CUDA(ev_record(ts->total[0], s));
+
+    // queries -> device float32 (normalised in place when the index is TAV_NORMALIZE)
+    const float* d_queries = queries;
+    const size_t q_bytes = static_cast<size_t>(n_queries) * ix->dim * sizeof(float);
+    if (!q_dev || (ix->flags & TAV_NORMALIZE)) {
+        TAV_CUDA(ix->queries.ensure(q_bytes));
+        if (ix->flags & TAV_NORMALIZE) {
+            const void* src = queries;
+            if (!q_dev) {
+                TAV_CUDA(ix->staging.ensure(q_bytes));
+                TAV_CUDA(cudaMemcpyAsync(ix->staging.p, queries, q_bytes, cudaMemcpyHostToDevice, s));
+                src = ix->staging.p;
+            }
+            TAV_CUDA(launch_convert(src, TAV_F32, ix->queries.p, TAV_F32, n_queries, ix->dim, 1, s));
+            ts->launches += 1;
+        } else {
+            const void* src = queries;
+            cudaPointerAttributes qa{};
+            const bool q_pinned = !o_dev &&  // (device outputs: the call returns before the copy ends, staging protects the caller's buffer)
+                                  cudaPointerGetAttributes(&qa, queries) == cudaSuccess && qa.type == cudaMemoryTypeHost;
+            if (!q_pinned) cudaGetLastError();
+            if (q_bytes <= kPinnedStageLimit && !q_pinned) {
+                // via pinned staging: a pageable source would make the copy synchronous (a caller that
+                // already passes pinned memory is copied from directly)
+                const size_t sub_bytes = subset ? static_cast<size_t>(subset_len) * sizeof(int64_t) : 0;
+                const size_t sub_off = sub_bytes <= kPinnedStageLimit ? ((sub_bytes + 15) & ~size_t(15)) : 0;
+                TAV_CUDA(pin_in_acquire(ix, sub_off + q_bytes));
+                memcpy(static_cast<char*>(ix->pin_in.p) + sub_off, queries, q_bytes);
+                src = static_cast<char*>(ix->pin_in.p) + sub_off;
+            }
+            TAV_CUDA(cudaMemcpyAsync(ix->queries.p, src, q_bytes, cudaMemcpyHostToDevice, s));
+        }
+        d_queries = static_cast<const float*>(ix->queries.p);
+    }
+
+    if (o_dev && (!q_dev || subset)) {  // no synchronisation at the end of this call
+        TAV_CUDA(cudaEventRecord(ix->ev_pin_in, s));
+        ix->pin_in_busy = true;
+    }
+
+    *out_queries = d_queries;
+    *out_subset = d_subset;
+    return TAV_OK;
+}
+
+// collect-mode row scans of nq queries (device, contiguous): query q's keys -> keys + q * stride, counts[q]
+static int collect_scans(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
+                         const int64_t* d_subset, int64_t n_scan, const uint32_t* d_mask, int ties_low,
+                         uint64_t* keys, int64_t stride, uint32_t* counts, cudaStream_t s) {
+    const int qb = scan_collect_max_queries(ix->dim);  // a smaller last block takes a smaller instantiation
+    if (qb < 1) {
+        set_error("threshold search: embedding size %d too large for the row-scan kernel", ix->dim);
+        return TAV_ERR_INVALID;
+    }
+    const int grid = scan_collect_grid(ix->device, ix->dim, qb, n_scan);
+    for (int q0 = 0; q0 < nq; q0 += qb) {
+        ScanArgs a{};
+        a.corpus = ix->rows;
+        a.dtype = ix->dtype;
+        a.n_corpus = ix->size;
+        a.dim = ix->dim;
+        a.subset = d_subset;
+        a.n_scan = n_scan;
+        a.queries = d_queries + static_cast<size_t>(q0) * ix->dim;
+        a.nq = std::min(qb, nq - q0);
+        a.floor_score = floor;
+        a.cand_keys = keys + static_cast<size_t>(q0) * stride;
+        a.collect_stride = stride;
+        a.cand_count = counts + q0;
+        a.grid = grid;
+        a.row_mask = d_mask;
+        a.ties_low = ties_low;
+        const bool timed = timing && ts->used < kMaxTimedKernels;
+        if (timed) TAV_CUDA(ev_record(ts->ev[ts->used][0], s));
+        TAV_CUDA(launch_scan_collect(a, s));
+        if (timed) {
+            ts->kind[ts->used] = 0;
+            TAV_CUDA(ev_record(ts->ev[ts->used++][1], s));
+        }
+        ts->launches += 1;
+    }
+    return TAV_OK;
+}
+
+// collect region per query: the caller's hint with headroom for queries above the average, at most every row
+static int64_t range_per_query(int64_t expected_hits, int nq, int64_t n_scan) {
+    int64_t per = kRangeDefaultPerQuery;
+    if (expected_hits > 0) {
+        const int64_t m = (expected_hits + nq - 1) / nq;
+        per = m + m / 2 + 32;
+    }
+    return std::max<int64_t>(1, std::min(per, n_scan));
+}
+
+// The segmented sort of the collected keys (segs[q].keys / .n / .out set) into ix->range_items / range_scores.
+static int range_sort(tav_index* ix, TimedSearch* ts, bool timing, std::vector<SortSeg>& segs, int64_t total,
+                      const int64_t* d_subset, int64_t item_offset, int ties_low, cudaStream_t s) {
+    const int nq = static_cast<int>(segs.size());
+    std::vector<int> large, tile_seg;
+    int64_t tmp_keys = 0;
+    for (int q = 0; q < nq; ++q) {
+        SortSeg& g = segs[q];
+        g.tmp = nullptr;
+        g.tile0 = 0;
+        if (g.n > kSmallSortMax) {
+            g.tmp = reinterpret_cast<uint64_t*>(static_cast<uintptr_t>(tmp_keys));  // offset for now
+            g.tile0 = static_cast<int64_t>(tile_seg.size());
+            const int64_t nt = (g.n + kRadixTile - 1) / kRadixTile;
+            for (int64_t t = 0; t < nt; ++t) tile_seg.push_back(static_cast<int>(large.size()));
+            large.push_back(q);
+            tmp_keys += g.n;
+        }
+    }
+    if (int rc = range_alloc(ix->range_items, static_cast<size_t>(total) * sizeof(int64_t), "the hits")) return rc;
+    if (int rc = range_alloc(ix->range_scores, static_cast<size_t>(total) * sizeof(float), "the hit scores")) return rc;
+    if (total == 0) return TAV_OK;
+    if (int rc = range_alloc(ix->range_tmp, static_cast<size_t>(tmp_keys) * sizeof(uint64_t), "the sort scratch")) return rc;
+    for (SortSeg& g : segs)
+        if (g.n > kSmallSortMax)
+            g.tmp = static_cast<uint64_t*>(ix->range_tmp.p) + reinterpret_cast<uintptr_t>(g.tmp);
+    // sort workspace: segs | large | tile_seg | minmax | hist | offs
+    const size_t n_tiles = tile_seg.size();
+    const size_t b_segs = segs.size() * sizeof(SortSeg);
+    const size_t o_large = (b_segs + 15) & ~size_t(15);
+    const size_t o_tiles = (o_large + large.size() * sizeof(int) + 15) & ~size_t(15);
+    const size_t o_minmax = (o_tiles + n_tiles * sizeof(int) + 15) & ~size_t(15);
+    const size_t o_hist = o_minmax + large.size() * 2 * sizeof(uint64_t);
+    const size_t o_offs = o_hist + n_tiles * 256 * sizeof(uint32_t);
+    const size_t ws_bytes = o_offs + n_tiles * 256 * sizeof(uint32_t);
+    if (int rc = range_alloc(ix->range_sortws, ws_bytes, "the sort workspace")) return rc;
+    std::vector<char> head(o_minmax, 0);
+    memcpy(head.data(), segs.data(), b_segs);
+    if (!large.empty()) memcpy(head.data() + o_large, large.data(), large.size() * sizeof(int));
+    if (n_tiles) memcpy(head.data() + o_tiles, tile_seg.data(), n_tiles * sizeof(int));
+    char* ws = static_cast<char*>(ix->range_sortws.p);
+    // from pageable memory: the copy has consumed `head` when the call returns
+    TAV_CUDA(cudaMemcpyAsync(ws, head.data(), head.size(), cudaMemcpyHostToDevice, s));
+
+    SortArgs sa{};
+    sa.segs = reinterpret_cast<const SortSeg*>(ws);
+    sa.n_segs = nq;
+    sa.large = reinterpret_cast<const int*>(ws + o_large);
+    sa.n_large = static_cast<int>(large.size());
+    sa.tile_seg = reinterpret_cast<const int*>(ws + o_tiles);
+    sa.n_tiles = static_cast<int64_t>(n_tiles);
+    sa.minmax = reinterpret_cast<uint64_t*>(ws + o_minmax);
+    sa.hist = reinterpret_cast<uint32_t*>(ws + o_hist);
+    sa.offs = reinterpret_cast<uint32_t*>(ws + o_offs);
+    sa.subset = d_subset;
+    sa.item_offset = item_offset;
+    sa.ties_low = ties_low;
+    sa.out_items = static_cast<int64_t*>(ix->range_items.p);
+    sa.out_scores = static_cast<float*>(ix->range_scores.p);
+    const bool timed = timing && !ix->timing_light && ts->used < kMaxTimedKernels;
+    if (timed) TAV_CUDA(ev_record(ts->ev[ts->used][0], s));
+    TAV_CUDA(launch_segmented_sort(sa, s, &ts->launches));
+    if (timed) {
+        ts->kind[ts->used] = 2;
+        TAV_CUDA(ev_record(ts->ev[ts->used++][1], s));
+    }
+    return TAV_OK;
+}
+
+// Row-scan collection: one collect scan per block of queries into regions sized from `expected_hits`; the
+// counters keep counting past a region, so after the one synchronisation the totals are exact and the
+// overflowed queries get exactly one more scan into regions of that size.
+static int range_collect_scan(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
+                              const int64_t* d_subset, int64_t n_scan, int64_t item_offset, const uint32_t* d_mask,
+                              int ties_low, int64_t expected_hits, std::vector<int64_t>& offsets, cudaStream_t s) {
+    const int64_t per = range_per_query(expected_hits, nq, n_scan);
+    if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(nq) * per * sizeof(uint64_t), "the hit regions")) return rc;
+    if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(nq) * sizeof(uint32_t), "the hit counters")) return rc;
+    uint32_t* d_counts = static_cast<uint32_t*>(ix->range_counts.p);
+    uint64_t* keys = static_cast<uint64_t*>(ix->range_keys.p);
+    TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(nq) * sizeof(uint32_t), s));
+    if (int rc = collect_scans(ix, ts, timing, d_queries, nq, floor, d_subset, n_scan, d_mask, ties_low, keys, per,
+                               d_counts, s))
+        return rc;
+
+    std::vector<uint32_t> cnt(static_cast<size_t>(nq));
+    TAV_CUDA(cudaMemcpyAsync(cnt.data(), d_counts, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaStreamSynchronize(s));
+    offsets.assign(static_cast<size_t>(nq) + 1, 0);
+    std::vector<int> over;
+    int64_t over_max = 0;
+    for (int q = 0; q < nq; ++q) {
+        offsets[q + 1] = offsets[q] + cnt[q];
+        if (cnt[q] > per) {
+            over.push_back(q);
+            over_max = std::max<int64_t>(over_max, cnt[q]);
+        }
+    }
+    // overflowed queries: one more scan, gathered, into regions of their now known size
+    uint64_t* keys2 = nullptr;
+    const int no = static_cast<int>(over.size());
+    if (no > 0) {
+        const size_t qrow = static_cast<size_t>(ix->dim) * sizeof(float);
+        if (int rc = range_alloc(ix->range_keys2, static_cast<size_t>(no) * over_max * sizeof(uint64_t), "the re-pass regions"))
+            return rc;
+        if (int rc = range_alloc(ix->range_qgather, no * qrow, "the re-pass queries")) return rc;
+        keys2 = static_cast<uint64_t*>(ix->range_keys2.p);
+        char* qg = static_cast<char*>(ix->range_qgather.p);
+        for (int i = 0; i < no; ++i)
+            TAV_CUDA(cudaMemcpyAsync(qg + i * qrow, reinterpret_cast<const char*>(d_queries) + over[i] * qrow, qrow,
+                                     cudaMemcpyDeviceToDevice, s));
+        TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(no) * sizeof(uint32_t), s));
+        if (int rc = collect_scans(ix, ts, timing, reinterpret_cast<const float*>(qg), no, floor, d_subset, n_scan,
+                                   d_mask, ties_low, keys2, over_max, d_counts, s))
+            return rc;
+    }
+    std::vector<SortSeg> segs(static_cast<size_t>(nq));
+    size_t oi = 0;
+    for (int q = 0; q < nq; ++q) {
+        const bool o = oi < over.size() && over[oi] == q;
+        segs[q].keys = o ? keys2 + static_cast<size_t>(oi++) * over_max : keys + static_cast<size_t>(q) * per;
+        segs[q].out = offsets[q];
+        segs[q].n = cnt[q];
+    }
+    return range_sort(ix, ts, timing, segs, offsets[nq], d_subset, item_offset, ties_low, s);
+}
+
+constexpr int kRangeUseScan = 1;  // range_collect_mma: the tensor-core form cannot serve this search
+
+// Tensor-core collection: the MAIN kernel without a sample pass and with the exact dot floor of min_score
+// as threshold, segments sized from `expected_hits`, a count kernel; after the one synchronisation the
+// overflowed queries get one more MAIN pass (only they, same rows per segment, segments of the counted size)
+// and every query's keys are gathered in CSR order.  Returns kRangeUseScan when the float32 split form met
+// a value beyond the fp16 range (the exact row scan then serves the search, as it does for top-k searches).
+static int range_collect_mma(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
+                             int64_t item_offset, const uint32_t* d_mask, int ties_low, int64_t expected_hits,
+                             std::vector<int64_t>& offsets, cudaStream_t s) {
+    const bool split = ix->dtype == TAV_F32;
+    if (split) {
+        const int rc = ensure_split_planes(ix, ts, s);
+        if (rc == TAV_ERR_OOM) return kRangeUseScan;  // a speed choice, not a correctness one
+        if (rc != TAV_OK) return rc;
+    }
+    // scratch: [nq] retry flags (query prep clears them) | [2] split overflow flags | [nq] gather offsets
+    const size_t o_flags = (static_cast<size_t>(nq) * sizeof(int32_t) + 15) & ~size_t(15);
+    const size_t o_dst = o_flags + 16;
+    if (int rc = range_alloc(ix->range_mmaaux, o_dst + static_cast<size_t>(nq) * sizeof(int64_t), "the tensor-core scratch"))
+        return rc;
+    char* aux = static_cast<char*>(ix->range_mmaaux.p);
+    int* d_qflag = reinterpret_cast<int*>(aux + o_flags);
+    int64_t* d_dst = reinterpret_cast<int64_t*>(aux + o_dst);
+    TAV_CUDA(cudaMemsetAsync(d_qflag, 0, 16, s));
+    if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(nq) * 2 * sizeof(uint32_t), "the hit counters")) return rc;
+    uint32_t* d_tot = static_cast<uint32_t*>(ix->range_counts.p);
+    uint32_t* d_max = d_tot + nq;
+    if (timing)  // the launcher records into existing events
+        for (int i = 0; i < kMaxTimedKernels; ++i)
+            for (int j = 0; j < 2; ++j)
+                if (!ts->ev[i][j]) TAV_CUDA(cudaEventCreate(&ts->ev[i][j]));
+    MmaArgs m{};
+    m.device = ix->device;
+    m.corpus = split ? ix->split_hi.p : ix->rows;
+    m.corpus_lo = split ? ix->split_lo.p : nullptr;
+    m.split = split ? 1 : 0;
+    m.split_overflow = split ? d_qflag : nullptr;
+    m.dtype = ix->dtype;
+    m.n_corpus = ix->size;
+    m.dim = ix->dim;
+    m.queries = d_queries;
+    m.nq = nq;
+    m.floor_score = floor;
+    m.k = 1;
+    m.item_offset = item_offset;
+    m.retry_flags = reinterpret_cast<int32_t*>(aux);
+    m.row_mask = d_mask;
+    int ev_used = ts->used;
+    m.ev = timing ? ts->ev : nullptr;
+    m.ev_kind = ts->kind;
+    m.ev_max = kMaxTimedKernels;
+    m.ev_used = &ev_used;
+    const int64_t per = range_per_query(expected_hits, nq, ix->size);
+    const MmaCollect shape = mma_collect_plan(m, 0, 1);
+    // segments: twice a query's even share of its region (rows reach segments unevenly), a little more
+    const MmaCollect c = mma_collect_plan(m, shape.per_chunk, 2 * ((per + shape.n_seg - 1) / shape.n_seg) + 8);
+    if (int rc = range_alloc(ix->range_mmaws, c.ws_bytes, "the tensor-core workspace")) return rc;
+    TAV_CUDA(launch_mma_collect(m, c, ix->range_mmaws.p, d_tot, d_max, s, &ts->launches));
+    ts->used = ev_used;
+
+    std::vector<uint32_t> host(2 * static_cast<size_t>(nq));
+    int flags[2] = {0, 0};
+    TAV_CUDA(cudaMemcpyAsync(host.data(), d_tot, host.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    if (split) {
+        TAV_CUDA(cudaMemcpyAsync(&flags[0], d_qflag, sizeof(int), cudaMemcpyDeviceToHost, s));
+        TAV_CUDA(cudaMemcpyAsync(&flags[1], ix->split_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+    }
+    TAV_CUDA(cudaStreamSynchronize(s));
+    if (flags[0] || flags[1]) return kRangeUseScan;
+    offsets.assign(static_cast<size_t>(nq) + 1, 0);
+    std::vector<int> over;
+    std::vector<int64_t> dst(static_cast<size_t>(nq));
+    uint32_t over_seg = 0;
+    for (int q = 0; q < nq; ++q) {
+        offsets[q + 1] = offsets[q] + host[q];
+        dst[q] = offsets[q];
+        if (host[nq + q] > c.cap_seg) {
+            over.push_back(q);
+            over_seg = std::max(over_seg, host[nq + q]);
+            dst[q] = -1;
+        }
+    }
+    const int64_t total = offsets[nq];
+    if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(total) * sizeof(uint64_t), "the hit keys")) return rc;
+    uint64_t* keys = static_cast<uint64_t*>(ix->range_keys.p);
+    TAV_CUDA(cudaMemcpyAsync(d_dst, dst.data(), dst.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    TAV_CUDA(launch_mma_gather(m, c, ix->range_mmaws.p, d_dst, keys, ties_low, s));
+    ts->launches += 1;
+
+    const int no = static_cast<int>(over.size());
+    if (no > 0) {
+        // the overflowed queries, gathered, through the same units per chunk: every segment receives the
+        // rows it received before, and the counts just read size it exactly
+        const size_t qrow = static_cast<size_t>(ix->dim) * sizeof(float);
+        if (int rc = range_alloc(ix->range_qgather, no * qrow, "the re-pass queries")) return rc;
+        char* qg = static_cast<char*>(ix->range_qgather.p);
+        for (int i = 0; i < no; ++i)
+            TAV_CUDA(cudaMemcpyAsync(qg + i * qrow, reinterpret_cast<const char*>(d_queries) + over[i] * qrow, qrow,
+                                     cudaMemcpyDeviceToDevice, s));
+        MmaArgs m2 = m;
+        m2.queries = reinterpret_cast<const float*>(qg);
+        m2.nq = no;
+        const MmaCollect c2 = mma_collect_plan(m2, c.per_chunk, over_seg);
+        if (c2.n_seg != c.n_seg || c2.cap_seg < over_seg) {
+            set_error("threshold search: tensor-core re-pass plan mismatch");
+            return TAV_ERR_CUDA;
+        }
+        if (int rc = range_alloc(ix->range_mmaws2, c2.ws_bytes, "the tensor-core re-pass workspace")) return rc;
+        ev_used = ts->used;
+        TAV_CUDA(launch_mma_collect(m2, c2, ix->range_mmaws2.p, d_tot, d_max, s, &ts->launches));
+        ts->used = ev_used;
+        // the re-pass must admit exactly the rows the first pass counted (a second look at its counts)
+        std::vector<uint32_t> host2(2 * static_cast<size_t>(no));
+        TAV_CUDA(cudaMemcpyAsync(host2.data(), d_tot, no * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        TAV_CUDA(cudaMemcpyAsync(host2.data() + no, d_max, no * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        TAV_CUDA(cudaStreamSynchronize(s));
+        for (int i = 0; i < no; ++i)
+            if (host2[i] != host[over[i]] || host2[no + i] > c2.cap_seg) return kRangeUseScan;
+        std::vector<int64_t> dst2(static_cast<size_t>(no));
+        for (int i = 0; i < no; ++i) dst2[i] = offsets[over[i]];
+        TAV_CUDA(cudaMemcpyAsync(d_dst, dst2.data(), dst2.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+        TAV_CUDA(launch_mma_gather(m2, c2, ix->range_mmaws2.p, d_dst, keys, ties_low, s));
+        ts->launches += 1;
+    }
+    std::vector<SortSeg> segs(static_cast<size_t>(nq));
+    for (int q = 0; q < nq; ++q) {
+        segs[q].keys = keys + offsets[q];
+        segs[q].out = offsets[q];
+        segs[q].n = host[q];
+    }
+    return range_sort(ix, ts, timing, segs, total, nullptr, item_offset, ties_low, s);
+}
+
+// Every row with score >= floor, for each of nq device queries -> ix->range_items / range_scores in CSR order
+// (offsets[nq + 1], host): collected by the tensor cores (use_mma) or the row scan, then the segmented sort.
+static int range_core(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
+                      const int64_t* d_subset, int64_t n_scan, int64_t item_offset, const uint32_t* d_mask,
+                      int ties_low, int64_t expected_hits, bool use_mma, std::vector<int64_t>& offsets, cudaStream_t s) {
+    if (use_mma) {
+        const int rc = range_collect_mma(ix, ts, timing, d_queries, nq, floor, item_offset, d_mask, ties_low,
+                                         expected_hits, offsets, s);
+        if (rc != kRangeUseScan) return rc;
+        ts->path = 1;  // a value beyond the fp16 range: the exact row scan serves the search
+    }
+    return range_collect_scan(ix, ts, timing, d_queries, nq, floor, d_subset, n_scan, item_offset, d_mask, ties_low,
+                              expected_hits, offsets, s);
+}
+
+// the hits of the last threshold search are complete once this event has passed (tav_range_fetch waits)
+static int range_mark_end(tav_index* ix, cudaStream_t s) {
+    if (!ix->ev_range) TAV_CUDA(cudaEventCreateWithFlags(&ix->ev_range, cudaEventDisableTiming));
+    TAV_CUDA(cudaEventRecord(ix->ev_range, s));
+    return TAV_OK;
+}
+
 extern "C" {
 
 const int32_t* tav_internal_retry_totals(tav_index* ix, int* count) {
@@ -784,19 +1206,6 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     // Small result sets are written by the kernels straight into the pinned host staging (zero
     // copy over PCIe: no D2H memcpy call on the single-lookup latency path).
     const bool zero_copy_out = !o_dev && pack_bytes <= kZeroCopyOutLimit;
-    if (zero_copy_out) {
-        TAV_CUDA(ix->pin_out.ensure(pack_bytes));
-        char* base = static_cast<char*>(ix->pin_out.p);
-        d_items = reinterpret_cast<int64_t*>(base);
-        d_scores = reinterpret_cast<float*>(base + off_scores);
-        d_counts = reinterpret_cast<int32_t*>(base + off_counts);
-    } else if (!o_dev) {
-        TAV_CUDA(ix->out_pack.ensure(pack_bytes));
-        char* base = static_cast<char*>(ix->out_pack.p);
-        d_items = reinterpret_cast<int64_t*>(base);
-        d_scores = reinterpret_cast<float*>(base + off_scores);
-        d_counts = reinterpret_cast<int32_t*>(base + off_counts);
-    }
 
     const int64_t n_scan = subset ? subset_len : ix->size;
     ix->last_first_slot = -1;
@@ -842,6 +1251,66 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     if ((flags & TAV_FORCE_MMA) && !use_mma) {
         set_error("tav_search: TAV_FORCE_MMA needs dim %% 8 == 0, no subset, k <= %d", kPassK);
         return TAV_ERR_INVALID;
+    }
+
+    // ---- every passing row of a large scan (k >= rows; the reference's max_hits = 0) ------------------
+    // The threshold engine (collect scan + segmented sort) reads the rows once where the paged form would
+    // run ceil(k / kPassK) passes; same kernels' dots and the same key order, so the same result, which is
+    // then laid out as [n_queries, k] with -1 / 0 padding.  Regions of n_scan keys per query: no re-pass.
+    if (!use_mma && !o_dev && k >= n_scan && n_scan > 4 * kPassK) {
+        ts->path = 1;
+        const float* d_q = nullptr;
+        const int64_t* d_sub = nullptr;
+        if (int rc = stage_inputs(ix, ts, timing, queries, n_queries, q_dev, false, subset, subset_len, &d_q, &d_sub, s))
+            return rc;
+        std::vector<int64_t> offsets;
+        ix->range_total = 0;
+        if (int rc = range_core(ix, ts, timing, d_q, n_queries, min_score, d_sub, n_scan, item_offset, d_mask, ties_low,
+                                static_cast<int64_t>(n_queries) * n_scan, false, offsets, s))
+            return rc;
+        if (timing) {
+            TAV_CUDA(ev_record(ts->total[1], s));
+            ++ix->search_seq;
+        }
+        ts->valid = true;
+        ix->range_total = offsets[n_queries];
+        if (int rc = range_mark_end(ix, s)) return rc;
+        // each query's hits straight into its row of the caller's arrays (copies from device memory into
+        // pageable memory return when done), then the padding
+        for (int q = 0; q < n_queries; ++q) {
+            const int64_t c = offsets[q + 1] - offsets[q];
+            int64_t* it = out_items + static_cast<size_t>(q) * k;
+            float* sc = out_scores + static_cast<size_t>(q) * k;
+            if (c > 0) {
+                TAV_CUDA(cudaMemcpyAsync(it, static_cast<const int64_t*>(ix->range_items.p) + offsets[q],
+                                         static_cast<size_t>(c) * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+                TAV_CUDA(cudaMemcpyAsync(sc, static_cast<const float*>(ix->range_scores.p) + offsets[q],
+                                         static_cast<size_t>(c) * sizeof(float), cudaMemcpyDeviceToHost, s));
+            }
+        }
+        TAV_CUDA(cudaStreamSynchronize(s));
+        for (int q = 0; q < n_queries; ++q) {
+            const int64_t c = offsets[q + 1] - offsets[q];
+            std::fill(out_items + static_cast<size_t>(q) * k + c, out_items + static_cast<size_t>(q + 1) * k, int64_t(-1));
+            std::fill(out_scores + static_cast<size_t>(q) * k + c, out_scores + static_cast<size_t>(q + 1) * k, 0.0f);
+            out_counts[q] = static_cast<int32_t>(c);
+        }
+        return TAV_OK;
+    }
+
+    // result staging for host outputs (after the routing above, which needs none)
+    if (zero_copy_out) {
+        TAV_CUDA(ix->pin_out.ensure(pack_bytes));
+        char* base = static_cast<char*>(ix->pin_out.p);
+        d_items = reinterpret_cast<int64_t*>(base);
+        d_scores = reinterpret_cast<float*>(base + off_scores);
+        d_counts = reinterpret_cast<int32_t*>(base + off_counts);
+    } else if (!o_dev) {
+        TAV_CUDA(ix->out_pack.ensure(pack_bytes));
+        char* base = static_cast<char*>(ix->out_pack.p);
+        d_items = reinterpret_cast<int64_t*>(base);
+        d_scores = reinterpret_cast<float*>(base + off_scores);
+        d_counts = reinterpret_cast<int32_t*>(base + off_counts);
     }
 
     // ---- single-lookup latency form: ONE launch, no copies -------------------------------------
@@ -971,62 +1440,10 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         return TAV_OK;
     }
 
-    // subset ordinals -> device
     const int64_t* d_subset = nullptr;
-    if (subset) {
-        const size_t sub_bytes = static_cast<size_t>(subset_len) * sizeof(int64_t);
-        TAV_CUDA(ix->subset.ensure(sub_bytes));
-        const void* src = subset;
-        if (sub_bytes <= kPinnedStageLimit) {
-            TAV_CUDA(pin_in_acquire(ix, ((sub_bytes + 15) & ~size_t(15)) +
-                                            static_cast<size_t>(n_queries) * ix->dim * sizeof(float)));
-            memcpy(ix->pin_in.p, subset, sub_bytes);
-            src = ix->pin_in.p;
-        }
-        TAV_CUDA(cudaMemcpyAsync(ix->subset.p, src, sub_bytes, cudaMemcpyHostToDevice, s));
-        d_subset = static_cast<const int64_t*>(ix->subset.p);
-    }
-
-    if (timing) TAV_CUDA(ev_record(ts->total[0], s));
-
-    // queries -> device float32 (normalised in place when the index is TAV_NORMALIZE)
-    const float* d_queries = queries;
-    const size_t q_bytes = static_cast<size_t>(n_queries) * ix->dim * sizeof(float);
-    if (!q_dev || (ix->flags & TAV_NORMALIZE)) {
-        TAV_CUDA(ix->queries.ensure(q_bytes));
-        if (ix->flags & TAV_NORMALIZE) {
-            const void* src = queries;
-            if (!q_dev) {
-                TAV_CUDA(ix->staging.ensure(q_bytes));
-                TAV_CUDA(cudaMemcpyAsync(ix->staging.p, queries, q_bytes, cudaMemcpyHostToDevice, s));
-                src = ix->staging.p;
-            }
-            TAV_CUDA(launch_convert(src, TAV_F32, ix->queries.p, TAV_F32, n_queries, ix->dim, 1, s));
-            ts->launches += 1;
-        } else {
-            const void* src = queries;
-            cudaPointerAttributes qa{};
-            const bool q_pinned = !o_dev &&  // (device outputs: the call returns before the copy ends, staging protects the caller's buffer)
-                                  cudaPointerGetAttributes(&qa, queries) == cudaSuccess && qa.type == cudaMemoryTypeHost;
-            if (!q_pinned) cudaGetLastError();
-            if (q_bytes <= kPinnedStageLimit && !q_pinned) {
-                // via pinned staging: a pageable source would make the copy synchronous (a caller that
-                // already passes pinned memory is copied from directly)
-                const size_t sub_bytes = subset ? static_cast<size_t>(subset_len) * sizeof(int64_t) : 0;
-                const size_t sub_off = sub_bytes <= kPinnedStageLimit ? ((sub_bytes + 15) & ~size_t(15)) : 0;
-                TAV_CUDA(pin_in_acquire(ix, sub_off + q_bytes));
-                memcpy(static_cast<char*>(ix->pin_in.p) + sub_off, queries, q_bytes);
-                src = static_cast<char*>(ix->pin_in.p) + sub_off;
-            }
-            TAV_CUDA(cudaMemcpyAsync(ix->queries.p, src, q_bytes, cudaMemcpyHostToDevice, s));
-        }
-        d_queries = static_cast<const float*>(ix->queries.p);
-    }
-
-    if (o_dev && (!q_dev || subset)) {  // no synchronisation at the end of this call
-        TAV_CUDA(cudaEventRecord(ix->ev_pin_in, s));
-        ix->pin_in_busy = true;
-    }
+    const float* d_queries = nullptr;
+    if (int rc = stage_inputs(ix, ts, timing, queries, n_queries, q_dev, o_dev, subset, subset_len, &d_queries, &d_subset, s))
+        return rc;
 
     if (use_split) {
         const int rc = ensure_split_planes(ix, ts, s);
@@ -1153,6 +1570,121 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             TAV_CUDA(cudaStreamSynchronize(s));
         }
     }
+    return TAV_OK;
+}
+
+int tav_range_search(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
+                     const int64_t* subset, int64_t subset_len, int64_t item_offset, int64_t expected_hits,
+                     int64_t* out_offsets, void* stream) {
+    if (!ix || n_queries < 0 || expected_hits < 0 || !out_offsets || (n_queries > 0 && !queries)) {
+        set_error("tav_range_search: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    if ((subset && subset_len < 0) || (!subset && subset_len != 0)) {
+        set_error("tav_range_search: subset / subset_len mismatch");
+        return TAV_ERR_INVALID;
+    }
+    if (flags & TAV_DEFER_RETRY) {
+        set_error("tav_range_search: TAV_DEFER_RETRY is not available for threshold searches");
+        return TAV_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (int rc = set_device(ix)) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
+    ix->range_total = 0;
+    std::vector<int64_t> offsets(static_cast<size_t>(n_queries) + 1, 0);
+    auto write_offsets = [&]() -> int {
+        const size_t bytes = offsets.size() * sizeof(int64_t);
+        if (o_dev) {  // from pageable memory: consumed when the call returns
+            TAV_CUDA(cudaMemcpyAsync(out_offsets, offsets.data(), bytes, cudaMemcpyHostToDevice, s));
+        } else {
+            memcpy(out_offsets, offsets.data(), bytes);
+        }
+        return range_mark_end(ix, s);
+    };
+    const uint32_t* d_mask = nullptr;
+    if (flags & TAV_USE_ROW_MASK) {
+        if (ix->row_mask_rows != ix->size || ix->size == 0) {
+            set_error("tav_range_search: TAV_USE_ROW_MASK without a current row mask (tav_set_row_mask)");
+            return TAV_ERR_STATE;
+        }
+        if (subset) {
+            set_error("tav_range_search: a row mask and a subset cannot be combined");
+            return TAV_ERR_INVALID;
+        }
+        d_mask = static_cast<const uint32_t*>(ix->row_mask.p);
+    }
+    const int64_t n_scan = subset ? subset_len : ix->size;
+    // NaN min_score, empty corpus or empty subset: no hits
+    if (n_queries == 0 || n_scan == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score) return write_offsets();
+    if (n_scan > 0xFFFFFFFFll) {
+        set_error("tav_range_search: more than 2^32 rows per index are not supported; shard the corpus");
+        return TAV_ERR_INVALID;
+    }
+    if (subset) {
+        for (int64_t i = 0; i < subset_len; ++i) {
+            if (subset[i] < -ix->size || subset[i] >= ix->size) {
+                set_error("index %lld is out of bounds for axis 0 with size %lld", (long long)subset[i],
+                          (long long)ix->size);
+                return TAV_ERR_RANGE;
+            }
+        }
+    }
+    // path choice as in tav_search: tensor cores for batches (no subset), the row scan otherwise
+    const bool mma_able = (mma_supported(ix->dtype, ix->dim) || (ix->dtype == TAV_F32 && mma_split_supported(ix->dim))) &&
+                          !subset && n_queries <= kMmaMaxQueries && ix->size < (1ll << 31);
+    const bool use_mma = !(flags & TAV_FORCE_SCAN) && mma_able &&
+                         ((flags & TAV_FORCE_MMA) || (n_queries >= 16 && ix->size >= 4096));
+    if ((flags & TAV_FORCE_MMA) && !use_mma) {
+        set_error("tav_range_search: TAV_FORCE_MMA needs dim %% 8 == 0, no subset, at most %d queries", kMmaMaxQueries);
+        return TAV_ERR_INVALID;
+    }
+    TimedSearch* ts = cur_timed(ix);
+    if (!ts) ts = &ix->untimed;
+    const bool timing = ts != &ix->untimed;
+    ts->used = 0;
+    ts->launches = 0;
+    ts->path = use_mma ? (ix->dtype == TAV_F32 ? 3 : 2) : 1;
+    ts->valid = false;
+    const float* d_queries = nullptr;
+    const int64_t* d_subset = nullptr;
+    if (int rc = stage_inputs(ix, ts, timing, queries, n_queries, q_dev, false, subset, subset_len, &d_queries, &d_subset, s))
+        return rc;
+    if (int rc = range_core(ix, ts, timing, d_queries, n_queries, min_score, d_subset, n_scan, item_offset, d_mask,
+                            (flags & TAV_TIES_LOW_FIRST) ? 1 : 0, expected_hits, use_mma, offsets, s))
+        return rc;
+    if (timing) {
+        TAV_CUDA(ev_record(ts->total[1], s));
+        ++ix->search_seq;
+    }
+    ts->valid = true;
+    ix->range_total = offsets[n_queries];
+    return write_offsets();
+}
+
+int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items, float* out_scores, int flags,
+                    void* stream) {
+    if (!ix || first < 0 || n < 0 || (n > 0 && (!out_items || !out_scores))) {
+        set_error("tav_range_fetch: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (first + n > ix->range_total) {
+        set_error("tav_range_fetch: hits [%lld, %lld) out of range (the last range search has %lld)", (long long)first,
+                  (long long)(first + n), (long long)ix->range_total);
+        return TAV_ERR_RANGE;
+    }
+    if (n == 0) return TAV_OK;
+    if (int rc = set_device(ix)) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (ix->ev_range) TAV_CUDA(cudaStreamWaitEvent(s, ix->ev_range, 0));
+    const cudaMemcpyKind kind = (flags & TAV_OUTPUTS_ON_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    TAV_CUDA(cudaMemcpyAsync(out_items, static_cast<const int64_t*>(ix->range_items.p) + first,
+                             static_cast<size_t>(n) * sizeof(int64_t), kind, s));
+    TAV_CUDA(cudaMemcpyAsync(out_scores, static_cast<const float*>(ix->range_scores.p) + first,
+                             static_cast<size_t>(n) * sizeof(float), kind, s));
+    if (!(flags & TAV_OUTPUTS_ON_DEVICE)) TAV_CUDA(cudaStreamSynchronize(s));
     return TAV_OK;
 }
 

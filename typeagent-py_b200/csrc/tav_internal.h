@@ -40,6 +40,9 @@ struct ScanArgs {
     uint32_t* done_flag;      // mapped pinned host word set to done_seq once the hits are written, or nullptr
     uint32_t done_seq;
     unsigned long long* trace;  // diagnostic (TAV_TRACE=1): %globaltimer stamps of the single-launch form's phases
+    // collect mode (launch_scan_collect): query q's keys go to cand_keys + q * collect_stride; cand_count[q]
+    // (zero on entry) counts every admitted row, also those beyond collect_stride, which are not stored
+    int64_t collect_stride;
 };
 constexpr int kFusedSelectMax = 8192;   // survivors the last CTA of the single-launch form can merge
 constexpr int kFusedSelOut = 1024;      // ... of which it sorts at most this many after the histogram selection
@@ -54,6 +57,41 @@ cudaError_t launch_scan1(const ScanArgs& a, const float* q_host, const int64_t* 
 int scan_max_queries(int dim, int k);            // how many queries one pass can take (smem)
 int scan_grid(int device, int dtype, int dim, int nq, int k, int64_t n_scan);
 cudaError_t launch_scan(const ScanArgs& a, cudaStream_t s);
+int scan_collect_max_queries(int dim);          // queries one collect-mode pass can take (1/2/4/8)
+int scan_collect_grid(int device, int dim, int nq, int64_t n_scan);
+cudaError_t launch_scan_collect(const ScanArgs& a, cudaStream_t s);
+
+// ---- segmented sort of the threshold search's keys (tav_sort.cu) -----------------------
+// One segment per query: n keys (unsorted, unique) at `keys`; sorted descending and decoded into
+// out_items / out_scores [out, out + n).  Segments above kSmallSortMax keys also need `tmp` (n keys of
+// scratch) and their radix tiles [tile0, tile0 + ceil(n / kRadixTile)).
+struct SortSeg {
+    uint64_t* keys;
+    uint64_t* tmp;
+    int64_t out;
+    int64_t n;
+    int64_t tile0;
+};
+constexpr int kSmallSortMax = 4096;  // keys one CTA sorts in shared memory
+constexpr int kRadixTile = 8192;     // keys per CTA in a radix pass
+struct SortArgs {
+    const SortSeg* segs;      // device [n_segs]: every query
+    int n_segs;
+    const int* large;         // device [n_large]: indexes of the segments above kSmallSortMax
+    int n_large;
+    const int* tile_seg;      // device [n_tiles]: large segment (index into `large`) of every radix tile
+    int64_t n_tiles;
+    uint64_t* minmax;         // device [2 * n_large] scratch
+    uint32_t* hist;           // device [n_tiles * 256] scratch
+    uint32_t* offs;           // device [n_tiles * 256] scratch
+    const int64_t* subset;    // item = subset[pos] (or pos) + item_offset
+    int64_t item_offset;
+    int ties_low;
+    int64_t* out_items;
+    float* out_scores;
+};
+// returns the number of kernels launched in *launches
+cudaError_t launch_segmented_sort(const SortArgs& a, cudaStream_t s, int* launches);
 
 struct SelectArgs {
     const uint64_t* cand_keys;   // [nq, cand_stride]
@@ -130,6 +168,25 @@ constexpr int kMmaMaxQueries = 32768;  // queries per launch_mma_search call (25
 size_t mma_workspace_bytes(const MmaArgs& a);
 cudaError_t launch_mma_search(const MmaArgs& a, void* workspace, size_t workspace_bytes,
                               cudaStream_t s, int* launches);
+// Threshold search on the tensor cores (tav_range_search): the MAIN kernel without a sample pass, admission
+// threshold = the exact dot floor of min_score, so every row whose score passes lands in one of the query's
+// n_seg private segments of cap_seg keys (counts keep counting past cap_seg).  Needs a.retry_flags [nq]
+// (scratch) and, split, a.split_overflow [2]; a.k is unused.
+struct MmaCollect {
+    int per_chunk = 0;    // units per query chunk (fixes which rows feed which segment)
+    int n_seg = 0;        // segments per query
+    uint32_t cap_seg = 0; // keys a segment holds
+    size_t ws_bytes = 0;  // workspace of this plan
+};
+// per_chunk 0: the plan's own; cap_seg is clamped to what a segment can see
+MmaCollect mma_collect_plan(const MmaArgs& a, int per_chunk, int64_t cap_seg);
+// query prep + MAIN + a count kernel: totals[q] = rows admitted, maxseg[q] = fullest segment (> cap_seg:
+// overflowed, its keys incomplete).  With a.ev / a.ev_used: one event pair (kind 0) around MAIN.
+cudaError_t launch_mma_collect(const MmaArgs& a, const MmaCollect& c, void* workspace, uint32_t* totals,
+                               uint32_t* maxseg, cudaStream_t s, int* launches);
+// the keys of every query with dst_off[q] >= 0 (device [nq]), as library keys, to dst + dst_off[q]
+cudaError_t launch_mma_gather(const MmaArgs& a, const MmaCollect& c, void* workspace, const int64_t* dst_off,
+                              uint64_t* dst, int ties_low, cudaStream_t s);
 // verification aid: every raw dot product of the tensor-core path, out[nq, n_corpus] on the device
 cudaError_t launch_mma_dump(const MmaArgs& a, void* workspace, size_t workspace_bytes, float* out,
                             cudaStream_t s);

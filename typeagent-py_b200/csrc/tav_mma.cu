@@ -674,6 +674,69 @@ finalize_kernel(const uint64_t* cand, const uint32_t* cand_count, int n_seg, uin
     if (tid == 0) out_counts[q] = n;
 }
 
+// ---- threshold search (collect plan): per-query totals, then the keys of every segment in CSR order ------
+// one warp per query: total admitted rows and the fullest segment (> cap_seg: the query overflowed)
+__global__ void collect_count_kernel(const uint32_t* cand_count, int n_seg, int nq, uint32_t* totals, uint32_t* maxseg) {
+    const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (q >= nq) return;
+    uint32_t sum = 0, mx = 0;
+    for (int sgm = lane; sgm < n_seg; sgm += 32) {
+        const uint32_t c = cand_count[static_cast<size_t>(q) * n_seg + sgm];
+        sum += c;
+        mx = max(mx, c);
+    }
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) {
+        sum += __shfl_xor_sync(0xFFFFFFFFu, sum, off);
+        mx = max(mx, __shfl_xor_sync(0xFFFFFFFFu, mx, off));
+    }
+    if (lane == 0) {
+        totals[q] = sum;
+        maxseg[q] = mx;
+    }
+}
+
+// one CTA per query with dst_off[q] >= 0: its (dot bits << 32 | row) candidates -> library keys
+// (score bits << 32 | row, ~row with ties_low) at dst + dst_off[q], segment after segment
+__global__ void __launch_bounds__(kSelectThreads)
+collect_gather_kernel(const uint64_t* cand, const uint32_t* cand_count, int n_seg, uint32_t cap_seg,
+                      const int64_t* dst_off, uint64_t* dst, int ties_low) {
+    __shared__ uint32_t s_prefix[kMaxSegments + 1];
+    const int q = blockIdx.x, tid = threadIdx.x;
+    const int64_t base = dst_off[q];
+    if (base < 0) return;
+    const uint32_t* counts = cand_count + static_cast<size_t>(q) * n_seg;
+    if (tid < 32) {  // exclusive scan of the segment counts by one warp
+        uint32_t carry = 0;
+        for (int b0 = 0; b0 < n_seg; b0 += 32) {
+            const int i = b0 + tid;
+            const uint32_t c = i < n_seg ? min(counts[i], cap_seg) : 0u;
+            uint32_t v = c;
+#pragma unroll
+            for (int off = 1; off < 32; off <<= 1) {
+                const uint32_t o = __shfl_up_sync(0xFFFFFFFFu, v, off);
+                if (tid >= off) v += o;
+            }
+            if (i < n_seg) s_prefix[i] = carry + v - c;
+            carry += __shfl_sync(0xFFFFFFFFu, v, 31);
+        }
+        if (tid == 0) s_prefix[n_seg] = carry;
+    }
+    __syncthreads();
+    const uint64_t* in = cand + static_cast<size_t>(q) * n_seg * cap_seg;
+    const int warp = tid >> 5, lane = tid & 31;
+    for (int sgm = warp; sgm < n_seg; sgm += kSelectThreads / 32) {  // a warp per segment, coalesced
+        const uint32_t n = s_prefix[sgm + 1] - s_prefix[sgm];
+        const uint64_t* src = in + static_cast<size_t>(sgm) * cap_seg;
+        uint64_t* out = dst + base + s_prefix[sgm];
+        for (uint32_t i = lane; i < n; i += 32) {
+            const uint64_t e = src[i];
+            const uint32_t row = static_cast<uint32_t>(e);
+            out[i] = make_key(score_from_dot(__uint_as_float(static_cast<uint32_t>(e >> 32))), ties_low ? ~row : row);
+        }
+    }
+}
+
 // ---- host side --------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -726,7 +789,12 @@ struct Plan {
     size_t off_q, off_q_lo, off_sample, off_thr, off_floor, off_count, off_done, off_cand, total;
 };
 
-Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split) {
+// collect_cap >= 0: the threshold search's collect plan (tav_range_search): no sample pass, segments of
+// collect_cap keys (at most what a segment can see), `force_per_chunk` units per query chunk when > 0 (a
+// re-pass must split the rows into the same segments as its first pass), candidates of padded queries not
+// stored (they admit nothing)
+Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split, int force_per_chunk = 0,
+               int64_t collect_cap = -1) {
     Plan p{};
     p.sms = 132;
     cudaDeviceGetAttribute(&p.sms, cudaDevAttrMultiProcessorCount, device);
@@ -757,7 +825,7 @@ Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split) {
                                : std::max<int64_t>(16ll * k, std::min<int64_t>(2048, std::max<int64_t>(128, n_rows / 4096)));
     int64_t admitted = n_rows;  // rows a query is expected to admit
     const int64_t per_tile = static_cast<int64_t>(p.tile_n / 128);  // 128-row spans per tile (x sample_gph blocks)
-    if (n_rows <= 16384 || 8 * target >= n_rows || p.n_full_tiles < 8) {
+    if (collect_cap >= 0 || n_rows <= 16384 || 8 * target >= n_rows || p.n_full_tiles < 8) {
         p.n_sample = 0;
     } else {
         // Block size: the m-th largest of L block maxima sits at the row quantile p when 1 - (1-p)^b = m / L;
@@ -786,7 +854,7 @@ Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split) {
         // every unit of a chunk owns four candidate segments per query (one per thread of the quad that
         // holds the query): room for 16x the expected share of a segment (at least half a tile's share),
         // and for every row it can see when nothing is cut
-        const int per_chunk = std::max(
+        const int per_chunk = force_per_chunk > 0 ? force_per_chunk : std::max(
             1, std::min(std::min(std::max(1, max_units / p.nqc), p.n_tiles), kMaxSegments / kSegPerUnit));
         p.main_units = per_chunk * p.nqc;
         p.n_seg = kSegPerUnit * per_chunk;
@@ -794,6 +862,7 @@ Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split) {
         const int64_t seen = tiles_per_unit * (p.tile_n / kSegPerUnit);
         const int64_t want = p.n_sample == 0 ? seen : std::max<int64_t>(p.tile_n / (2 * kSegPerUnit), (16 * admitted + p.n_seg - 1) / p.n_seg);
         p.cap_seg = static_cast<uint32_t>(std::min<int64_t>(want, seen));
+        if (collect_cap >= 0) p.cap_seg = static_cast<uint32_t>(std::max<int64_t>(1, std::min<int64_t>(collect_cap, seen)));
     }
     auto align = [](size_t v) { return (v + 255) & ~size_t(255); };
     // the sampler's self-resetting unit counters live at a FIXED place (offset 0), whatever the shape of
@@ -815,7 +884,7 @@ Plan make_plan(int device, int64_t n_rows, int dim, int nq, int k, bool split) {
     p.off_count = off;
     off = align(off + static_cast<size_t>(p.nq_pad) * p.n_seg * sizeof(uint32_t));
     p.off_cand = off;
-    off = align(off + static_cast<size_t>(p.nq_pad) * p.n_seg * p.cap_seg * sizeof(uint64_t));
+    off = align(off + static_cast<size_t>(collect_cap >= 0 ? nq : p.nq_pad) * p.n_seg * p.cap_seg * sizeof(uint64_t));
     p.total = off;
     return p;
 }
@@ -1043,6 +1112,72 @@ cudaError_t launch_mma_search(const MmaArgs& a, void* workspace, size_t workspac
     if (launches) *launches = n_launch;
     if (a.ev_used) *a.ev_used = ev_used;
     return cudaSuccess;
+}
+
+MmaCollect mma_collect_plan(const MmaArgs& a, int per_chunk, int64_t cap_seg) {
+    const Plan p = make_plan(a.device, a.n_corpus, a.dim, a.nq, 1, a.split != 0, per_chunk, std::max<int64_t>(cap_seg, 1));
+    MmaCollect c;
+    c.per_chunk = p.n_seg / kSegPerUnit;
+    c.n_seg = p.n_seg;
+    c.cap_seg = p.cap_seg;
+    c.ws_bytes = p.total;
+    return c;
+}
+
+cudaError_t launch_mma_collect(const MmaArgs& a, const MmaCollect& c, void* workspace, uint32_t* totals,
+                               uint32_t* maxseg, cudaStream_t s, int* launches) {
+    if (!args_ok(a) || a.nq < 1 || a.nq > kMmaMaxQueries || !a.retry_flags) return cudaErrorInvalidValue;
+    const Plan p = make_plan(a.device, a.n_corpus, a.dim, a.nq, 1, a.split != 0, c.per_chunk, c.cap_seg);
+    if (p.n_seg != c.n_seg || p.cap_seg != c.cap_seg) return cudaErrorInvalidValue;
+    char* ws = static_cast<char*>(workspace);
+    void* d_q = ws + p.off_q;
+    void* d_q_lo = ws + p.off_q_lo;
+    float* d_thr = reinterpret_cast<float*>(ws + p.off_thr);
+    float* d_floor = reinterpret_cast<float*>(ws + p.off_floor);
+    uint32_t* d_count = reinterpret_cast<uint32_t*>(ws + p.off_count);
+    Maps maps;
+    if (!build_maps(a, d_q, d_q_lo, p.nq_pad, maps)) return cudaErrorUnknown;
+    // queries -> storage dtype, thresholds = the exact dot floor of min_score (no sample pass)
+    cudaError_t e = prep_queries(a, d_q, d_q_lo, p.nq_pad, 1, d_thr, d_floor, s);
+    if (e != cudaSuccess) return e;
+    KernelArgs ka{};
+    ka.n_rows = a.n_corpus;
+    ka.kb_count = p.kb_count;
+    ka.nq = a.nq;
+    ka.nqc = p.nqc;
+    ka.nq_pad = p.nq_pad;
+    ka.thr = d_thr;
+    ka.floor_x = d_floor;
+    ka.cand = reinterpret_cast<uint64_t*>(ws + p.off_cand);
+    ka.cand_count = d_count;
+    ka.cap_seg = p.cap_seg;
+    ka.n_seg = p.n_seg;
+    ka.row_mask = a.row_mask;
+    ka.n_tiles_work = p.n_tiles;
+    ka.tile_mul = 1;
+    ka.tile_div = 1;
+    const bool timed = a.ev && a.ev_used && *a.ev_used < a.ev_max;
+    if (timed && (e = cudaEventRecord(a.ev[*a.ev_used][0], s)) != cudaSuccess) return e;
+    e = launch_kernel<kMain>(maps, ka, mma_dtype(a), a.split != 0, p.main_units, s);
+    if (e != cudaSuccess) return e;
+    if (timed) {
+        if (a.ev_kind) a.ev_kind[*a.ev_used] = 0;
+        if ((e = cudaEventRecord(a.ev[(*a.ev_used)++][1], s)) != cudaSuccess) return e;
+    }
+    collect_count_kernel<<<(a.nq + 7) / 8, 256, 0, s>>>(d_count, p.n_seg, a.nq, totals, maxseg);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if (launches) *launches += 3;
+    return cudaSuccess;
+}
+
+cudaError_t launch_mma_gather(const MmaArgs& a, const MmaCollect& c, void* workspace, const int64_t* dst_off,
+                              uint64_t* dst, int ties_low, cudaStream_t s) {
+    const Plan p = make_plan(a.device, a.n_corpus, a.dim, a.nq, 1, a.split != 0, c.per_chunk, c.cap_seg);
+    char* ws = static_cast<char*>(workspace);
+    collect_gather_kernel<<<a.nq, kSelectThreads, 0, s>>>(reinterpret_cast<const uint64_t*>(ws + p.off_cand),
+                                                          reinterpret_cast<const uint32_t*>(ws + p.off_count), p.n_seg,
+                                                          p.cap_seg, dst_off, dst, ties_low);
+    return cudaGetLastError();
 }
 
 // Debug / verification entry: all raw dot products of the tensor-core path, out[nq, n_rows] (device).

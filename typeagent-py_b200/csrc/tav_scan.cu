@@ -145,7 +145,9 @@ __device__ __forceinline__ unsigned long long global_ns() {
         if (a.trace && threadIdx.x == 0) a.trace[(slot)] = global_ns();   \
     } while (0)
 
-template <typename T, int QB, bool VEC, typename BLOB>
+// COLLECT (threshold search): no running top-k; every admitted key is appended to its query's region
+// (a.cand_keys + q * a.collect_stride) through a per-query counter that keeps counting past the region.
+template <typename T, int QB, bool VEC, typename BLOB, bool COLLECT = false>
 __global__ void __launch_bounds__(kScanThreads)
 scan_rows_kernel(const ScanArgs a, const __grid_constant__ BLOB blob) {
     constexpr bool kBlob = BlobTraits<BLOB>::kHas;
@@ -187,11 +189,12 @@ scan_rows_kernel(const ScanArgs a, const __grid_constant__ BLOB blob) {
 
     const T* corpus = reinterpret_cast<const T*>(a.corpus);
     const int64_t n_tiles = (a.n_scan + kRoundRows - 1) / kRoundRows;
+    if constexpr (COLLECT) __syncthreads();  // queries staged (no round barriers in this mode)
 
     int need = 0;  // my last push left a list above its watermark
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         // round barrier: previous pushes visible (first round: queries staged)
-        if (__syncthreads_or(need)) {
+        if (!COLLECT && __syncthreads_or(need)) {
             need = 0;
 #pragma unroll
             for (int q = 0; q < QB; ++q) {
@@ -270,7 +273,37 @@ scan_rows_kernel(const ScanArgs a, const __grid_constant__ BLOB blob) {
         warp_transpose_reduce<NV>(acc, lane);
 
         constexpr int kLanesPerValue = 32 / NV;
-        if ((lane & (kLanesPerValue - 1)) == 0) {
+        if constexpr (COLLECT) {
+            // same admission as below; the appends of a warp are aggregated per query (one atomic each)
+            const int idx = lane / kLanesPerValue;
+            const int r = idx / QB, q = idx % QB;
+            const int64_t pos = pos0 + r;
+            bool want = (lane & (kLanesPerValue - 1)) == 0 && pos < a.n_scan && q < a.nq;
+            if (want && a.row_mask) {
+                int64_t row = rrow[0];
+#pragma unroll
+                for (int rr = 1; rr < kRowsPerWarp; ++rr) row = (r == rr) ? rrow[rr] : row;
+                want = (a.row_mask[row >> 5] >> (row & 31)) & 1u;
+            }
+            const float s = score_from_dot(acc[0]);
+            want = want && s >= a.floor_score;  // float32 compare, NaN rejected
+            const uint32_t p32 = static_cast<uint32_t>(pos);
+            const uint64_t key = make_key(s, a.ties_low ? ~p32 : p32);
+#pragma unroll
+            for (int qq = 0; qq < QB; ++qq) {
+                const unsigned m = __ballot_sync(0xFFFFFFFFu, want && q == qq);
+                if (m == 0) continue;
+                const int leader = __ffs(m) - 1;
+                uint32_t base = 0;
+                if (lane == leader) base = atomicAdd(&a.cand_count[qq], static_cast<uint32_t>(__popc(m)));
+                base = __shfl_sync(0xFFFFFFFFu, base, leader);
+                if (want && q == qq) {
+                    const uint64_t slot = static_cast<uint64_t>(base) + __popc(m & ((1u << lane) - 1u));
+                    if (slot < static_cast<uint64_t>(a.collect_stride))
+                        a.cand_keys[static_cast<size_t>(qq) * a.collect_stride + slot] = key;
+                }
+            }
+        } else if ((lane & (kLanesPerValue - 1)) == 0) {
             const int idx = lane / kLanesPerValue;
             const int r = idx / QB, q = idx % QB;
             const int64_t pos = pos0 + r;
@@ -296,6 +329,8 @@ scan_rows_kernel(const ScanArgs a, const __grid_constant__ BLOB blob) {
             }
         }
     }
+
+    if constexpr (COLLECT) return;
 
     // hand the CTA's best k per query to the global candidate buffers
     __syncthreads();
@@ -449,6 +484,56 @@ cudaError_t launch_scan(const ScanArgs& a, cudaStream_t s) {
         case TAV_F32: return launch_scan_q<float>(a, s);
         case TAV_BF16: return launch_scan_q<__nv_bfloat16>(a, s);
         case TAV_F16: return launch_scan_q<__half>(a, s);
+    }
+    return cudaErrorInvalidValue;
+}
+
+// ---- collect mode (threshold search): shared memory holds only the queries ---------------------
+static inline size_t collect_smem_bytes(int qb, int dim) {
+    return (static_cast<size_t>(qb) * dim * sizeof(float) + 15) & ~size_t(15);
+}
+
+int scan_collect_max_queries(int dim) {
+    for (int qb = 8; qb >= 1; qb >>= 1)
+        if (collect_smem_bytes(qb, dim) <= static_cast<size_t>(kScanSmemBudget)) return qb;
+    return 0;
+}
+
+int scan_collect_grid(int device, int dim, int nq, int64_t n_scan) {
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    int per_sm = static_cast<int>((200 * 1024) / (collect_smem_bytes(nq, dim) + 1024));
+    per_sm = std::max(1, std::min(per_sm, 4));
+    const int64_t tiles = (n_scan + kRoundRows - 1) / kRoundRows;
+    return static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(tiles, static_cast<int64_t>(sms) * per_sm)));
+}
+
+template <typename T, int QB>
+static cudaError_t launch_collect_t(const ScanArgs& a, cudaStream_t s) {
+    const size_t row_bytes = static_cast<size_t>(a.dim) * sizeof(T);
+    const bool vec = (row_bytes % 16 == 0) && (reinterpret_cast<uintptr_t>(a.corpus) % 16 == 0);
+    const size_t smem = collect_smem_bytes(QB, a.dim);
+    auto kern = vec ? scan_rows_kernel<T, QB, true, NoBlob, true> : scan_rows_kernel<T, QB, false, NoBlob, true>;
+    static int granted[2][16] = {};
+    cudaError_t e = ensure_dynamic_smem(kern, smem, granted[vec ? 1 : 0]);
+    if (e != cudaSuccess) return e;
+    kern<<<a.grid, kScanThreads, smem, s>>>(a, NoBlob{});
+    return cudaGetLastError();
+}
+
+template <typename T>
+static cudaError_t launch_collect_q(const ScanArgs& a, cudaStream_t s) {
+    if (a.nq <= 1) return launch_collect_t<T, 1>(a, s);
+    if (a.nq <= 2) return launch_collect_t<T, 2>(a, s);
+    if (a.nq <= 4) return launch_collect_t<T, 4>(a, s);
+    return launch_collect_t<T, 8>(a, s);
+}
+
+cudaError_t launch_scan_collect(const ScanArgs& a, cudaStream_t s) {
+    switch (a.dtype) {
+        case TAV_F32: return launch_collect_q<float>(a, s);
+        case TAV_BF16: return launch_collect_q<__nv_bfloat16>(a, s);
+        case TAV_F16: return launch_collect_q<__half>(a, s);
     }
     return cudaErrorInvalidValue;
 }

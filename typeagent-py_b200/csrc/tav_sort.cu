@@ -1,0 +1,221 @@
+// tav_sort.cu — segmented sort of the threshold search's hits (tav_range_search): every query's
+// admitted keys, unsorted, in one segment each -> descending key order, decoded into CSR items / scores.
+//
+// Keys are the library's unique 64-bit (score_bits << 32 | position) keys (tav_common.cuh), so sorting
+// them exactly gives the library's total order, ties in score included, without a stable sort.
+//   * segments of at most kSmallSortMax keys: one CTA each, bitonic sort in shared memory;
+//   * larger segments: a multi-CTA LSD radix sort over 8-bit digits, all large segments in the same
+//     launches.  Only the digits below the highest bit that varies inside a segment (min key XOR max
+//     key) are sorted: keys sharing their upper bits need no pass over them.  A pass is histogram per
+//     tile of kRadixTile keys -> per-segment prefix over (digit, tile) -> stable scatter.  Descending
+//     order comes from sorting the bucket 255 - digit ascending.
+
+#include <algorithm>
+
+#include "tav_common.cuh"
+#include "tav_internal.h"
+
+namespace tav {
+
+constexpr int kSortThreads = 256;
+constexpr int kRadixBuckets = 256;
+constexpr int kMaxRadixPasses = 8;  // 64-bit keys
+
+__device__ __forceinline__ void decode_store(uint64_t key, const SortArgs& a, int64_t at) {
+    const uint32_t kp = key_pos(key);
+    const uint32_t pos = a.ties_low ? ~kp : kp;
+    a.out_items[at] = (a.subset ? a.subset[pos] : static_cast<int64_t>(pos)) + a.item_offset;
+    a.out_scores[at] = key_score(key);
+}
+
+__device__ __forceinline__ int radix_passes(const uint64_t* minmax, int l) {
+    const uint64_t v = minmax[2 * l] ^ minmax[2 * l + 1];
+    return v ? (64 - __clzll(static_cast<long long>(v)) + 7) / 8 : 0;
+}
+
+__device__ __forceinline__ uint32_t bucket_of(uint64_t key, int pass) {
+    return 255u - static_cast<uint32_t>((key >> (8 * pass)) & 0xFFu);
+}
+
+// ---- small segments: one CTA, shared memory ---------------------------------------------------------
+__global__ void __launch_bounds__(kSortThreads) small_sort_kernel(const SortArgs a) {
+    __shared__ uint64_t keys[kSmallSortMax];
+    const SortSeg seg = a.segs[blockIdx.x];
+    if (seg.n == 0 || seg.n > kSmallSortMax) return;
+    const int n = static_cast<int>(seg.n);
+    int cap = 2;
+    while (cap < n) cap <<= 1;
+    for (int i = threadIdx.x; i < cap; i += kSortThreads) keys[i] = i < n ? seg.keys[i] : 0;  // 0: below every key
+    bitonic_sort_desc<kSortThreads>(keys, cap);
+    for (int i = threadIdx.x; i < n; i += kSortThreads) decode_store(keys[i], a, seg.out + i);
+}
+
+// ---- large segments: LSD radix sort -------------------------------------------------------------------
+struct TileRef {
+    SortSeg seg;
+    int l;          // index into a.large
+    int64_t first;  // first key of the tile inside the segment
+    int n;          // keys in the tile
+};
+__device__ __forceinline__ TileRef tile_ref(const SortArgs& a, int64_t t) {
+    TileRef r;
+    r.l = a.tile_seg[t];
+    r.seg = a.segs[a.large[r.l]];
+    r.first = (t - r.seg.tile0) * kRadixTile;
+    r.n = static_cast<int>(min(static_cast<int64_t>(kRadixTile), r.seg.n - r.first));
+    return r;
+}
+
+__global__ void __launch_bounds__(kSortThreads) radix_minmax_kernel(const SortArgs a) {
+    const TileRef r = tile_ref(a, blockIdx.x);
+    unsigned long long lo = ~0ull, hi = 0ull;
+    for (int i = threadIdx.x; i < r.n; i += kSortThreads) {
+        const unsigned long long k = r.seg.keys[r.first + i];
+        lo = min(lo, k);
+        hi = max(hi, k);
+    }
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) {
+        lo = min(lo, __shfl_xor_sync(0xFFFFFFFFu, lo, off));
+        hi = max(hi, __shfl_xor_sync(0xFFFFFFFFu, hi, off));
+    }
+    if ((threadIdx.x & 31) == 0) {
+        atomicMin(reinterpret_cast<unsigned long long*>(a.minmax + 2 * r.l), lo);
+        atomicMax(reinterpret_cast<unsigned long long*>(a.minmax + 2 * r.l + 1), hi);
+    }
+}
+
+// pass p reads the keys from `keys` when p is even, from `tmp` when odd (and writes the other one)
+__device__ __forceinline__ const uint64_t* pass_src(const SortSeg& s, int p) { return (p & 1) ? s.tmp : s.keys; }
+__device__ __forceinline__ uint64_t* pass_dst(const SortSeg& s, int p) { return (p & 1) ? s.keys : s.tmp; }
+
+__global__ void __launch_bounds__(kSortThreads) radix_hist_kernel(const SortArgs a, int pass) {
+    __shared__ uint32_t h[kRadixBuckets];
+    const TileRef r = tile_ref(a, blockIdx.x);
+    if (pass >= radix_passes(a.minmax, r.l)) return;
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const uint64_t* src = pass_src(r.seg, pass) + r.first;
+    for (int i = threadIdx.x; i < r.n; i += kSortThreads) atomicAdd(&h[bucket_of(src[i], pass)], 1u);
+    __syncthreads();
+    a.hist[static_cast<size_t>(blockIdx.x) * kRadixBuckets + threadIdx.x] = h[threadIdx.x];
+}
+
+// one CTA per large segment, thread b = bucket b: offs[tile][b] = keys of the segment in buckets < b
+// + keys in bucket b of the segment's earlier tiles
+__global__ void __launch_bounds__(kRadixBuckets) radix_offsets_kernel(const SortArgs a, int pass) {
+    __shared__ uint32_t s_warp[kRadixBuckets / 32];
+    const int l = blockIdx.x;
+    if (pass >= radix_passes(a.minmax, l)) return;
+    const SortSeg seg = a.segs[a.large[l]];
+    const int64_t nt = (seg.n + kRadixTile - 1) / kRadixTile;
+    const int b = threadIdx.x, lane = b & 31, warp = b >> 5;
+    const uint32_t* h = a.hist + static_cast<size_t>(seg.tile0) * kRadixBuckets + b;
+    uint32_t total = 0;
+    for (int64_t t = 0; t < nt; t += 8) {  // eight independent loads in flight
+        uint32_t v[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) v[u] = t + u < nt ? h[(t + u) * kRadixBuckets] : 0u;
+#pragma unroll
+        for (int u = 0; u < 8; ++u) total += v[u];
+    }
+    // exclusive scan of the bucket totals over the CTA
+    uint32_t incl = total;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, off);
+        if (lane >= off) incl += y;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    uint32_t run = incl - total;
+    for (int w = 0; w < warp; ++w) run += s_warp[w];
+    uint32_t* o = a.offs + static_cast<size_t>(seg.tile0) * kRadixBuckets + b;
+    for (int64_t t = 0; t < nt; t += 8) {
+        uint32_t v[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) v[u] = t + u < nt ? h[(t + u) * kRadixBuckets] : 0u;
+#pragma unroll
+        for (int u = 0; u < 8; ++u)
+            if (t + u < nt) {
+                o[(t + u) * kRadixBuckets] = run;
+                run += v[u];
+            }
+    }
+}
+
+// stable scatter: the tile is walked in chunks of 256 keys; inside a chunk a key's rank among equal
+// buckets is (earlier warps' count) + (earlier lanes of its warp, from __match_any_sync)
+__global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(const SortArgs a, int pass) {
+    constexpr int kWarps = kSortThreads / 32;
+    __shared__ uint32_t s_base[kRadixBuckets];
+    __shared__ uint32_t s_wcnt[kWarps][kRadixBuckets];
+    const TileRef r = tile_ref(a, blockIdx.x);
+    if (pass >= radix_passes(a.minmax, r.l)) return;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    s_base[tid] = a.offs[static_cast<size_t>(blockIdx.x) * kRadixBuckets + tid];
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) s_wcnt[w][tid] = 0;
+    __syncthreads();
+    const uint64_t* src = pass_src(r.seg, pass) + r.first;
+    uint64_t* dst = pass_dst(r.seg, pass);
+    for (int c0 = 0; c0 < r.n; c0 += kSortThreads) {
+        const int i = c0 + tid;
+        const bool valid = i < r.n;
+        const uint64_t key = valid ? src[i] : 0;
+        const uint32_t b = valid ? bucket_of(key, pass) : kRadixBuckets;
+        const unsigned peers = __match_any_sync(0xFFFFFFFFu, b);
+        const int rank = __popc(peers & ((1u << lane) - 1u));
+        if (valid && rank == 0) s_wcnt[warp][b] = __popc(peers);
+        __syncthreads();
+        if (valid) {
+            uint32_t at = s_base[b] + rank;
+            for (int w = 0; w < warp; ++w) at += s_wcnt[w][b];
+            dst[at] = key;
+        }
+        __syncthreads();
+        uint32_t add = 0;
+#pragma unroll
+        for (int w = 0; w < kWarps; ++w) {
+            add += s_wcnt[w][tid];
+            s_wcnt[w][tid] = 0;
+        }
+        s_base[tid] += add;
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(kSortThreads) radix_decode_kernel(const SortArgs a) {
+    const TileRef r = tile_ref(a, blockIdx.x);
+    const int np = radix_passes(a.minmax, r.l);
+    const uint64_t* src = ((np & 1) ? r.seg.tmp : r.seg.keys) + r.first;  // where the last pass left them
+    for (int i = threadIdx.x; i < r.n; i += kSortThreads) decode_store(src[i], a, r.seg.out + r.first + i);
+}
+
+cudaError_t launch_segmented_sort(const SortArgs& a, cudaStream_t s, int* launches) {
+    int n = 0;
+    if (a.n_segs > 0) {
+        small_sort_kernel<<<a.n_segs, kSortThreads, 0, s>>>(a);
+        ++n;
+    }
+    if (a.n_large > 0) {
+        cudaError_t e = cudaMemsetAsync(a.minmax, 0, 2 * sizeof(uint64_t) * a.n_large, s);
+        if (e != cudaSuccess) return e;
+        // min starts at ~0: the even words
+        e = cudaMemset2DAsync(a.minmax, 2 * sizeof(uint64_t), 0xFF, sizeof(uint64_t), a.n_large, s);
+        if (e != cudaSuccess) return e;
+        const unsigned tiles = static_cast<unsigned>(a.n_tiles);
+        radix_minmax_kernel<<<tiles, kSortThreads, 0, s>>>(a);
+        for (int p = 0; p < kMaxRadixPasses; ++p) {
+            radix_hist_kernel<<<tiles, kSortThreads, 0, s>>>(a, p);
+            radix_offsets_kernel<<<a.n_large, kRadixBuckets, 0, s>>>(a, p);
+            radix_scatter_kernel<<<tiles, kSortThreads, 0, s>>>(a, p);
+        }
+        radix_decode_kernel<<<tiles, kSortThreads, 0, s>>>(a);
+        n += 2 + 3 * kMaxRadixPasses;
+    }
+    if (launches) *launches += n;
+    return cudaGetLastError();
+}
+
+}  // namespace tav

@@ -13,6 +13,8 @@ Additions (not in the reference; all opt-in):
   * ``fuzzy_lookup_embeddings`` / ``search_arrays`` — batched lookups, the replacement for
     the one-query-at-a-time loops in storage/memory/reltermsindex.py:320-332 and
     storage/sqlite/reltermsindex.py:259-271;
+  * ``search_range`` — threshold (range) search: every row at or above min_score, CSR results in
+    one read of the rows; ``fuzzy_lookup_embeddings(max_hits=0)`` builds its lists from it;
   * ``search_arrays(..., allowed=mask)`` — predicate / post-filter pushdown as a row bitmask
     evaluated inside the kernels (vectorbase.py:191-201, storage/sqlite/messageindex.py:296-326);
   * constructor keywords ``device``, ``storage_dtype``, ``normalize``;
@@ -128,13 +130,16 @@ class VectorBase:
         self._adopted_tensor = None
         self._single_out: dict[int, tuple] = {}  # k -> reusable result arrays of fuzzy_lookup_embedding
         self._subset_buf: tuple | None = None  # (reusable int64 buffer for list subsets, its address)
-        self._single_lock = threading.Lock()   # guards the two reusable buffers above
+        # guards the two reusable buffers above, and the index's threshold-search hits between a search and
+        # their fetch (a lookup with k >= rows may be served by that engine too)
+        self._single_lock = threading.Lock()
         self.force_path: str | None = None  # "scan" | "mma" | "scan2" (two-kernel scan) | None (tests / benchmarks)
         self._timing = False
         self._pending: list = []             # tensors of deferred device searches, kept alive until finish_search()
         self._mask_key = None                # identity of the row mask currently on the device
         self._mask_ref = None                # ... and the object(s) that identity belongs to (so id() cannot be recycled)
         self._predicate_masks: dict = {}     # (id(predicate), generation, n) -> packed bitmask
+        self._range_hint = 0                 # hits of the last search_range: the next one's capacity hint
         self.clear()
 
     # ------------------------------------------------------------------ housekeeping
@@ -430,16 +435,78 @@ class VectorBase:
             flags |= _capi.TAV_USE_ROW_MASK
         if ties_low_first:
             flags |= _capi.TAV_TIES_LOW_FIRST
+        with self._single_lock:
+            _capi.check(
+                lib.tav_search(
+                    ix, q.ctypes.data_as(C.c_void_p), b, k_eff, C.c_float(float(floor)), flags,
+                    sub.ctypes.data_as(C.c_void_p) if sub is not None else None,
+                    len(sub) if sub is not None else 0, 0,
+                    items.ctypes.data_as(C.c_void_p), scores.ctypes.data_as(C.c_void_p),
+                    counts.ctypes.data_as(C.c_void_p), None,
+                )
+            )
+        return items, scores, counts
+
+    def search_range(
+        self,
+        queries: np.ndarray,
+        min_score: float = 0.0,
+        subset: Sequence[int] | np.ndarray | None = None,
+        allowed: np.ndarray | None = None,
+        ties_low_first: bool = False,
+    ) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """Threshold (range) search: EVERY row whose score is >= min_score, per query, in one read of
+        the rows.  Returns CSR arrays: offsets int64 [B + 1], items int64 [T], scores float32 [T];
+        query b's hits are items[offsets[b]:offsets[b + 1]], in the library's order (score descending,
+        equal scores higher ordinal first, or lower first with ``ties_low_first``).  ``subset`` and
+        ``allowed`` as in ``search_arrays``.  Batches run on the tensor cores (16-bit storage, or float32
+        through its fp16 planes), like ``search_arrays``.  The previous call's total sizes the device buffers."""
+        q = self._check_queries(queries)
+        b = len(q)
+        n_rows = len(self)
+        sub = None
+        if subset is not None:
+            sub = np.ascontiguousarray(subset)
+            if sub.size and not np.issubdtype(sub.dtype, np.integer):
+                raise IndexError("arrays used as indices must be of integer (or boolean) type")
+            sub = sub.astype(np.int64, copy=False).reshape(-1)
+            n_rows = len(sub)
+        if allowed is not None and sub is not None:
+            raise ValueError("allowed= and subset= cannot be combined")
+        offsets = np.zeros(b + 1, dtype=np.int64)
+        floor = _as_f32_scalar(min_score)
+        if b == 0 or n_rows == 0 or len(self) == 0 or np.isnan(floor):
+            return offsets, np.empty(0, np.int64), np.empty(0, np.float32)
+        # the hits wait in the index's buffers between the two calls: no other lookup of this object may
+        # search in between (ctypes releases the GIL)
+        with self._single_lock:
+            return self._search_range_locked(q, floor, sub, allowed, ties_low_first, offsets)
+
+    def _search_range_locked(self, q, floor, sub, allowed, ties_low_first, offsets):
+        b = len(q)
+        lib, ix = self._ensure_device()
+        flags = self._flags() & ~_capi.TAV_NO_FUSED_SCAN
+        if allowed is not None:
+            self._use_row_mask(lib, ix, allowed)
+            flags |= _capi.TAV_USE_ROW_MASK
+        if ties_low_first:
+            flags |= _capi.TAV_TIES_LOW_FIRST
         _capi.check(
-            lib.tav_search(
-                ix, q.ctypes.data_as(C.c_void_p), b, k_eff, C.c_float(float(floor)), flags,
+            lib.tav_range_search(
+                ix, q.ctypes.data_as(C.c_void_p), b, C.c_float(float(floor)), flags,
                 sub.ctypes.data_as(C.c_void_p) if sub is not None else None,
-                len(sub) if sub is not None else 0, 0,
-                items.ctypes.data_as(C.c_void_p), scores.ctypes.data_as(C.c_void_p),
-                counts.ctypes.data_as(C.c_void_p), None,
+                len(sub) if sub is not None else 0, 0, self._range_hint,
+                offsets.ctypes.data_as(C.c_void_p), None,
             )
         )
-        return items, scores, counts
+        total = int(offsets[-1])
+        items = np.empty(total, dtype=np.int64)
+        scores = np.empty(total, dtype=np.float32)
+        if total:
+            _capi.check(lib.tav_range_fetch(ix, 0, total, items.ctypes.data_as(C.c_void_p),
+                                            scores.ctypes.data_as(C.c_void_p), 0, None))
+        self._range_hint = total
+        return offsets, items, scores
 
     def enable_timing(self, enabled: bool = True, main_only: bool = False) -> None:
         """Record CUDA events around the kernels of subsequent lookups (see ``last_timing``);
@@ -645,6 +712,12 @@ class VectorBase:
         if len(self) == 0:
             return [[] for _ in range(len(q))]
         k = self._resolve_k(max_hits, len(self))
+        if max_hits == 0:
+            # every passing row: CSR lists from the threshold search instead of [B, N] arrays
+            offsets, items, scores = self.search_range(q, min_score)
+            il, sl, ol = items.tolist(), scores.tolist(), offsets.tolist()
+            return [[ScoredInt(i, s) for i, s in zip(il[ol[b]:ol[b + 1]], sl[ol[b]:ol[b + 1]])]
+                    for b in range(len(q))]
         items, scores, counts = self.search_arrays(q, k, min_score)
         # three bulk conversions, then plain list slices: 1.6x faster than slicing the arrays per query
         il, sl, cl = items.tolist(), scores.tolist(), counts.tolist()
