@@ -54,7 +54,13 @@ enum tav_index_flags {
     /* L2-normalise every appended row (fused into the convert-on-append kernel) and every
      * query (fused into query staging): cosine similarity for un-normalised inputs.  The
      * default (0) is the reference's behaviour: a plain dot product that relies on the
-     * caller's unit-norm embeddings (vectorbase.py:176, model_adapters.py:176-184). */
+     * caller's unit-norm embeddings (vectorbase.py:176, model_adapters.py:176-184).
+     * A row (or query) is first scaled by the power of two of its largest magnitude, which is
+     * exact, so rows of any finite scale normalise to within a few float32 ulps of v / ||v||
+     * (then one rounding to the storage type).  Edge cases:
+     *   - a zero row stays zero and is returned with score 0.5 (dot 0);
+     *   - a row with a NaN or +-inf element has NaN dots and is never returned;
+     *   - a zero query stays zero and returns every row without NaN or inf at score 0.5. */
     TAV_NORMALIZE = 1
 };
 
@@ -161,8 +167,10 @@ int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items,
 /* Completes EVERY outstanding TAV_DEFER_RETRY search of the index: synchronises `stream`, redoes
  * each search's flagged queries exactly into that search's own outputs and reports how many
  * (*redone).  The caller keeps the query and output buffers of deferred searches alive until
- * then.  Up to 64 searches may be outstanding (a 65th finishes the earlier ones first).  No-op
- * when nothing is pending. */
+ * then.  Up to 64 searches may be outstanding (a 65th finishes the earlier ones first, and the
+ * queries redone then are not counted in *redone).  On a TAV_NORMALIZE index each outstanding
+ * search keeps its normalised queries in device memory of its own (grown as needed, never by
+ * finishing searches early) until this call.  No-op when nothing is pending. */
 int tav_finish_search(tav_index* ix, void* stream, int* redone);
 
 /* Row mask for TAV_USE_ROW_MASK: `n_rows` bits (bit r of word r/32 = row r allowed), host or
@@ -230,7 +238,8 @@ int tav_fold_groups(int device, int n_queries, int k, const int32_t* row_to_grou
 
 /* Verification aid for the tensor-core path: every raw dot product it computes,
  * out_device[n_queries, size] float32 (device memory); float32 indexes go through their fp16 planes.  `flags` may
- * carry TAV_QUERIES_ON_DEVICE.  Synchronises.  Not a hot-path entry point. */
+ * carry TAV_QUERIES_ON_DEVICE.  On a TAV_NORMALIZE index the queries are normalised first, as a search
+ * does.  Synchronises.  Not a hot-path entry point. */
 int tav_mma_scores(tav_index* ix, const float* queries, int n_queries, int flags, float* out_device,
                    void* stream);
 

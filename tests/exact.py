@@ -105,8 +105,8 @@ _U = 2.0 ** -23  # unit roundoff per addition: the tensor cores' adder is not sp
 #                  so a truncating one (error < 1 ulp) is allowed for
 
 
-def _gamma(m: int) -> float:
-    return m * _U / (1.0 - m * _U)
+def _gamma(m: int, u: float = _U) -> float:
+    return m * u / (1.0 - m * u)
 
 
 def dot_error_bound(q, v, split=False):
@@ -125,3 +125,147 @@ def dot_error_bound(q, v, split=False):
     eta = 2.0 ** -36
     rep = (2 * rel + rel * rel) * mag + eta * (q.sum(1)[:, None] + v.sum(1)[None, :] + d * eta)
     return (_gamma(2 * d + 1) + rel) * (mag + rep) + rep + _U * (mag + rep)
+
+
+# ---------------------------------------------------------------- storage conversion
+def round_to(x, dtype: str) -> np.ndarray:
+    """float32 values rounded once, to nearest even, to `dtype` and upcast (exactly) back to float32:
+    numpy's own conversion for float16, ``round_to_bfloat16`` for bfloat16.  NaN stays NaN."""
+    x = np.asarray(x, np.float32)
+    if dtype == "float32":
+        return x.copy()
+    if dtype == "float16":
+        with np.errstate(over="ignore"):
+            return x.astype(np.float16).astype(np.float32)
+    from oracle.vectorbase_oracle import round_to_bfloat16
+
+    return round_to_bfloat16(x)
+
+
+def to_bits16(x, dtype: str) -> np.ndarray:
+    """The uint16 encoding of float32 values already representable in `dtype` (bfloat16 or float16)."""
+    x = np.asarray(x, np.float32)
+    if dtype == "float16":
+        with np.errstate(over="ignore"):
+            return x.astype(np.float16).view(np.uint16)
+    assert dtype == "bfloat16"
+    bits = x.view(np.uint32)
+    assert ((bits & 0xFFFF) == 0)[~np.isnan(x)].all(), "not a bfloat16 value"
+    return (bits >> 16).astype(np.uint16)
+
+
+def _f32(bits) -> np.ndarray:
+    return np.array(bits, np.uint32).view(np.float32)
+
+
+def conversion_edges() -> dict[str, np.ndarray]:
+    """float32 values where a conversion to bfloat16 or float16 goes wrong first, by class (positive
+    values: the sign is added where they are used, except in "zero_inf_nan")."""
+    bf = np.array([0x3F80, 0x3F81, 0x4049, 0x404A, 0x0080, 0x0081, 0x0001, 0x0002, 0x7F7E], np.uint32)
+    h = np.array([0x3C00, 0x3C01, 0x0001, 0x0002, 0x03FF, 0x7BFE, 0x0400, 0x5BFF], np.uint16)
+    h_lo = h.view(np.float16).astype(np.float64)
+    h_hi = (h + 1).astype(np.uint16).view(np.float16).astype(np.float64)
+    fp16_mid = ((h_lo + h_hi) / 2).astype(np.float32)  # exact in float32
+    bf_max, fp_max = _f32([0x7F7F0000])[0], np.float32(65504)
+    return {
+        # tie at bfloat16 precision: even and odd last bit, normal, subnormal and large; and one float32 ulp off
+        "bf16_halfway": _f32(np.concatenate([(bf << 16) | 0x8000, (bf << 16) | 0x7FFF, (bf << 16) | 0x8001])),
+        "fp16_halfway": np.concatenate([fp16_mid, np.nextafter(fp16_mid, np.float32(0)),
+                                        np.nextafter(fp16_mid, np.float32(np.inf))]),
+        # the largest finite value of each format, one float32 ulp past it, half a target ulp past it
+        "max_finite": np.array([bf_max, np.nextafter(bf_max, np.float32(np.inf)), _f32([0x7F7F7FFF])[0],
+                                _f32([0x7F7F8000])[0], np.finfo(np.float32).max, fp_max,
+                                np.nextafter(fp_max, np.float32(np.inf)), 65519.996, 65536.0], np.float32),
+        "fp16_overflow": np.array([65520.0, np.nextafter(np.float32(65520), np.float32(0)), 65521.0, 1e5, 1e38],
+                                  np.float32),
+        "subnormal": np.array([2.0 ** -24, 3 * 2.0 ** -24, 2.0 ** -14, 2.0 ** -14 - 2.0 ** -24, 2.0 ** -133,
+                               2.0 ** -126, 2.0 ** -149, 2.0 ** -127 * 3], np.float32),
+        "rounds_to_zero": np.array([2.0 ** -25, np.nextafter(np.float32(2.0 ** -25), np.float32(0)),
+                                    np.nextafter(np.float32(2.0 ** -25), np.float32(1)), 2.0 ** -26, 2.0 ** -134,
+                                    2.0 ** -135, 2.0 ** -149, 1e-30], np.float32),
+        "zero_inf_nan": np.array([0.0, -0.0, np.inf, -np.inf, np.nan, -np.nan], np.float32),
+    }
+
+
+_U_RN = 2.0 ** -24  # unit roundoff of the CUDA cores' float32 fma, sqrtf and division (round to nearest)
+# storage rounding: (relative unit roundoff, absolute error in the subnormal range)
+_STORE = {"float32": (0.0, 0.0), "bfloat16": (2.0 ** -8, 2.0 ** -134), "float16": (2.0 ** -11, 2.0 ** -25)}
+
+
+def normalize_error_bound(v, storage="float32"):
+    """float64 [N, D]: a rigorous bound on |stored - v / ||v||| for rows normalised as the append kernel
+    does: v scaled by a power of two (exact), the float32 sum of squares in ANY order (gamma_d relative; at
+    most d roundings on any path, plus d * 2^-149 for squares of scaled values below the normal range:
+    the scaled sum is >= 1/4), the square root and the division (one rounding each, 2^-148 for a scaled
+    value or quotient in the subnormal range), then the storage rounding of that float32 quotient (a second
+    rounding on 16-bit storage, bounded separately: the bound holds for double rounding).  Zero rows: 0."""
+    v = np.asarray(v, np.float64)
+    d = v.shape[1]
+    x = np.abs(v) / np.maximum(np.sqrt((v * v).sum(1, keepdims=True)), np.finfo(np.float64).tiny)
+    d_ss = _gamma(d, _U_RN) * (1 + _U_RN) + d * 2.0 ** -147
+    e_nrm = d_ss + _U_RN + d_ss * _U_RN  # sqrt(1 + a) - 1 <= a: halving the relative error is not needed
+    rel = (1 + _U_RN) / (1 - e_nrm) - 1
+    err32 = rel * x + 2.0 ** -148
+    u_s, abs_s = _STORE[storage]
+    return err32 + u_s * (x + err32) + abs_s
+
+
+def _two_squares_table(amp: int) -> dict[int, tuple[int, int]]:
+    t: dict[int, tuple[int, int]] = {}
+    for a in range(amp + 1):
+        for b in range(a, amp + 1):
+            t.setdefault(a * a + b * b, (a, b))
+    return t
+
+
+def four_squares(r: int, amp: int, table=None) -> tuple[int, int, int, int]:
+    """Non-negative integers <= amp whose squares sum to r (raises ValueError when there are none)."""
+    table = table if table is not None else _two_squares_table(amp)
+    for a in range(min(amp, math.isqrt(r)), -1, -1):
+        for b in range(min(a, math.isqrt(r - a * a)), -1, -1):
+            pair = table.get(r - a * a - b * b)
+            if pair is not None:
+                return a, b, pair[0], pair[1]
+    raise ValueError(f"{r} is not a sum of four squares <= {amp}^2")
+
+
+def unit_rows(n, d, amp, seed, e_range=(-100, 64)):
+    """Integer rows a [n, d] with |a_i| <= amp and sum a_i^2 = 4^m exactly (one m for all rows), each
+    multiplied by its own power of two 2^e, e uniform in ``e_range``.  Returns (rows float32 = a * 2^e,
+    a int64, m, e int64 [n]).  The normalised row is exactly a / 2^m — held by float32, and with amp <= 255
+    (m <= 11) by bfloat16 and float16 too — and dots of two such rows are exact in float32 (d amp^2 < 2^24).
+    The first d - 4 coordinates are drawn, adjusted until the remainder to 4^m is at most 2 amp^2, and
+    the last four are a four-square decomposition of that remainder."""
+    assert d >= 4 and d * amp * amp < (1 << 24)
+    rng = np.random.default_rng(seed)
+    mean_sq = amp * (amp + 1) / 3.0  # E[a^2] of an integer uniform on [-amp, amp]
+    m = max(1, int(math.floor(math.log(max(4.0, (d - 4) * mean_sq + amp * amp), 4))))
+    target, cap = 4 ** m, 2 * amp * amp
+    a = rng.integers(-amp, amp + 1, size=(n, d), dtype=np.int64)
+    a[:, d - 4:] = 0
+    free = max(d - 4, 1)
+    rem = target - (a * a).sum(1)
+    for _ in range(100 * d + 1000):
+        over, under = rem < 0, rem > cap
+        if not (over.any() or under.any()):
+            break
+        j = rng.integers(0, free, size=n)
+        rows = np.arange(n)
+        old = a[rows, j] ** 2
+        # too large: zero a coordinate; too small: raise one as far as the remainder allows
+        grow = np.minimum(amp, np.sqrt((old + np.maximum(rem, 0)).astype(np.float64)).astype(np.int64))
+        new = np.where(over, 0, np.where(under, grow * grow, old))
+        sign = np.where(a[rows, j] < 0, -1, 1)
+        if d > 4:
+            a[rows, j] = sign * np.where(over, 0, np.where(under, grow, np.abs(a[rows, j])))
+        rem -= new - old
+    assert ((rem >= 0) & (rem <= cap)).all(), "remainders did not settle"
+    table = _two_squares_table(amp)
+    for i in range(n):
+        a[i, d - 4:] = np.array(four_squares(int(rem[i]), amp, table)) * rng.choice([-1, 1], size=4)
+    perm = rng.permuted(np.tile(np.arange(d), (n, 1)), axis=1)  # the four fill-ins anywhere in the row
+    a = np.take_along_axis(a, perm, axis=1)
+    assert ((a * a).sum(1) == target).all() and np.abs(a).max() <= amp
+    e = rng.integers(e_range[0], e_range[1] + 1, size=n)
+    rows = (a.astype(np.float64) * np.exp2(e.astype(np.float64))[:, None]).astype(np.float32)
+    return rows, a, m, e

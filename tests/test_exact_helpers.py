@@ -116,3 +116,128 @@ def test_dot_error_bound_covers_float32_accumulation():
             naive += q[:, i:i + 1] * v[:, i][None, :]
         assert (np.abs(naive - exact) <= dot_error_bound(q, v)).all()
         assert (dot_error_bound(q, v) <= dot_error_bound(q, v, split=True)).all()
+
+
+# ---------------------------------------------------------------- storage conversion references
+def test_bfloat16_and_float16_references_match_torch():
+    import torch
+
+    from tests.exact import conversion_edges, round_to
+
+    rng = np.random.default_rng(6)
+    edges = np.concatenate(list(conversion_edges().values()))
+    x = np.concatenate([edges, -edges, (rng.standard_normal(20000) * np.exp2(rng.integers(-150, 126, 20000)))
+                        .astype(np.float32)])
+    for dtype, tdtype in (("bfloat16", torch.bfloat16), ("float16", torch.float16)):
+        want = torch.from_numpy(x).to(tdtype).to(torch.float32).numpy()
+        got = round_to(x, dtype)
+        nan = np.isnan(want)
+        np.testing.assert_array_equal(np.isnan(got), nan)
+        np.testing.assert_array_equal(got[~nan].view(np.uint32), want[~nan].view(np.uint32))  # -0.0 too
+
+
+def test_conversion_edges_hit_their_cases():
+    from tests.exact import conversion_edges, round_to, to_bits16
+
+    e = conversion_edges()
+    bf_ties = e["bf16_halfway"][:9]
+    up = round_to(bf_ties, "bfloat16")
+    # ties go to the even neighbour: last bfloat16 bit of the result is 0
+    assert ((up.view(np.uint32) >> 16) & 1 == 0).all() and (up != bf_ties).all()
+    h_ties = e["fp16_halfway"][:8]
+    r = round_to(h_ties, "float16")
+    assert (to_bits16(r, "float16") & 1 == 0).all() and (r != h_ties).all()
+    assert round_to(np.float32([65520.0]), "float16")[0] == np.inf
+    assert round_to(np.float32([np.nextafter(np.float32(65520), np.float32(0))]), "float16")[0] == 65504
+    assert np.isinf(round_to(e["max_finite"][3:4], "bfloat16")).all()  # half a bfloat16 ulp past the max
+    assert (round_to(e["rounds_to_zero"][:2], "float16") == 0).all()
+    assert round_to(e["rounds_to_zero"][2:3], "float16")[0] == 2.0 ** -24
+    assert round_to(np.float32([-2.0 ** -26]), "float16").view(np.uint32)[0] == 0x80000000  # -0.0
+    assert round_to(np.float32([2.0 ** -133]), "bfloat16")[0] == 2.0 ** -133
+
+
+# ---------------------------------------------------------------- normalisation: exact rows and the bound
+def test_four_squares():
+    from tests.exact import four_squares
+
+    for r in list(range(0, 300)) + [2 * 255 * 255, 130049, 99991]:
+        parts = four_squares(r, 255)
+        assert sum(p * p for p in parts) == r and max(parts) <= 255
+    with pytest.raises(ValueError):
+        four_squares(4 * 9 + 1, 3)
+
+
+@pytest.mark.parametrize("d", [4, 5, 64, 136, 1536])
+def test_unit_rows_normalise_exactly(d):
+    from oracle import vectorbase_oracle as O
+    from tests.exact import unit_rows
+
+    amp = min(255, int(np.sqrt((1 << 24) / d - 1)))
+    rows, a, m, e = unit_rows(400, d, amp, seed=d)
+    assert ((a * a).sum(1) == 4 ** m).all() and np.abs(a).max() <= amp and m <= 11
+    assert e.min() <= -90 and e.max() >= 55  # the scales span [2^-100, 2^64]
+    np.testing.assert_array_equal(rows.astype(np.float64), a * np.exp2(e.astype(np.float64))[:, None])
+    unit = a.astype(np.float32) * np.float32(2.0 ** -m)
+    for storage in ("bfloat16", "float16"):
+        np.testing.assert_array_equal(O.round_to_storage(unit, storage), unit)
+    # the float32 sum of squares of the raw rows leaves the float32 range at both ends
+    with np.errstate(over="ignore", under="ignore"):
+        ss = (rows * rows).sum(1, dtype=np.float32)
+    assert (ss[e <= -80] < 2.0 ** -126).all() and np.isinf(ss[e >= 64 - 2]).all()
+
+
+def _normalise_f32(v, scaled=True, order="seq"):
+    """The append kernel's arithmetic in numpy float32: power-of-two scaling (exact), sum of squares
+    in the given order, sqrt, division."""
+    v = np.asarray(v, np.float32)
+    with np.errstate(over="ignore", under="ignore", invalid="ignore", divide="ignore"):
+        amax = np.abs(v).max(1, keepdims=True)
+        shift = np.frexp(amax)[1] if scaled else np.zeros_like(amax, np.int32)
+        w = np.ldexp(v, -shift).astype(np.float32)
+        sq = w * w
+        if order == "seq":
+            ss = np.zeros(len(v), np.float32)
+            for i in range(v.shape[1]):
+                ss = ss + sq[:, i]
+        elif order == "reverse":
+            ss = np.zeros(len(v), np.float32)
+            for i in reversed(range(v.shape[1])):
+                ss = ss + sq[:, i]
+        else:
+            ss = sq.sum(1, dtype=np.float32)  # numpy's pairwise order
+        nrm = np.sqrt(ss)[:, None]
+        return np.where(nrm > 0, w / nrm, v).astype(np.float32)
+
+
+@pytest.mark.parametrize("storage", ["float32", "bfloat16", "float16"])
+def test_normalize_error_bound_covers_the_kernel_arithmetic(storage):
+    from tests.exact import normalize_error_bound, round_to
+
+    rng = np.random.default_rng(8)
+    for d in (1, 7, 64, 1536):
+        n = 200
+        v = rng.standard_normal((n, d)) * np.exp2(rng.integers(-140, 101, (n, 1)))
+        v *= np.where(rng.random((n, d)) < 0.2, 2.0 ** -60, 1.0)
+        v = v.astype(np.float32)
+        v = v[np.abs(v).max(1) > 0]
+        vv = v.astype(np.float64)
+        exact = vv / np.sqrt((vv * vv).sum(1, keepdims=True))
+        bound = normalize_error_bound(v, storage)
+        for order in ("seq", "reverse", "pairwise"):
+            got = round_to(_normalise_f32(v, True, order), storage).astype(np.float64)
+            assert (np.abs(got - exact) <= bound).all(), (d, order)
+        # not vacuous: a few float32 ulps (plus the storage rounding)
+        u_s = {"float32": 0.0, "bfloat16": 2.0 ** -8, "float16": 2.0 ** -11}[storage]
+        assert (bound <= (d + 8) * 2.0 ** -24 * np.abs(exact) + u_s * np.abs(exact) * 1.01 + 2.0 ** -25 + 2.0 ** -140).all()
+        # unscaled arithmetic breaks the bound on rows whose squares leave the float32 range
+        tiny_or_huge = np.abs(v).max(1) < 1e-20
+        if tiny_or_huge.any():
+            got = round_to(_normalise_f32(v[tiny_or_huge], False), storage).astype(np.float64)
+            assert (np.abs(got - exact[tiny_or_huge]) > bound[tiny_or_huge]).any()
+
+
+def test_normalize_error_bound_zero_rows():
+    from tests.exact import normalize_error_bound
+
+    b = normalize_error_bound(np.zeros((2, 5), np.float32), "bfloat16")
+    assert (b < 2.0 ** -100).all()

@@ -114,7 +114,7 @@ struct TimedSearch {
 
 // a TAV_DEFER_RETRY search whose "redo exactly" flags have not been looked at yet
 struct Pending {
-    const float* queries;  // device
+    const float* queries;  // device: the caller's, or normalised ones in tav_index::held_queries
     int nq, k;
     float floor;
     int64_t item_offset;
@@ -163,6 +163,11 @@ struct tav_index {
     int retry_cap = 0;
     std::vector<Pending> pending;
     int next_slot = 0;
+    // normalised queries of deferred searches (TAV_NORMALIZE): each pending search owns a region here that
+    // later searches do not touch, until tav_finish_search has redone its flagged queries
+    DevBuf held_queries;
+    size_t held_used = 0;        // bytes of held_queries used by pending searches
+    std::vector<DevBuf> held_retired;  // outgrown held_queries buffers that pending searches still read
     int last_first_slot = -1, last_n_slots = 0;   // bookkeeping slots of the most recent search (-1: row scan)
     // float32 indexes: the rows as two fp16 planes for the tensor-core path (built lazily,
     // extended on append); split_flag[0] = a corpus value left the fp16 range
@@ -294,12 +299,13 @@ int tav_destroy(tav_index* ix) {
     cudaSetDevice(ix->device);
     cudaDeviceSynchronize();  // searches may still be in flight on the caller's streams
     if (ix->rows && !ix->adopted) cudaFree(ix->rows);
-    for (DevBuf* b : {&ix->queries, &ix->subset, &ix->cand_keys, &ix->cand_count, &ix->out_pack, &ix->staging,
+    for (DevBuf* b : {&ix->queries, &ix->held_queries, &ix->subset, &ix->cand_keys, &ix->cand_count, &ix->out_pack, &ix->staging,
                       &ix->mma_ws, &ix->retry, &ix->split_hi, &ix->split_lo, &ix->split_flag, &ix->row_mask,
                       &ix->range_keys, &ix->range_keys2, &ix->range_counts, &ix->range_qgather, &ix->range_tmp,
                       &ix->range_sortws, &ix->range_items, &ix->range_scores, &ix->range_mmaws,
                       &ix->range_mmaws2, &ix->range_mmaaux})
         b->release();
+    for (DevBuf& b : ix->held_retired) b.release();
     if (ix->ev_range) cudaEventDestroy(ix->ev_range);
     ix->pin_in.release();
     ix->pin_out.release();
@@ -724,11 +730,15 @@ static int finish_pending(tav_index* ix, cudaStream_t s, int* redone) {
             if (rc != TAV_OK) return rc;
         }
     }
-    if (dirty) {
-        TAV_CUDA(cudaMemsetAsync(ix->retry.p, 0, sizeof(totals), s));
-        TAV_CUDA(cudaStreamSynchronize(s));
-        memset(ix->retry_host.p, 0, sizeof(totals));
-    }
+    if (dirty) TAV_CUDA(cudaMemsetAsync(ix->retry.p, 0, sizeof(totals), s));
+    if (dirty || n_redone > 0) TAV_CUDA(cudaStreamSynchronize(s));
+    if (dirty) memset(ix->retry_host.p, 0, sizeof(totals));
+    // No queued work reads a held query region now, whatever stream a later search uses: the searches ended
+    // at the first synchronisation above, their redo scans at the last.  So the regions can be reused and the
+    // outgrown buffers freed.
+    ix->held_used = 0;
+    for (DevBuf& b : ix->held_retired) b.release();
+    ix->held_retired.clear();
     if (redone) *redone = n_redone;
     return TAV_OK;
 }
@@ -747,10 +757,11 @@ static int range_alloc(DevBuf& b, size_t bytes, const char* what) {
 
 // host queries / subset -> device, shared by tav_search and the threshold search: subset ordinals through
 // pinned staging, queries float32 (normalised when the index is TAV_NORMALIZE).  `o_dev`: the call returns
-// without synchronising, so the pinned staging stays busy until the copies are done.
+// without synchronising, so the pinned staging stays busy until the copies are done.  `held`: where normalised
+// queries go instead of ix->queries (a deferred search's own region).
 static int stage_inputs(tav_index* ix, TimedSearch* ts, bool timing, const float* queries, int n_queries, bool q_dev,
                         bool o_dev, const int64_t* subset, int64_t subset_len, const float** out_queries,
-                        const int64_t** out_subset, cudaStream_t s) {
+                        const int64_t** out_subset, cudaStream_t s, float* held = nullptr) {
     const int64_t* d_subset = nullptr;
     // subset ordinals -> device
     if (subset) {
@@ -773,7 +784,8 @@ static int stage_inputs(tav_index* ix, TimedSearch* ts, bool timing, const float
     const float* d_queries = queries;
     const size_t q_bytes = static_cast<size_t>(n_queries) * ix->dim * sizeof(float);
     if (!q_dev || (ix->flags & TAV_NORMALIZE)) {
-        TAV_CUDA(ix->queries.ensure(q_bytes));
+        if (!held) TAV_CUDA(ix->queries.ensure(q_bytes));
+        float* dst = held ? held : static_cast<float*>(ix->queries.p);
         if (ix->flags & TAV_NORMALIZE) {
             const void* src = queries;
             if (!q_dev) {
@@ -781,7 +793,7 @@ static int stage_inputs(tav_index* ix, TimedSearch* ts, bool timing, const float
                 TAV_CUDA(cudaMemcpyAsync(ix->staging.p, queries, q_bytes, cudaMemcpyHostToDevice, s));
                 src = ix->staging.p;
             }
-            TAV_CUDA(launch_convert(src, TAV_F32, ix->queries.p, TAV_F32, n_queries, ix->dim, 1, s));
+            TAV_CUDA(launch_convert(src, TAV_F32, dst, TAV_F32, n_queries, ix->dim, 1, s));
             ts->launches += 1;
         } else {
             const void* src = queries;
@@ -798,9 +810,9 @@ static int stage_inputs(tav_index* ix, TimedSearch* ts, bool timing, const float
                 memcpy(static_cast<char*>(ix->pin_in.p) + sub_off, queries, q_bytes);
                 src = static_cast<char*>(ix->pin_in.p) + sub_off;
             }
-            TAV_CUDA(cudaMemcpyAsync(ix->queries.p, src, q_bytes, cudaMemcpyHostToDevice, s));
+            TAV_CUDA(cudaMemcpyAsync(dst, src, q_bytes, cudaMemcpyHostToDevice, s));
         }
-        d_queries = static_cast<const float*>(ix->queries.p);
+        d_queries = dst;
     }
 
     if (o_dev && (!q_dev || subset)) {  // no synchronisation at the end of this call
@@ -1440,9 +1452,33 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         return TAV_OK;
     }
 
+    // A deferred search redoes its flagged queries at tav_finish_search, after later searches on this index
+    // have restaged ix->queries: normalised queries then go to a region of held_queries that is its own
+    // until then.  When they do not fit, a buffer of at least twice the size takes over and the old one is
+    // kept (not freed) until the searches that read it are finished: no search is finished early.
+    const bool defer = (flags & TAV_DEFER_RETRY) && o_dev && q_dev;
+    float* held = nullptr;
+    size_t held_end = 0;
+    if (use_mma && defer && (ix->flags & TAV_NORMALIZE)) {
+        const size_t q_bytes = (static_cast<size_t>(n_queries) * ix->dim * sizeof(float) + 255) & ~size_t(255);
+        const size_t need = ix->held_used + q_bytes;
+        if (need > ix->held_queries.bytes) {
+            const size_t want = std::max(need, 2 * ix->held_queries.bytes);
+            if (ix->held_used > 0) {  // pending searches read the current buffer
+                ix->held_retired.push_back(ix->held_queries);
+                ix->held_queries = DevBuf{};
+                ix->held_used = 0;
+            }
+            TAV_CUDA(ix->held_queries.ensure(want));
+        }
+        held = reinterpret_cast<float*>(static_cast<char*>(ix->held_queries.p) + ix->held_used);
+        held_end = ix->held_used + q_bytes;
+    }
+
     const int64_t* d_subset = nullptr;
     const float* d_queries = nullptr;
-    if (int rc = stage_inputs(ix, ts, timing, queries, n_queries, q_dev, o_dev, subset, subset_len, &d_queries, &d_subset, s))
+    if (int rc = stage_inputs(ix, ts, timing, queries, n_queries, q_dev, o_dev, subset, subset_len, &d_queries, &d_subset, s,
+                              held))
         return rc;
 
     if (use_split) {
@@ -1527,11 +1563,12 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             Pending p{m.queries, nq, k, min_score, item_offset, m.out_items, m.out_scores, m.out_counts, slot,
                       use_split, d_mask != nullptr};
             ix->pending.push_back(p);
+            ix->held_used = std::max(ix->held_used, held_end);  // (a finish_pending above may have reset it)
         }
         // Queries the sampled admission threshold could not settle (fewer than k admitted rows
         // although rows were cut, or candidate overflow) are redone exactly by the row scan —
         // now, or in tav_finish_search when the caller defers the (synchronising) check.
-        if (!((flags & TAV_DEFER_RETRY) && o_dev && q_dev)) {
+        if (!defer) {
             int redone = 0;
             if (int rc = finish_pending(ix, s, &redone)) return rc;
         }
@@ -1699,13 +1736,13 @@ int tav_mma_scores(tav_index* ix, const float* queries, int n_queries, int flags
     }
     if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const float* d_queries = queries;
-    if (!(flags & TAV_QUERIES_ON_DEVICE)) {
-        const size_t q_bytes = static_cast<size_t>(n_queries) * ix->dim * sizeof(float);
-        TAV_CUDA(ix->queries.ensure(q_bytes));
-        TAV_CUDA(cudaMemcpyAsync(ix->queries.p, queries, q_bytes, cudaMemcpyHostToDevice, s));
-        d_queries = static_cast<const float*>(ix->queries.p);
-    }
+    // staged as a search stages them: normalised on a TAV_NORMALIZE index, so these are the search's dots
+    TimedSearch not_timed;
+    const float* d_queries = nullptr;
+    const int64_t* no_subset = nullptr;
+    if (int rc = stage_inputs(ix, &not_timed, false, queries, n_queries, flags & TAV_QUERIES_ON_DEVICE, false, nullptr, 0,
+                              &d_queries, &no_subset, s))
+        return rc;
     if (split)
         if (int rc = ensure_split_planes(ix, nullptr, s)) return rc;
     MmaArgs m{};

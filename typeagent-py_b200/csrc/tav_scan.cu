@@ -849,20 +849,32 @@ __global__ void __launch_bounds__(256) convert_rows_kernel(const S* src, D* dst,
         const S* s = src + row * dim;
         D* d = dst + row * dim;
         float inv = 1.0f;
+        int shift = 0;
         if (normalize) {
+            // Scale by 2^-shift, the power of two of the largest magnitude, so that the sum of squares of
+            // the scaled row lies in [1/4, dim] whatever the row's scale: without it rows below ~1e-19
+            // underflow to a zero or subnormal sum and rows above ~1e19 overflow it.  The scaling is exact,
+            // so rows whose squares stay in the normal range get the same bits as unscaled arithmetic.
+            // fmaxf skips NaN; an infinite maximum leaves the row unscaled (its quotients are then NaN or 0).
+            float amax = 0.0f;
+            for (int c = lane; c < dim; c += 32) amax = fmaxf(amax, fabsf(to_float(s[c])));
+#pragma unroll
+            for (int off = 16; off >= 1; off >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xFFFFFFFFu, amax, off));
+            if (amax > 0.0f && isfinite(amax)) frexpf(amax, &shift);
             float ss = 0.0f;
             for (int c = lane; c < dim; c += 32) {
-                const float v = to_float(s[c]);
+                const float v = ldexpf(to_float(s[c]), -shift);
                 ss = fmaf(v, v, ss);
             }
 #pragma unroll
             for (int off = 16; off >= 1; off >>= 1) ss += __shfl_xor_sync(0xFFFFFFFFu, ss, off);
             const float nrm = sqrtf(ss);
             inv = nrm > 0.0f ? nrm : 1.0f;  // the divisor; zero rows stay zero (model_adapters.py:182)
+            if (!(nrm > 0.0f)) shift = 0;   // zero rows and rows with a NaN are stored as they are
         }
         for (int c = lane; c < dim; c += 32) {
             float v = to_float(s[c]);
-            if (normalize) v = v / inv;
+            if (normalize) v = ldexpf(v, -shift) / inv;
             d[c] = convert_elem<float, D>(v);
         }
     }
