@@ -22,7 +22,14 @@
  * caller's stream (`stream`, a cudaStream_t passed as void*; NULL = the CUDA legacy default
  * stream, as everywhere in the CUDA runtime).  Entry points that take host output pointers
  * synchronise that stream before returning; with TAV_OUTPUTS_ON_DEVICE they return as soon
- * as the work is enqueued, ordered after earlier work on the same stream.
+ * as the work is enqueued.
+ * The device work of the calls on one index runs in the order the calls were made, whatever
+ * stream each call names: a call on another stream than the previous call's first makes its
+ * stream wait (cudaStreamWaitEvent) for the work of the calls before it, and the calls without
+ * a stream (tav_clear, tav_adopt_device, tav_reserve) wait for it on the host.  Consecutive
+ * calls on one stream add no CUDA call for this.  Hazards in the caller's own buffers stay the
+ * caller's: queries or a device row mask written on stream X and passed with stream Y, or
+ * outputs read on another stream than the search's.
  */
 #ifndef TAVEC_H
 #define TAVEC_H
@@ -164,8 +171,9 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
 int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items, float* out_scores,
                     int flags, void* stream);
 
-/* Completes EVERY outstanding TAV_DEFER_RETRY search of the index: synchronises `stream`, redoes
- * each search's flagged queries exactly into that search's own outputs and reports how many
+/* Completes EVERY outstanding TAV_DEFER_RETRY search of the index, whatever stream each was issued
+ * on: waits until they have run (`stream` first waits for them, then is synchronised), redoes
+ * each search's flagged queries exactly on `stream` into that search's own outputs and reports how many
  * (*redone).  The caller keeps the query and output buffers of deferred searches alive until
  * then.  Up to 64 searches may be outstanding (a 65th finishes the earlier ones first, and the
  * queries redone then are not counted in *redone).  On a TAV_NORMALIZE index each outstanding

@@ -182,7 +182,12 @@ struct tav_index {
     DevBuf range_mmaws, range_mmaws2, range_mmaaux;  // tensor-core collection: workspaces, scratch
     DevBuf range_items, range_scores;
     int64_t range_total = 0;     // hits of the last range search held in range_items / range_scores
-    cudaEvent_t ev_range = nullptr;  // end of the last range search (tav_range_fetch waits for it)
+
+    // call order on the device (join_stream / mark_queued / wait_queued): ev_last marks the end of the work
+    // of the calls so far while `outstanding`; last_stream is ordered after it
+    cudaEvent_t ev_last = nullptr;
+    cudaStream_t last_stream = nullptr;
+    bool outstanding = false;
 
     // timing
     TimedSearch* hist = nullptr; // [kHistory], created by tav_set_timing(1)
@@ -213,6 +218,33 @@ static cudaError_t pin_in_acquire(tav_index* ix, size_t bytes) {
 
 static int set_device(const tav_index* ix) {
     TAV_CUDA(cudaSetDevice(ix->device));
+    return TAV_OK;
+}
+
+// The device work of the calls on one index runs in the order of the calls, whatever stream each names.
+// A call that may return with work still queued records ev_last behind it (mark_queued); a call that
+// synchronises its stream after joining it leaves nothing queued (mark_done).  On entry a call on another
+// stream makes that stream wait for ev_last (an event, not the earlier stream: that one may be gone by now);
+// consecutive calls on one stream issue no CUDA call for this.
+static int join_stream(tav_index* ix, cudaStream_t s) {
+    if (ix->outstanding && s != ix->last_stream) TAV_CUDA(cudaStreamWaitEvent(s, ix->ev_last, 0));
+    ix->last_stream = s;  // whatever is enqueued on s from here on runs after ev_last
+    return TAV_OK;
+}
+
+static int mark_queued(tav_index* ix, cudaStream_t s) {
+    TAV_CUDA(cudaEventRecord(ix->ev_last, s));
+    ix->last_stream = s;
+    ix->outstanding = true;
+    return TAV_OK;
+}
+
+static void mark_done(tav_index* ix) { ix->outstanding = false; }
+
+// the entry points without a stream (clear, adopt, reserve): the host waits for the earlier calls' work
+static int wait_queued(tav_index* ix) {
+    if (ix->outstanding) TAV_CUDA(cudaEventSynchronize(ix->ev_last));
+    ix->outstanding = false;
     return TAV_OK;
 }
 
@@ -275,6 +307,7 @@ int tav_create(int device, int dim, int store_dtype, int index_flags, int64_t re
     ix->dtype = store_dtype;
     ix->flags = index_flags;
     cudaError_t ce = cudaEventCreateWithFlags(&ix->ev_pin_in, cudaEventDisableTiming);
+    if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&ix->ev_last, cudaEventDisableTiming);
     for (int i = 0; ce == cudaSuccess && i < 2; ++i)
         ce = cudaEventCreateWithFlags(&ix->ev_append[i], cudaEventDisableTiming);
     if (ce != cudaSuccess) {
@@ -306,7 +339,7 @@ int tav_destroy(tav_index* ix) {
                       &ix->range_mmaws2, &ix->range_mmaaux})
         b->release();
     for (DevBuf& b : ix->held_retired) b.release();
-    if (ix->ev_range) cudaEventDestroy(ix->ev_range);
+    if (ix->ev_last) cudaEventDestroy(ix->ev_last);
     ix->pin_in.release();
     ix->pin_out.release();
     ix->retry_host.release();
@@ -322,22 +355,23 @@ int tav_destroy(tav_index* ix) {
 int tav_clear(tav_index* ix) {
     if (!ix) return TAV_ERR_INVALID;
     std::lock_guard<std::mutex> lock(ix->mu);
+    // queued searches read the rows (or the adopted memory) that later appends overwrite
+    if (int rc = set_device(ix)) return rc;
+    if (int rc = wait_queued(ix)) return rc;
     if (ix->adopted) {
         ix->rows = nullptr;
         ix->adopted = false;
         ix->capacity = 0;
     }
     ix->size = 0;
+    // (the "a corpus value left the fp16 range" flag is reset where the planes are rebuilt from row 0)
     ix->split_rows = 0;
     ix->row_mask_rows = 0;
-    if (ix->split_flag.p) {  // the sticky "a corpus value left the fp16 range" flag dies with the rows
-        cudaSetDevice(ix->device);
-        cudaMemset(ix->split_flag.p, 0, sizeof(int));
-    }
     return TAV_OK;
 }
 
-static int reserve_locked(tav_index* ix, int64_t rows) {
+// the caller has joined `s` (or waited for the earlier calls' work): the copy reads complete rows
+static int reserve_locked(tav_index* ix, int64_t rows, cudaStream_t s) {
     if (ix->adopted) {
         set_error("tav_reserve: index uses adopted device memory");
         return TAV_ERR_STATE;
@@ -352,9 +386,9 @@ static int reserve_locked(tav_index* ix, int64_t rows) {
     void* fresh = nullptr;
     TAV_CUDA(cudaMalloc(&fresh, std::max<size_t>(static_cast<size_t>(rows) * row_bytes, 256)));
     if (ix->size > 0) {
-        // in-order with whatever was enqueued on the index stream; then make it visible to all
-        cudaError_t e = cudaMemcpy(fresh, ix->rows, static_cast<size_t>(ix->size) * row_bytes,
-                                   cudaMemcpyDeviceToDevice);
+        cudaError_t e = cudaMemcpyAsync(fresh, ix->rows, static_cast<size_t>(ix->size) * row_bytes,
+                                        cudaMemcpyDeviceToDevice, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
         if (e != cudaSuccess) {
             cudaFree(fresh);
             set_error("tav_reserve: copy failed: %s", cudaGetErrorString(e));
@@ -373,7 +407,11 @@ static int reserve_locked(tav_index* ix, int64_t rows) {
 int tav_reserve(tav_index* ix, int64_t rows) {
     if (!ix || rows < 0) return TAV_ERR_INVALID;
     std::lock_guard<std::mutex> lock(ix->mu);
-    return reserve_locked(ix, rows);
+    if (rows > ix->capacity && !ix->adopted) {  // the copy must see every queued append
+        if (int rc = set_device(ix)) return rc;
+        if (int rc = wait_queued(ix)) return rc;
+    }
+    return reserve_locked(ix, rows, nullptr);
 }
 
 int tav_append(tav_index* ix, const void* rows, int64_t n, int dim, int src_dtype,
@@ -395,11 +433,13 @@ int tav_append(tav_index* ix, const void* rows, int64_t n, int dim, int src_dtyp
     if (n == 0) return TAV_OK;
     if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;
     if (ix->size + n > ix->capacity) {
         int64_t want = std::max<int64_t>(ix->size + n, ix->capacity * 2);
         want = std::max<int64_t>(want, 1024);
         TAV_CUDA(cudaStreamSynchronize(s));
-        if (int rc = reserve_locked(ix, want)) return rc;
+        mark_done(ix);
+        if (int rc = reserve_locked(ix, want, s)) return rc;
     }
     const size_t dst_row = static_cast<size_t>(ix->dim) * dtype_size(ix->dtype);
     const size_t src_row = static_cast<size_t>(ix->dim) * dtype_size(src_dtype);
@@ -442,7 +482,7 @@ int tav_append(tav_index* ix, const void* rows, int64_t n, int dim, int src_dtyp
         // re-acquired through their events, so no synchronisation is needed here
     }
     ix->size += n;
-    return TAV_OK;
+    return mark_queued(ix, s);
 }
 
 int tav_adopt_device(tav_index* ix, void* device_rows, int64_t n, int dim) {
@@ -460,15 +500,15 @@ int tav_adopt_device(tav_index* ix, void* device_rows, int64_t n, int dim) {
         set_error("tav_adopt_device: pointer must be 16-byte aligned");
         return TAV_ERR_INVALID;
     }
-    cudaSetDevice(ix->device);
+    if (int rc = set_device(ix)) return rc;
+    if (int rc = wait_queued(ix)) return rc;  // queued searches read the rows replaced here
     if (ix->rows && !ix->adopted) {
         cudaDeviceSynchronize();
         cudaFree(ix->rows);
     }
     ix->dim = dim;
     ix->rows = device_rows;
-    ix->split_rows = 0;
-    if (ix->split_flag.p) cudaMemset(ix->split_flag.p, 0, sizeof(int));
+    ix->split_rows = 0;  // (the planes' overflow flag is reset where they are rebuilt from row 0)
     ix->row_mask_rows = 0;
     ix->adopted = true;
     ix->size = n;
@@ -492,6 +532,7 @@ int tav_read_rows(tav_index* ix, int64_t first, int64_t n, float* out_host, void
     if (n == 0) return TAV_OK;
     if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;
     const size_t row = static_cast<size_t>(ix->dim) * dtype_size(ix->dtype);
     const char* src = static_cast<const char*>(ix->rows) + static_cast<size_t>(first) * row;
     if (ix->dtype == TAV_F32) {
@@ -503,6 +544,7 @@ int tav_read_rows(tav_index* ix, int64_t first, int64_t n, float* out_host, void
         TAV_CUDA(cudaMemcpyAsync(out_host, ix->staging.p, bytes, cudaMemcpyDeviceToHost, s));
     }
     TAV_CUDA(cudaStreamSynchronize(s));
+    mark_done(ix);
     return TAV_OK;
 }
 
@@ -511,6 +553,7 @@ int tav_set_row_mask(tav_index* ix, const uint32_t* bits, int64_t n_rows, int on
     std::lock_guard<std::mutex> lock(ix->mu);
     if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;  // queued searches read the old mask
     if (!ix->pending.empty()) {  // an outstanding search may still need the old mask for its exact redo
         int redone = 0;
         if (int rc = finish_pending(ix, s, &redone)) return rc;
@@ -530,8 +573,10 @@ int tav_set_row_mask(tav_index* ix, const uint32_t* bits, int64_t n_rows, int on
     TAV_CUDA(cudaMemsetAsync(ix->row_mask.p, 0, words * sizeof(uint32_t), s));
     TAV_CUDA(cudaMemcpyAsync(ix->row_mask.p, bits, src_words * sizeof(uint32_t),
                              on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
-    if (!on_device) TAV_CUDA(cudaStreamSynchronize(s));
     ix->row_mask_rows = n_rows;
+    if (on_device) return mark_queued(ix, s);
+    TAV_CUDA(cudaStreamSynchronize(s));
+    mark_done(ix);
     return TAV_OK;
 }
 
@@ -695,6 +740,7 @@ static inline int32_t* retry_flags(tav_index* ix, int slot) {
 static int finish_pending(tav_index* ix, cudaStream_t s, int* redone) {
     if (redone) *redone = 0;
     if (ix->pending.empty()) return TAV_OK;
+    if (int rc = join_stream(ix, s)) return rc;  // the searches may have been issued on other streams
     int32_t totals[2 * kMaxPending];
     int corpus_overflow = 0;
     bool any_split = false;
@@ -733,9 +779,10 @@ static int finish_pending(tav_index* ix, cudaStream_t s, int* redone) {
     if (dirty) TAV_CUDA(cudaMemsetAsync(ix->retry.p, 0, sizeof(totals), s));
     if (dirty || n_redone > 0) TAV_CUDA(cudaStreamSynchronize(s));
     if (dirty) memset(ix->retry_host.p, 0, sizeof(totals));
+    mark_done(ix);
     // No queued work reads a held query region now, whatever stream a later search uses: the searches ended
-    // at the first synchronisation above, their redo scans at the last.  So the regions can be reused and the
-    // outgrown buffers freed.
+    // at the first synchronisation above (s joined the stream of the last call first), their redo scans at the
+    // last.  So the regions can be reused and the outgrown buffers freed.
     ix->held_used = 0;
     for (DevBuf& b : ix->held_retired) b.release();
     ix->held_retired.clear();
@@ -1150,13 +1197,6 @@ static int range_core(tav_index* ix, TimedSearch* ts, bool timing, const float* 
                               expected_hits, offsets, s);
 }
 
-// the hits of the last threshold search are complete once this event has passed (tav_range_fetch waits)
-static int range_mark_end(tav_index* ix, cudaStream_t s) {
-    if (!ix->ev_range) TAV_CUDA(cudaEventCreateWithFlags(&ix->ev_range, cudaEventDisableTiming));
-    TAV_CUDA(cudaEventRecord(ix->ev_range, s));
-    return TAV_OK;
-}
-
 extern "C" {
 
 const int32_t* tav_internal_retry_totals(tav_index* ix, int* count) {
@@ -1190,6 +1230,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     std::lock_guard<std::mutex> lock(ix->mu);
     if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;
     const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
     const size_t nk = static_cast<size_t>(n_queries) * k;
     const uint32_t* d_mask = nullptr;
@@ -1233,8 +1274,11 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     // a NaN min_score admits nothing on every path (`scores >= nan` is all-false in the reference)
     if (n_scan == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score) {
         // empty corpus / empty subset: no hits (vectorbase.py:174-175, :214-215)
-        if (o_dev) TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(n_queries) * sizeof(int32_t), s));
-        else memset(out_counts, 0, static_cast<size_t>(n_queries) * sizeof(int32_t));
+        if (o_dev) {
+            TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(n_queries) * sizeof(int32_t), s));
+            return mark_queued(ix, s);
+        }
+        memset(out_counts, 0, static_cast<size_t>(n_queries) * sizeof(int32_t));
         return TAV_OK;
     }
     if (n_scan > 0xFFFFFFFFll) {
@@ -1286,7 +1330,6 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         }
         ts->valid = true;
         ix->range_total = offsets[n_queries];
-        if (int rc = range_mark_end(ix, s)) return rc;
         // each query's hits straight into its row of the caller's arrays (copies from device memory into
         // pageable memory return when done), then the padding
         for (int q = 0; q < n_queries; ++q) {
@@ -1301,6 +1344,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             }
         }
         TAV_CUDA(cudaStreamSynchronize(s));
+        mark_done(ix);
         for (int q = 0; q < n_queries; ++q) {
             const int64_t c = offsets[q + 1] - offsets[q];
             std::fill(out_items + static_cast<size_t>(q) * k + c, out_items + static_cast<size_t>(q + 1) * k, int64_t(-1));
@@ -1430,6 +1474,9 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             if ((spin & 0x3FFF) == 0x3FFF && cudaStreamQuery(s) != cudaErrorNotReady) break;
         }
         if (!seen) TAV_CUDA(cudaStreamSynchronize(s));
+        // the kernel started after the earlier calls' work (join_stream) and has written its hits: nothing of
+        // this index is left queued (only its last CTA's counter reset may still be retiring)
+        mark_done(ix);
         std::atomic_thread_fence(std::memory_order_acquire);  // the copies below read what the spin saw
         if (trace_host) {
             timespec tsn;
@@ -1584,13 +1631,14 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     }
     ts->valid = true;
 
+    if (o_dev) return mark_queued(ix, s);
     if (zero_copy_out) {
         TAV_CUDA(cudaStreamSynchronize(s));
         const char* h = static_cast<const char*>(ix->pin_out.p);
         memcpy(out_items, h, nk * sizeof(int64_t));
         memcpy(out_scores, h + off_scores, nk * sizeof(float));
         memcpy(out_counts, h + off_counts, static_cast<size_t>(n_queries) * sizeof(int32_t));
-    } else if (!o_dev) {
+    } else {
         if (pack_bytes <= kPinnedStageLimit) {
             TAV_CUDA(ix->pin_out.ensure(pack_bytes));
             TAV_CUDA(cudaMemcpyAsync(ix->pin_out.p, ix->out_pack.p, off_done, cudaMemcpyDeviceToHost, s));
@@ -1607,6 +1655,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             TAV_CUDA(cudaStreamSynchronize(s));
         }
     }
+    mark_done(ix);  // host outputs: s was synchronised above
     return TAV_OK;
 }
 
@@ -1628,6 +1677,7 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
     std::lock_guard<std::mutex> lock(ix->mu);
     if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;  // (also: a queued tav_range_fetch reads the hits replaced here)
     const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
     ix->range_total = 0;
     std::vector<int64_t> offsets(static_cast<size_t>(n_queries) + 1, 0);
@@ -1638,7 +1688,7 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
         } else {
             memcpy(out_offsets, offsets.data(), bytes);
         }
-        return range_mark_end(ix, s);
+        return mark_queued(ix, s);  // the sort after the last synchronisation may still run
     };
     const uint32_t* d_mask = nullptr;
     if (flags & TAV_USE_ROW_MASK) {
@@ -1715,13 +1765,15 @@ int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items,
     if (n == 0) return TAV_OK;
     if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (ix->ev_range) TAV_CUDA(cudaStreamWaitEvent(s, ix->ev_range, 0));
+    if (int rc = join_stream(ix, s)) return rc;  // after the range search that wrote the hits
     const cudaMemcpyKind kind = (flags & TAV_OUTPUTS_ON_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     TAV_CUDA(cudaMemcpyAsync(out_items, static_cast<const int64_t*>(ix->range_items.p) + first,
                              static_cast<size_t>(n) * sizeof(int64_t), kind, s));
     TAV_CUDA(cudaMemcpyAsync(out_scores, static_cast<const float*>(ix->range_scores.p) + first,
                              static_cast<size_t>(n) * sizeof(float), kind, s));
-    if (!(flags & TAV_OUTPUTS_ON_DEVICE)) TAV_CUDA(cudaStreamSynchronize(s));
+    if (flags & TAV_OUTPUTS_ON_DEVICE) return mark_queued(ix, s);
+    TAV_CUDA(cudaStreamSynchronize(s));
+    mark_done(ix);
     return TAV_OK;
 }
 
@@ -1736,6 +1788,7 @@ int tav_mma_scores(tav_index* ix, const float* queries, int n_queries, int flags
     }
     if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;
     // staged as a search stages them: normalised on a TAV_NORMALIZE index, so these are the search's dots
     TimedSearch not_timed;
     const float* d_queries = nullptr;
@@ -1765,6 +1818,7 @@ int tav_mma_scores(tav_index* ix, const float* queries, int n_queries, int flags
     }
     TAV_CUDA(launch_mma_dump(m, ix->mma_ws.p, ix->mma_ws.bytes, out_device, s));
     TAV_CUDA(cudaStreamSynchronize(s));
+    mark_done(ix);
     return TAV_OK;
 }
 
