@@ -204,6 +204,29 @@ int tav_merge_topk(int device, int n_lists, int n_queries, int k, const int64_t*
                    float* out_scores, int32_t* out_counts, void* stream);
 
 /*
+ * Merge step of the row-sharded threshold search: `n_lists` per-shard CSR results of tav_range_search
+ * (items already global: item_offset = the shard's first row) -> every hit of every list, per query, in
+ * the library's order (score descending, then item descending, or ascending with ties_low_first).  List g:
+ *   offsets + g * offsets_stride   [n_queries + 1] int64, starting at 0: query q's hits are
+ *   items   + g * items_stride     [offsets[q], offsets[q + 1])  int64
+ *   scores  + g * scores_stride                                  float32
+ * (strides in elements), so one padded all-gather buffer is merged in place.  Each list must already be
+ * in the library's order; items are compared as int64 and must be distinct across lists for the result
+ * not to depend on the list order.  Scores are compared as float32 values (tav_range_search's are in
+ * [0, 1]); they must not be NaN.  Outputs: out_offsets [n_queries + 1] = the per-query sums of the
+ * lists' offsets, out_items / out_scores [out_offsets[n_queries]].  A merge (co-rank tiles spread evenly
+ * over the GPU whatever the queries' sizes, each input hit read once), not a sort; no synchronisation
+ * (8 * (n_queries + 1) bytes of stream-ordered scratch, cudaMallocAsync).  All pointers are device
+ * pointers on `device` and must be non-NULL when n_queries > 0 (the counts live on the device);
+ * 1 <= n_lists <= 32; negative strides are invalid; n_queries == 0 does nothing.  Lists with no hits
+ * are normal input.
+ */
+int tav_merge_range(int device, int n_lists, int n_queries, const int64_t* offsets, int64_t offsets_stride,
+                    const int64_t* items, int64_t items_stride, const float* scores, int64_t scores_stride,
+                    int ties_low_first, int64_t* out_offsets, int64_t* out_items, float* out_scores,
+                    void* stream);
+
+/*
  * Row-sharded search across the GPUs of one box, one process per GPU (SURVEY.md §8e).  A group is
  * this rank's end of the candidate exchange: an "exchange region" in its HBM which the peers map
  * through a CUDA IPC handle.  Create it on every rank with the same arguments, exchange the handles

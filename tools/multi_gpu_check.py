@@ -8,7 +8,9 @@ Every rank builds the same seeded corpus on the host, keeps its own row block on
 (ShardedVectorBase), and checks that the sharded lookup — local search, candidate exchange (libtavec's
 peer-memory publish/merge over NVLink, and the NCCL all-gather form), merge kernel — is BIT-IDENTICAL to
 the single-GPU lookup over the whole corpus on that rank's GPU, for the float32 row-scan path, the
-float32 split form and the bf16 / fp16 tensor-core paths, and agrees with the CPU oracle.
+float32 split form and the bf16 / fp16 tensor-core paths, and agrees with the CPU oracle.  The sharded
+threshold search (``search_range``: offsets and hits all-gathered, ``tav_merge_range``) must equal the
+single-GPU ``search_range`` bit for bit on every rank: float32 row scan, bf16 tensor cores, float32 split form.
 """
 import os
 import sys
@@ -94,6 +96,26 @@ def main():
         if rank == 0:
             print(f"multi-gpu ok: world={world} exact fallback through finish(), one and three outstanding, "
                   f"exchange={exchange}", flush=True)
+    # threshold search (search_range: offsets + hits all-gathered, tav_merge_range): bit-identical to the single-GPU
+    # search_range over the whole corpus, at sizes where every rank takes the same path as the whole-corpus search
+    for storage, n, d, b, ms, path in (("float32", 70001, 96, 5, 0.55, "scan"),
+                                       ("bfloat16", 160001, 128, 32, 0.6, "mma"),
+                                       ("float32", 90001, 64, 20, 0.58, "mma_split")):
+        v, q = O.make_corpus(n, d, seed=n + 1, n_queries=b)
+        sh = ShardedVectorBase(settings, device=local, storage_dtype=storage)
+        sh.deserialize(v)
+        whole = tab.VectorBase(settings, device=local, storage_dtype=storage)
+        whole.add_embeddings(None, v)
+        got = sh.search_range(q, ms)
+        want = whole.search_range(q, ms)
+        assert whole.last_timing()["path"] == path and sh._engine.base.last_timing()["path"] == path
+        np.testing.assert_array_equal(got[0], want[0])
+        np.testing.assert_array_equal(got[1], want[1])
+        np.testing.assert_array_equal(got[2].view(np.uint32), want[2].view(np.uint32))
+        dist.barrier()
+        if rank == 0:
+            print(f"multi-gpu ok: world={world} search_range {storage} n={n} d={d} b={b} min_score={ms} path={path} "
+                  f"hits={int(want[0][-1])}", flush=True)
     dist.destroy_process_group()
 
 

@@ -66,6 +66,8 @@ SIGNATURES = {
     "tav_merge_topk": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_int64, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tav_merge_range": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                  C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tav_mma_scores": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "tav_set_timing": (C.c_int, [C.c_void_p, C.c_int]),
     "tav_timing_breakdown": (C.c_int, [C.c_void_p, _f32p, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]),

@@ -17,6 +17,10 @@ Two exchanges:
   * ``exchange="nccl"``: ONE ``all_gather_into_tensor`` + ``tav_merge_topk`` (also what the CPU tests
     drive over ``gloo`` with an injected engine).
 
+Threshold searches (``search_range``; ``max_hits=0`` lookups and ``search_arrays`` with k >= rows > 8192) have
+results whose size is known only after the local searches: they exchange over the process group (offsets, then
+the hits padded to the largest rank's total) and merge with ``tav_merge_range``.
+
 ``torch`` is plumbing here (process group, device buffers); the search, exchange and merge are
 libtavec kernels.  The engine is injectable so that the host logic (partitioning, packing, gather,
 offsets) is testable on CPU with the ``gloo`` backend.
@@ -29,7 +33,9 @@ import ctypes as C
 import numpy as np
 
 from . import _capi
-from .vectorbase import ScoredInt, TextEmbeddingIndexSettings, VectorBase
+from .vectorbase import ScoredInt, TextEmbeddingIndexSettings, VectorBase, _as_f32_scalar
+
+RANGE_ROUTE_MIN_ROWS = 4 * 2048  # search_arrays with k >= rows above this (4 * TAV_PASS_K) -> search_range
 
 
 def shard_bounds(n_rows: int, world: int) -> list[tuple[int, int]]:
@@ -186,6 +192,110 @@ class CudaShardEngine:
                                C.c_void_p(counts.data_ptr()), C.c_void_p(stream))
         )
         return items, scores, counts
+
+    # ---- threshold search (search_range) ---------------------------------------------------
+    def range_local(self, queries: np.ndarray, min_score: float, item_offset: int, ties_low_first: bool):
+        """``tav_range_search`` on this rank's rows (items shifted by ``item_offset``).  Returns a
+        ``LocalRange``: host offsets [B + 1] now, the hits later straight into the caller's buffers.  The
+        hits wait in the index between the two calls, so the base's lookup lock is held until then."""
+        base = self.base
+        b = len(queries)
+        if self.n_local() == 0:
+            return LocalRange(np.zeros(b + 1, np.int64), None, None)
+        q = base._check_queries(queries)
+        base._single_lock.acquire()
+        try:
+            lib, ix = base._ensure_device()
+            flags = base._flags() & ~_capi.TAV_NO_FUSED_SCAN
+            if ties_low_first:
+                flags |= _capi.TAV_TIES_LOW_FIRST
+            offsets = np.zeros(b + 1, np.int64)
+            _capi.check(lib.tav_range_search(ix, q.ctypes.data_as(C.c_void_p), b, C.c_float(min_score), flags, None, 0,
+                                             item_offset, base._range_hint, offsets.ctypes.data_as(C.c_void_p), None))
+            base._range_hint = int(offsets[-1])
+        except BaseException:
+            base._single_lock.release()
+            raise
+        stream = self.torch.cuda.current_stream(self.device).cuda_stream
+
+        def fetch(items, scores):
+            n = int(offsets[-1])
+            if n == 0:
+                return
+            on_device = not isinstance(items, np.ndarray)
+            ip = C.c_void_p(items.data_ptr()) if on_device else items.ctypes.data_as(C.c_void_p)
+            sp = C.c_void_p(scores.data_ptr()) if on_device else scores.ctypes.data_as(C.c_void_p)
+            _capi.check(lib.tav_range_fetch(ix, 0, n, ip, sp, _capi.TAV_OUTPUTS_ON_DEVICE if on_device else 0,
+                                            C.c_void_p(stream) if on_device else None))
+
+        return LocalRange(offsets, fetch, base._single_lock)
+
+    def merge_range(self, offsets_all, payload, world: int, n_queries: int, t_pad: int, total: int,
+                    ties_low_first: bool):
+        """``tav_merge_range`` over the all-gathered lists: ``offsets_all`` int64 [world, B + 2] (offsets and a
+        status word per rank), ``payload`` uint8 [world, 12 * t_pad] (items int64 [t_pad], then scores float32
+        [t_pad]) -> (offsets int64 [B + 1], items int64 [total], scores float32 [total]) device tensors."""
+        torch = self.torch
+        out_offsets = torch.empty(n_queries + 1, dtype=torch.int64, device=self.device)
+        items = torch.empty(max(total, 1), dtype=torch.int64, device=self.device)
+        scores = torch.empty(max(total, 1), dtype=torch.float32, device=self.device)
+        base = payload.data_ptr()
+        stream = self.torch.cuda.current_stream(self.device).cuda_stream
+        _capi.check(_capi.load().tav_merge_range(
+            self.device.index, world, n_queries, C.c_void_p(offsets_all.data_ptr()), offsets_all.shape[1],
+            C.c_void_p(base), 12 * t_pad // 8, C.c_void_p(base + 8 * t_pad), 12 * t_pad // 4, int(ties_low_first),
+            C.c_void_p(out_offsets.data_ptr()), C.c_void_p(items.data_ptr()), C.c_void_p(scores.data_ptr()),
+            C.c_void_p(stream)))
+        return out_offsets, items[:total], scores[:total]
+
+
+MAX_RANGE_RANKS = 32  # lists tav_merge_range merges in one call
+
+
+def offsets_with_status(offsets: np.ndarray, failed: bool) -> np.ndarray:
+    """One rank's first exchange of a threshold search: its offsets [B + 1], then a status word (1 = failed)."""
+    return np.concatenate([np.asarray(offsets, np.int64), [int(failed)]]).astype(np.int64)
+
+
+def range_pad(totals) -> int:
+    """Hits per rank in the payload exchange: the largest rank's total, rounded up to even so that every rank's
+    scores section stays 8-byte aligned."""
+    t = int(np.max(totals))
+    return t + (t & 1)
+
+
+def pack_range_payload(local, t_pad: int, device):
+    """One rank's payload of the second exchange, uint8 [12 * t_pad]: items int64 [t_pad], then scores float32
+    [t_pad], the hits first; ``local.fetch`` writes them straight into it."""
+    import torch
+
+    send = torch.empty(12 * t_pad, dtype=torch.uint8, device=device)
+    n = int(local.offsets[-1])
+    local.fetch(send[: 8 * n].view(torch.int64), send[8 * t_pad: 8 * t_pad + 4 * n].view(torch.float32))
+    return send
+
+
+class LocalRange:
+    """One rank's threshold-search result between the search and the fetch of its hits: ``offsets`` (host
+    int64 [B + 1]); ``fetch(items, scores)`` writes the hits into the given buffers (device tensors or host
+    arrays) and releases ``lock``; ``release()`` releases it without fetching.  Exactly one of them is called."""
+
+    def __init__(self, offsets: np.ndarray, fetch, lock=None):
+        self.offsets = offsets
+        self._fetch = fetch
+        self._lock = lock
+
+    def fetch(self, items, scores) -> None:
+        try:
+            if self._fetch is not None:
+                self._fetch(items, scores)
+        finally:
+            self.release()
+
+    def release(self) -> None:
+        lock, self._lock = self._lock, None
+        if lock is not None:
+            lock.release()
 
 
 class ShardedVectorBase:
@@ -356,14 +466,107 @@ class ShardedVectorBase:
         if len(self) == 0 or np.isnan(np.float32(min_score)):
             return (np.full((len(q), 1), -1, np.int64), np.zeros((len(q), 1), np.float32),
                     np.zeros(len(q), np.int32))
+        n = len(self)
+        if k >= n > RANGE_ROUTE_MIN_ROWS and hasattr(self._engine, "range_local"):
+            # every passing row, as tav_search routes it on one GPU: one threshold search, laid out [B, n]
+            offsets, hits, hit_scores = self.search_range(q, min_score)
+            counts = np.diff(offsets).astype(np.int32)
+            items = np.full((len(q), n), -1, np.int64)
+            scores = np.zeros((len(q), n), np.float32)
+            cols = np.arange(len(hits)) - np.repeat(offsets[:-1], counts)
+            rows = np.repeat(np.arange(len(q)), counts)
+            items[rows, cols] = hits
+            scores[rows, cols] = hit_scores
+            return items, scores, counts
         items, scores, counts = self.search_tensors(q, k, min_score)
         return items.cpu().numpy(), scores.cpu().numpy(), counts.cpu().numpy()
+
+    def search_range(self, queries, min_score: float = 0.0, ties_low_first: bool = False):
+        """Threshold search over the whole corpus: EVERY row whose score is >= min_score, per query, as
+        ``VectorBase.search_range`` returns it on one GPU — CSR numpy arrays offsets int64 [B + 1], items int64
+        [T], scores float32 [T], in the library's order — replicated on every rank.  SPMD.
+
+        Each rank runs the threshold search on its rows; one all-gather carries every rank's offsets (and a
+        status word, so that a rank's failure raises on every rank instead of leaving the others in the next
+        collective), a second one every rank's hits, padded to the largest rank's total (after a one-word
+        all-reduce that makes a failure to stage them raise on every rank); ``tav_merge_range`` merges them on
+        every rank.  The exchanges go through the process group whatever ``exchange`` says.  At most
+        ``MAX_RANGE_RANKS`` (32) ranks: larger groups get ValueError on every rank before any exchange."""
+        import torch
+
+        q = np.ascontiguousarray(queries, dtype=np.float32)
+        if q.ndim == 1:
+            q = q.reshape(1, -1)
+        b = len(q)
+        floor = _as_f32_scalar(min_score)
+        empty = (np.zeros(b + 1, np.int64), np.empty(0, np.int64), np.empty(0, np.float32))
+        # early returns on replicated state only: every rank takes them together
+        if b == 0 or len(self) == 0 or np.isnan(floor):
+            return empty
+        if q.shape[1] != self._embedding_size:
+            raise ValueError("query width does not match the embedding size")
+        if self.world > MAX_RANGE_RANKS:
+            raise ValueError(f"search_range merges at most {MAX_RANGE_RANKS} ranks (tav_merge_range), not {self.world}")
+        lo, _ = self.local_range
+        error, local = None, None
+        try:
+            local = self._engine.range_local(q, float(floor), lo, bool(ties_low_first))
+            offsets = np.asarray(local.offsets, np.int64)
+        except Exception as e:  # noqa: BLE001
+            error, offsets = e, np.zeros(b + 1, np.int64)
+        if self.world == 1:
+            if error is not None:
+                raise error
+            total = int(offsets[-1])
+            items, scores = np.empty(total, np.int64), np.empty(total, np.float32)
+            local.fetch(items, scores)
+            return offsets.copy(), items, scores
+        try:
+            dev = self._engine.comm_device() if hasattr(self._engine, "comm_device") else torch.device("cpu")
+            # exchange 1: offsets [B + 1] and a status word per rank
+            mine = torch.from_numpy(offsets_with_status(offsets, error is not None)).to(dev)
+            flag = torch.zeros(1, dtype=torch.int64, device=dev)
+            offsets_all = torch.empty((self.world, b + 2), dtype=torch.int64, device=dev)
+            self._dist.all_gather_into_tensor(offsets_all.view(-1), mine, group=self._group)
+            host = offsets_all.cpu().numpy()
+            if host[:, -1].any():
+                raise error if error is not None else RuntimeError("search_range: another rank's threshold search failed")
+            totals = host[:, b]
+            total = int(totals.sum())
+            if total == 0:
+                return empty
+            # exchange 2: every rank's hits, padded to the largest total.  Staging them (two allocations and the
+            # fetch) can fail on one rank; the ranks agree on that first, so nobody waits in the all-gather alone
+            t_pad = range_pad(totals)
+            stage_error, send = None, None
+            try:
+                payload = torch.empty((self.world, 12 * t_pad), dtype=torch.uint8, device=dev)
+                send = pack_range_payload(local, t_pad, dev)
+            except Exception as e:  # noqa: BLE001
+                stage_error = e
+            flag.fill_(int(stage_error is not None))
+            self._dist.all_reduce(flag, group=self._group)
+            if int(flag.item()):
+                raise stage_error if stage_error is not None else RuntimeError(
+                    "search_range: another rank failed to stage its hits")
+            self._dist.all_gather_into_tensor(payload.view(-1), send, group=self._group)
+            out = self._engine.merge_range(offsets_all, payload, self.world, b, t_pad, total, bool(ties_low_first))
+            return tuple(np.asarray(t.cpu().numpy() if hasattr(t, "cpu") else t) for t in out)
+        finally:
+            if local is not None:
+                local.release()
 
     def fuzzy_lookup_embeddings(self, embeddings, max_hits=None, min_score=None):
         if min_score is None:
             min_score = 0.0
         if len(self) == 0:
             return [[] for _ in range(len(embeddings))]
+        if max_hits == 0 and hasattr(self._engine, "range_local"):
+            # every passing row (the reference's max_hits=0): CSR lists from the threshold search
+            offsets, items, scores = self.search_range(embeddings, min_score)
+            il, sl, ol = items.tolist(), scores.tolist(), offsets.tolist()
+            return [[ScoredInt(i, s) for i, s in zip(il[ol[b]:ol[b + 1]], sl[ol[b]:ol[b + 1]])]
+                    for b in range(len(ol) - 1)]
         k = VectorBase._resolve_k(max_hits, len(self))
         items, scores, counts = self.search_arrays(embeddings, k, min_score)
         il, sl, cl = items.tolist(), scores.tolist(), counts.tolist()
