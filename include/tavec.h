@@ -26,7 +26,9 @@
  * The device work of the calls on one index runs in the order the calls were made, whatever
  * stream each call names: a call on another stream than the previous call's first makes its
  * stream wait (cudaStreamWaitEvent) for the work of the calls before it, and the calls without
- * a stream (tav_clear, tav_adopt_device, tav_reserve) wait for it on the host.  Consecutive
+ * a stream (tav_clear, tav_adopt_device, tav_reserve) wait for it on the host.  So a search queued
+ * before tav_remove_rows / tav_write_rows sees the old rows and one queued after it the new ones,
+ * whatever streams they name.  Consecutive
  * calls on one stream add no CUDA call for this.  Hazards in the caller's own buffers stay the
  * caller's: queries or a device row mask written on stream X and passed with stream Y, or
  * outputs read on another stream than the search's.
@@ -123,6 +125,26 @@ int tav_device(const tav_index* ix);
 /* Read rows [first, first+n) back as float32 into host memory (storage -> f32 is exact). */
 int tav_read_rows(tav_index* ix, int64_t first, int64_t n, float* out_host, void* stream);
 
+/* Remove rows, as numpy.delete does: `ordinals` (host int64 [n]) may be negative (counted from the end),
+ * repeated (one row removed) and in any order.  The surviving rows keep their order: row r becomes row
+ * r - #{removed rows < r}.  Every search afterwards equals a search of a fresh index built from the
+ * surviving rows.  The rows move on the device (an order-preserving compaction of the rows after the first
+ * removed one, which are not written); nothing is re-uploaded.  The compaction runs in place, in
+ * ascending windows through a buffer of at most 256 MB (smaller when that does not fit).  Any
+ * ordinal out of range: TAV_ERR_RANGE and the index is
+ * unchanged.  Adopted memory: TAV_ERR_STATE.  The row mask is dropped (ordinals change meaning); the
+ * hits of the last threshold search are results and stay as they were.  Outstanding TAV_DEFER_RETRY
+ * searches are finished first (their exact redo reads the rows).  Synchronises `stream` when rows move. */
+int tav_remove_rows(tav_index* ix, const int64_t* ordinals, int64_t n, void* stream);
+
+/* Overwrite rows [first, first + n) in place with `n` rows of `dim` elements of `src_dtype` from host
+ * (src_on_device = 0) or device memory, converted exactly as tav_append converts (RNE; normalised on a
+ * TAV_NORMALIZE index; host sources through the same pinned double buffer).  first + n beyond tav_size():
+ * TAV_ERR_RANGE.  Adopted memory: TAV_ERR_STATE.  The row mask stays (ordinals keep their meaning).
+ * Outstanding TAV_DEFER_RETRY searches are finished first.  Does not synchronise. */
+int tav_write_rows(tav_index* ix, int64_t first, const void* rows, int64_t n, int dim, int src_dtype,
+                   int src_on_device, void* stream);
+
 /*
  * The hot path.  For each of `n_queries` query vectors (float32 [n_queries, dim]):
  *   x      = dot(row, query)                       float32 accumulate
@@ -183,7 +205,8 @@ int tav_finish_search(tav_index* ix, void* stream, int* redone);
 
 /* Row mask for TAV_USE_ROW_MASK: `n_rows` bits (bit r of word r/32 = row r allowed), host or
  * device memory; n_rows must equal tav_size().  Kept on the device until the rows change
- * (tav_clear / tav_adopt_device drop it; appends invalidate it) or n_rows == 0 clears it. */
+ * (tav_clear / tav_adopt_device / tav_remove_rows drop it; appends invalidate it) or n_rows == 0
+ * clears it.  tav_write_rows keeps it. */
 int tav_set_row_mask(tav_index* ix, const uint32_t* bits, int64_t n_rows, int on_device, void* stream);
 
 /*

@@ -43,6 +43,9 @@ SIGNATURES = {
     "tav_store_dtype": (C.c_int, [C.c_void_p]),
     "tav_device": (C.c_int, [C.c_void_p]),
     "tav_read_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "tav_remove_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "tav_write_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                 C.c_void_p]),
     "tav_search": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int,
                              C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                              C.c_void_p]),

@@ -174,6 +174,16 @@ struct tav_index {
     DevBuf split_hi, split_lo, split_flag;
     int64_t split_rows = 0;      // rows [0, split_rows) of the planes are current
     int64_t split_cap = 0;
+    // rows were removed or overwritten since the planes were built: the overflow flag may stand for rows that
+    // are gone, so the next build looks at it and rebuilds from row 0 (which resets it) when it is set
+    bool split_recheck = false;
+    // removal (tav_remove_rows): the device copy of the removed-row keys, the compaction policy and what the
+    // last removal did (tav_internal_compact_policy / _stats)
+    DevBuf compact_keys;
+    int compact_mode = 0;            // 0 the default (in place), 1 out of place, 2 in place
+    int64_t compact_scratch = 0;     // bytes of the in-place window buffer (0: kCompactScratchBytes)
+    int compact_path = 0;            // 0 nothing moved, 1 out of place, 2 in place
+    int64_t compact_windows = 0;
     // predicate pushdown: one bit per row (tav_set_row_mask)
     DevBuf row_mask;
     int64_t row_mask_rows = 0;   // 0 = no mask set
@@ -263,6 +273,53 @@ static void destroy_history(tav_index* ix) {
     ix->hist = nullptr;
 }
 
+// Rows [first, first + n) of the index <- n rows of src_dtype from host or device memory, converted to the
+// storage dtype as appends convert them (RNE, TAV_NORMALIZE); queued on s, which the caller has joined.
+static int store_rows(tav_index* ix, int64_t first, const void* rows, int64_t n, int src_dtype, int src_on_device,
+                      cudaStream_t s) {
+    const size_t dst_row = static_cast<size_t>(ix->dim) * dtype_size(ix->dtype);
+    const size_t src_row = static_cast<size_t>(ix->dim) * dtype_size(src_dtype);
+    char* dst = static_cast<char*>(ix->rows) + static_cast<size_t>(first) * dst_row;
+    const bool plain = (src_dtype == ix->dtype) && !(ix->flags & TAV_NORMALIZE);
+    const int norm = (ix->flags & TAV_NORMALIZE) ? 1 : 0;
+    if (src_on_device) {
+        if (plain)
+            TAV_CUDA(cudaMemcpyAsync(dst, rows, static_cast<size_t>(n) * src_row, cudaMemcpyDeviceToDevice, s));
+        else
+            TAV_CUDA(launch_convert(rows, src_dtype, dst, ix->dtype, n, ix->dim, norm, s));
+    } else {
+        // Host source (bulk load at open, storage/sqlite/messageindex.py:33-45; incremental appends):
+        // through a pinned double buffer, so that the H2D copies are truly asynchronous and the host
+        // memcpy of chunk i+1 overlaps the DMA (+ conversion kernel) of chunk i.
+        const int64_t chunk_rows = std::max<int64_t>(1, static_cast<int64_t>(kAppendStageBytes / src_row));
+        const size_t stage_bytes = static_cast<size_t>(std::min(n, chunk_rows)) * src_row;
+        if (!plain) TAV_CUDA(ix->staging.ensure(2 * stage_bytes));
+        int b = 0;
+        for (int64_t done = 0; done < n; done += chunk_rows, b ^= 1) {
+            const int64_t m = std::min(chunk_rows, n - done);
+            const size_t bytes = static_cast<size_t>(m) * src_row;
+            if (ix->append_busy[b]) {  // also across calls: the previous append may still be queued on its stream
+                TAV_CUDA(cudaEventSynchronize(ix->ev_append[b]));
+                ix->append_busy[b] = false;
+            }
+            TAV_CUDA(ix->pin_append[b].ensure(stage_bytes));
+            memcpy(ix->pin_append[b].p, static_cast<const char*>(rows) + done * src_row, bytes);
+            if (plain) {
+                TAV_CUDA(cudaMemcpyAsync(dst + done * dst_row, ix->pin_append[b].p, bytes, cudaMemcpyHostToDevice, s));
+            } else {
+                char* stage = static_cast<char*>(ix->staging.p) + static_cast<size_t>(b) * stage_bytes;
+                TAV_CUDA(cudaMemcpyAsync(stage, ix->pin_append[b].p, bytes, cudaMemcpyHostToDevice, s));
+                TAV_CUDA(launch_convert(stage, src_dtype, dst + done * dst_row, ix->dtype, m, ix->dim, norm, s));
+            }
+            TAV_CUDA(cudaEventRecord(ix->ev_append[b], s));
+            ix->append_busy[b] = true;
+        }
+        // the caller's buffer was fully consumed by the memcpys above; the pinned buffers are
+        // re-acquired through their events, so no synchronisation is needed here
+    }
+    return TAV_OK;
+}
+
 extern "C" {
 
 int tav_abi_version(void) { return TAV_ABI_VERSION; }
@@ -336,7 +393,7 @@ int tav_destroy(tav_index* ix) {
                       &ix->mma_ws, &ix->retry, &ix->split_hi, &ix->split_lo, &ix->split_flag, &ix->row_mask,
                       &ix->range_keys, &ix->range_keys2, &ix->range_counts, &ix->range_qgather, &ix->range_tmp,
                       &ix->range_sortws, &ix->range_items, &ix->range_scores, &ix->range_mmaws,
-                      &ix->range_mmaws2, &ix->range_mmaaux})
+                      &ix->range_mmaws2, &ix->range_mmaaux, &ix->compact_keys})
         b->release();
     for (DevBuf& b : ix->held_retired) b.release();
     if (ix->ev_last) cudaEventDestroy(ix->ev_last);
@@ -441,46 +498,7 @@ int tav_append(tav_index* ix, const void* rows, int64_t n, int dim, int src_dtyp
         mark_done(ix);
         if (int rc = reserve_locked(ix, want, s)) return rc;
     }
-    const size_t dst_row = static_cast<size_t>(ix->dim) * dtype_size(ix->dtype);
-    const size_t src_row = static_cast<size_t>(ix->dim) * dtype_size(src_dtype);
-    char* dst = static_cast<char*>(ix->rows) + static_cast<size_t>(ix->size) * dst_row;
-    const bool plain = (src_dtype == ix->dtype) && !(ix->flags & TAV_NORMALIZE);
-    const int norm = (ix->flags & TAV_NORMALIZE) ? 1 : 0;
-    if (src_on_device) {
-        if (plain)
-            TAV_CUDA(cudaMemcpyAsync(dst, rows, static_cast<size_t>(n) * src_row, cudaMemcpyDeviceToDevice, s));
-        else
-            TAV_CUDA(launch_convert(rows, src_dtype, dst, ix->dtype, n, ix->dim, norm, s));
-    } else {
-        // Host source (bulk load at open, storage/sqlite/messageindex.py:33-45; incremental appends):
-        // through a pinned double buffer, so that the H2D copies are truly asynchronous and the host
-        // memcpy of chunk i+1 overlaps the DMA (+ conversion kernel) of chunk i.
-        const int64_t chunk_rows = std::max<int64_t>(1, static_cast<int64_t>(kAppendStageBytes / src_row));
-        const size_t stage_bytes = static_cast<size_t>(std::min(n, chunk_rows)) * src_row;
-        if (!plain) TAV_CUDA(ix->staging.ensure(2 * stage_bytes));
-        int b = 0;
-        for (int64_t done = 0; done < n; done += chunk_rows, b ^= 1) {
-            const int64_t m = std::min(chunk_rows, n - done);
-            const size_t bytes = static_cast<size_t>(m) * src_row;
-            if (ix->append_busy[b]) {  // also across calls: the previous append may still be queued on its stream
-                TAV_CUDA(cudaEventSynchronize(ix->ev_append[b]));
-                ix->append_busy[b] = false;
-            }
-            TAV_CUDA(ix->pin_append[b].ensure(stage_bytes));
-            memcpy(ix->pin_append[b].p, static_cast<const char*>(rows) + done * src_row, bytes);
-            if (plain) {
-                TAV_CUDA(cudaMemcpyAsync(dst + done * dst_row, ix->pin_append[b].p, bytes, cudaMemcpyHostToDevice, s));
-            } else {
-                char* stage = static_cast<char*>(ix->staging.p) + static_cast<size_t>(b) * stage_bytes;
-                TAV_CUDA(cudaMemcpyAsync(stage, ix->pin_append[b].p, bytes, cudaMemcpyHostToDevice, s));
-                TAV_CUDA(launch_convert(stage, src_dtype, dst + done * dst_row, ix->dtype, m, ix->dim, norm, s));
-            }
-            TAV_CUDA(cudaEventRecord(ix->ev_append[b], s));
-            ix->append_busy[b] = true;
-        }
-        // the caller's buffer was fully consumed by the memcpys above; the pinned buffers are
-        // re-acquired through their events, so no synchronisation is needed here
-    }
+    if (int rc = store_rows(ix, ix->size, rows, n, src_dtype, src_on_device, s)) return rc;
     ix->size += n;
     return mark_queued(ix, s);
 }
@@ -716,6 +734,15 @@ static int ensure_split_planes(tav_index* ix, TimedSearch* ts, cudaStream_t s) {
             return TAV_ERR_OOM;
         }
         ix->split_cap = cap;
+    }
+    if (ix->split_recheck) {  // the flag may stand for rows that were removed or overwritten since
+        ix->split_recheck = false;
+        if (ix->split_rows > 0) {
+            int flag = 0;
+            TAV_CUDA(cudaMemcpyAsync(&flag, ix->split_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+            TAV_CUDA(cudaStreamSynchronize(s));
+            if (flag) ix->split_rows = 0;  // rebuilt from row 0, which resets it
+        }
     }
     if (ix->split_rows < ix->size) {
         if (ix->split_rows == 0) TAV_CUDA(cudaMemsetAsync(ix->split_flag.p, 0, sizeof(int), s));  // planes rebuilt from row 0
@@ -1197,7 +1224,185 @@ static int range_core(tav_index* ix, TimedSearch* ts, bool timing, const float* 
                               expected_hits, offsets, s);
 }
 
+// ---- removal and overwrite (tav_remove_rows, tav_write_rows) -----------------------------------------------
+constexpr size_t kCompactScratchBytes = size_t(256) << 20;  // window buffer of the in-place compaction
+
+// Entry of the calls that change rows in place, after join_stream: the outstanding deferred searches are
+// finished first, because their exact redo reads the rows.
+static int finish_before_row_change(tav_index* ix, cudaStream_t s) {
+    if (ix->pending.empty()) return TAV_OK;
+    int redone = 0;
+    return finish_pending(ix, s, &redone);
+}
+
+// Compacts the rows after the removal of `rem` (sorted, distinct, not empty) on s and synchronises s.  Rows
+// [0, rem[0]) are not written.  Out of place (tav_internal_compact_policy mode 1) — a fresh allocation of the
+// capacity, the rows before rem[0] copied over unchanged, each moving row read and written once; the old
+// allocation is handed back in *old_rows for the caller to free.  In place by default: ascending windows of destinations, each gathered into a scratch buffer and copied back (the
+// sources of a window lie at or above its first row, and rows above it are written only by later windows).
+static int compact_rows(tav_index* ix, const std::vector<int64_t>& rem, cudaStream_t s, void** old_rows) {
+    *old_rows = nullptr;
+    ix->compact_path = 0;
+    ix->compact_windows = 0;
+    const int64_t m = static_cast<int64_t>(rem.size());
+    const int64_t first = rem[0], new_size = ix->size - m;
+    const int64_t moving = new_size - first;  // surviving rows after the first removed one
+    if (moving == 0) return TAV_OK;           // only the last rows were removed
+    const size_t row = static_cast<size_t>(ix->dim) * dtype_size(ix->dtype);
+    std::vector<int64_t> keys(rem.size());
+    for (int64_t i = 0; i < m; ++i) keys[i] = rem[i] - i;
+    TAV_CUDA(ix->compact_keys.ensure(keys.size() * sizeof(int64_t)));
+    // from pageable memory: the copy has consumed `keys` when the call returns
+    TAV_CUDA(cudaMemcpyAsync(ix->compact_keys.p, keys.data(), keys.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    const int64_t* d_keys = static_cast<const int64_t*>(ix->compact_keys.p);
+
+    // Bytes moved: out of place 2 * (first + moving) rows, in place 4 * moving (one scratch round trip).  The
+    // in-place form is the default all the same: at 10M x 768 bf16 the cudaMalloc / cudaFree of a second copy
+    // of the rows cost about what the scratch round trip costs (DESIGN.md §3.5), and it needs no second copy.
+    if (ix->compact_mode == 1) {
+        void* fresh = nullptr;
+        cudaError_t e = cudaMalloc(&fresh, std::max<size_t>(static_cast<size_t>(ix->capacity) * row, 256));
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            set_error("tav_remove_rows: no device memory for an out-of-place compaction");
+            return TAV_ERR_OOM;
+        }
+        e = first > 0 ? cudaMemcpyAsync(fresh, ix->rows, static_cast<size_t>(first) * row, cudaMemcpyDeviceToDevice, s)
+                      : cudaSuccess;
+        if (e == cudaSuccess) e = launch_compact_gather(ix->rows, fresh, d_keys, m, first, new_size, 0, row, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess) {
+            cudaFree(fresh);
+            set_error("tav_remove_rows: compaction failed: %s", cudaGetErrorString(e));
+            return TAV_ERR_CUDA;
+        }
+        *old_rows = ix->rows;
+        ix->rows = fresh;
+        ix->compact_path = 1;
+        ix->compact_windows = 1;
+        return TAV_OK;
+    }
+    const size_t scratch_bytes = ix->compact_scratch > 0 ? static_cast<size_t>(ix->compact_scratch) : kCompactScratchBytes;
+    int64_t win = std::min<int64_t>(moving, std::max<int64_t>(1, static_cast<int64_t>(scratch_bytes / row)));
+    // the form for short memory: when the window buffer does not fit, halve it (down to one row) rather than fail
+    DevBuf scratch;
+    for (;;) {
+        const cudaError_t ae = scratch.ensure(static_cast<size_t>(win) * row);
+        if (ae == cudaSuccess) break;
+        cudaGetLastError();
+        if (ae != cudaErrorMemoryAllocation || win == 1) {
+            set_error("tav_remove_rows: cannot allocate the compaction window (%zu bytes): %s",
+                      static_cast<size_t>(win) * row, cudaGetErrorString(ae));
+            return ae == cudaErrorMemoryAllocation ? TAV_ERR_OOM : TAV_ERR_CUDA;
+        }
+        win = std::max<int64_t>(1, win / 2);
+    }
+    cudaError_t e = cudaSuccess;
+    int64_t windows = 0;
+    for (int64_t d0 = first; d0 < new_size && e == cudaSuccess; d0 += win, ++windows) {
+        const int64_t d1 = std::min(new_size, d0 + win);
+        e = launch_compact_gather(ix->rows, scratch.p, d_keys, m, d0, d1, d0, row, s);
+        if (e == cudaSuccess)
+            e = launch_compact_copy(ix->device, scratch.p, static_cast<char*>(ix->rows) + static_cast<size_t>(d0) * row,
+                                    d1 - d0, row, s);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    scratch.release();
+    if (e != cudaSuccess) {
+        set_error("tav_remove_rows: compaction failed: %s", cudaGetErrorString(e));
+        return TAV_ERR_CUDA;
+    }
+    ix->compact_path = 2;
+    ix->compact_windows = windows;
+    return TAV_OK;
+}
+
 extern "C" {
+
+int tav_remove_rows(tav_index* ix, const int64_t* ordinals, int64_t n, void* stream) {
+    if (!ix || n < 0 || (n > 0 && !ordinals)) {
+        set_error("tav_remove_rows: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (ix->adopted) {
+        set_error("tav_remove_rows: index uses adopted device memory");
+        return TAV_ERR_STATE;
+    }
+    // np.delete semantics: negative ordinals count from the end, duplicates remove one row, order is free
+    std::vector<int64_t> rem(static_cast<size_t>(n));
+    for (int64_t i = 0; i < n; ++i) {
+        const int64_t v = ordinals[i];
+        if (v < -ix->size || v >= ix->size) {
+            set_error("index %lld is out of bounds for axis 0 with size %lld", (long long)v, (long long)ix->size);
+            return TAV_ERR_RANGE;
+        }
+        rem[i] = v < 0 ? v + ix->size : v;
+    }
+    if (n == 0) return TAV_OK;
+    if (!std::is_sorted(rem.begin(), rem.end())) std::sort(rem.begin(), rem.end());
+    rem.erase(std::unique(rem.begin(), rem.end()), rem.end());
+    if (int rc = set_device(ix)) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;  // queued searches read the old rows
+    if (int rc = finish_before_row_change(ix, s)) return rc;
+    void* old_rows = nullptr;
+    if (int rc = compact_rows(ix, rem, s, &old_rows)) return rc;
+    if (ix->compact_path != 0) mark_done(ix);  // s was synchronised after the compaction
+    if (old_rows) cudaFree(old_rows);
+    ix->size -= static_cast<int64_t>(rem.size());
+    ix->split_rows = std::min(ix->split_rows, rem[0]);
+    ix->split_recheck = true;
+    ix->row_mask_rows = 0;  // ordinals changed meaning (a later append can restore the old size)
+    return TAV_OK;
+}
+
+int tav_write_rows(tav_index* ix, int64_t first, const void* rows, int64_t n, int dim, int src_dtype,
+                   int src_on_device, void* stream) {
+    if (!ix || n < 0 || dim <= 0 || !dtype_ok(src_dtype) || (n > 0 && !rows)) {
+        set_error("tav_write_rows: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (ix->adopted) {
+        set_error("tav_write_rows: index uses adopted device memory");
+        return TAV_ERR_STATE;
+    }
+    if (first < 0 || n > ix->size - first) {
+        set_error("tav_write_rows: rows [%lld, %lld) out of range (size %lld)", (long long)first,
+                  (long long)(first + n), (long long)ix->size);
+        return TAV_ERR_RANGE;
+    }
+    if (dim != ix->dim) {
+        set_error("Embedding size mismatch: expected %d, got %d", ix->dim, dim);
+        return TAV_ERR_INVALID;
+    }
+    if (n == 0) return TAV_OK;
+    if (int rc = set_device(ix)) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;  // queued searches read the old rows
+    if (int rc = finish_before_row_change(ix, s)) return rc;
+    if (int rc = store_rows(ix, first, rows, n, src_dtype, src_on_device, s)) return rc;
+    ix->split_rows = std::min(ix->split_rows, first);
+    ix->split_recheck = true;
+    return mark_queued(ix, s);
+}
+
+int tav_internal_compact_policy(tav_index* ix, int mode, int64_t scratch_bytes) {
+    if (!ix || mode < 0 || mode > 2 || scratch_bytes < 0) return TAV_ERR_INVALID;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    ix->compact_mode = mode;
+    ix->compact_scratch = scratch_bytes;
+    return TAV_OK;
+}
+
+int tav_internal_compact_stats(tav_index* ix, int* path, int64_t* windows) {
+    if (!ix) return TAV_ERR_INVALID;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (path) *path = ix->compact_path;
+    if (windows) *windows = ix->compact_windows;
+    return TAV_OK;
+}
 
 const int32_t* tav_internal_retry_totals(tav_index* ix, int* count) {
     if (count) *count = 0;

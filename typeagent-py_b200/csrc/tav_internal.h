@@ -124,6 +124,16 @@ cudaError_t launch_merge(int n_lists, int n_queries, int k, const int64_t* items
                          int64_t scores_stride, int64_t counts_stride, int64_t* out_items,
                          float* out_scores, int32_t* out_counts, cudaStream_t s, const MergeSync* sync = nullptr);
 
+// ---- compaction after a removal (tav_compact.cu) -----------------------------------------
+// keys: device [m], keys[i] = rem[i] - i over the sorted distinct removed ordinals.  Destinations
+// [d_begin, d_end) of the compacted rows: dst row (d - d_base) = src row (d + #{keys <= d}).  src and dst
+// must not overlap.
+cudaError_t launch_compact_gather(const void* src, void* dst, const int64_t* keys, int64_t m, int64_t d_begin,
+                                  int64_t d_end, int64_t d_base, size_t row_bytes, cudaStream_t s);
+// n_rows whole rows src -> dst (no overlap), on `device`
+cudaError_t launch_compact_copy(int device, const void* src, void* dst, int64_t n_rows, size_t row_bytes,
+                                cudaStream_t s);
+
 // rows [n, dim] of src dtype -> dst dtype (RNE), optionally L2-normalised per row (fp32 math)
 cudaError_t launch_convert(const void* src, int src_dtype, void* dst, int dst_dtype, int64_t n,
                            int dim, int normalize, cudaStream_t s);
@@ -201,6 +211,13 @@ void set_error(const char* fmt, ...);
 // published candidate list so that every rank learns, without a second exchange, whether some rank will
 // correct its candidates at finish.
 extern "C" const int32_t* tav_internal_retry_totals(tav_index* ix, int* count);
+
+// library-internal: how tav_remove_rows compacts on this index.  `mode` 0 the default (in place), 1 out of
+// place (TAV_ERR_OOM when its allocation fails), 2 in place; `scratch_bytes` bounds the in-place window buffer (0: the
+// default).  tav_internal_compact_stats reports the last removal: path 0 nothing moved, 1 out of place,
+// 2 in place, and the number of windows.  Tests use them to reach both paths on small indexes.
+extern "C" int tav_internal_compact_policy(tav_index* ix, int mode, int64_t scratch_bytes);
+extern "C" int tav_internal_compact_stats(tav_index* ix, int* path, int64_t* windows);
 
 namespace tav {
 

@@ -65,6 +65,15 @@ class EmbeddingIndex:
     async def add_texts(self, texts: list[str]) -> None:
         await self._vector_base.add_keys(texts)
 
+    def remove_at(self, pos: int) -> None:
+        """Remove the embedding at ``pos``; the rows after it move up by one (compacted on the device)."""
+        if 0 <= pos < len(self._vector_base):
+            self._vector_base.remove_embedding_at(pos)
+        else:
+            raise IndexError(
+                f"Index {pos} out of bounds for embedding index of size {len(self._vector_base)}"
+            )
+
     async def get_embedding(self, key: str, cache: bool = True):
         return await self._vector_base.get_embedding(key, cache)
 

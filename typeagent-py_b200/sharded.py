@@ -33,7 +33,7 @@ import ctypes as C
 import numpy as np
 
 from . import _capi
-from .vectorbase import ScoredInt, TextEmbeddingIndexSettings, VectorBase, _as_f32_scalar
+from .vectorbase import ScoredInt, TextEmbeddingIndexSettings, VectorBase, _as_f32_scalar, removal_ordinals
 
 RANGE_ROUTE_MIN_ROWS = 4 * 2048  # search_arrays with k >= rows above this (4 * TAV_PASS_K) -> search_range
 
@@ -152,6 +152,9 @@ class CudaShardEngine:
 
     def append_rows(self, rows: np.ndarray) -> None:
         self.base.add_embeddings(None, rows)
+
+    def remove_rows(self, local_ordinals: np.ndarray) -> None:
+        self.base.remove_embeddings(local_ordinals)
 
     def finish(self) -> int:
         return self.base.finish_search()
@@ -383,6 +386,25 @@ class ShardedVectorBase:
         if keys is not None:
             for key, row in zip(keys, embeddings):
                 self.settings.embedding_model.add_embedding(key, row)
+
+    def remove_embeddings(self, ordinals) -> None:
+        """Remove rows by global ordinal, as ``VectorBase.remove_embeddings`` does on one GPU (``np.delete``
+        semantics: integer ordinals or a boolean mask over every row; IndexError, with nothing removed, for an
+        ordinal out of range).  SPMD: every rank passes the same ordinals.  Deferred lookups are finished first
+        (``finish()``, collective): the local removal redoes their flagged queries on the old rows, and only
+        ``finish()`` exchanges and merges the corrected candidates again.  Each rank then removes its own block's
+        share and recomputes the block starts from the replicated list, without a collective; blocks may become
+        uneven (a block may empty)."""
+        removed = removal_ordinals(ordinals, len(self))
+        if removed.size == 0:
+            return
+        self.finish()
+        lo, hi = self.local_range
+        mine = removed[(removed >= lo) & (removed < hi)] - lo
+        if len(mine):
+            self._engine.remove_rows(mine)
+        starts = np.asarray(self._starts, np.int64)
+        self._starts = (starts - np.searchsorted(removed, starts, side="left")).tolist()
 
     # ---- lookups -----------------------------------------------------------------------
     def _gather_and_merge(self, local, b: int, k: int):

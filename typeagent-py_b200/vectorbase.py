@@ -94,6 +94,26 @@ def _create_default_embedding_model():
     return create_embedding_model()
 
 
+def removal_ordinals(ordinals, n: int) -> np.ndarray:
+    """The rows ``np.delete(rows, ordinals, axis=0)`` removes from n rows, sorted and distinct (int64): integer
+    ordinals (negative ones count from the end, repeats remove one row) or a boolean mask of length n.  The same
+    errors as numpy: IndexError for an ordinal out of range or a non-integer array, ValueError for a mask of
+    the wrong shape."""
+    idx = np.asarray(ordinals)
+    if idx.dtype == bool:
+        if idx.ndim != 1 or len(idx) != n:
+            raise ValueError("boolean array argument obj to delete must be one dimensional and match the axis "
+                             f"length of {n}")
+        return np.flatnonzero(idx).astype(np.int64)
+    if idx.size and not np.issubdtype(idx.dtype, np.integer):
+        raise IndexError("arrays used as indices must be of integer (or boolean) type")
+    idx = idx.astype(np.int64, copy=False).reshape(-1)
+    bad = (idx < -n) | (idx >= n)
+    if bad.any():
+        raise IndexError(f"index {int(idx[bad][0])} is out of bounds for axis 0 with size {n}")
+    return np.unique(np.where(idx < 0, idx + n, idx))
+
+
 def _as_f32_scalar(value: float) -> np.float32:
     # a Python float is a weak scalar in `scores >= min_score` (NEP 50): compared as float32
     return np.float32(value)
@@ -122,6 +142,7 @@ class VectorBase:
         self._buf = np.empty((0, 0), dtype=np.float32)
         self._count = 0
         self._generation = 0  # bumped whenever rows are replaced rather than appended
+        self._buf_is_callers = False  # _buf was handed in by deserialize(): rows never change in it
         # device side (created on first lookup)
         self._ix: C.c_void_p | None = None
         self._ix_generation = -1
@@ -167,6 +188,7 @@ class VectorBase:
         value = np.asarray(value, dtype=np.float32)
         if value.ndim == 2:
             self._buf = value
+            self._buf_is_callers = True
             self._count = len(value)
             if value.shape[1] > 0:
                 self._embedding_size = value.shape[1]
@@ -212,6 +234,7 @@ class VectorBase:
             fresh = np.empty((cap, self._embedding_size), dtype=np.float32)
             fresh[: self._count] = self._buf[: self._count]
             self._buf = fresh
+            self._buf_is_callers = False
         self._buf[self._count : need] = rows
         self._count = need
 
@@ -279,10 +302,91 @@ class VectorBase:
         if data.dtype != np.float32:
             data = data.astype(np.float32)
         self._buf = data  # adopted without a copy, as the reference does
+        self._buf_is_callers = True
         self._count = len(data)
         self._generation += 1
         self._device_only_rows = 0
         self._adopted_tensor = None
+
+    # ------------------------------------------------------------------ remove / overwrite
+    def _device_in_sync(self) -> bool:
+        """The device holds the host mirror's rows [0, _ix_rows) (rows after that are appended at the next
+        lookup; after a deserialize() the next lookup re-uploads everything)."""
+        return self._ix is not None and self._ix_generation == self._generation and self._ix_rows > 0
+
+    def _own_buffer(self) -> None:
+        """Rows are about to change in place: never write into an array adopted from deserialize()."""
+        if self._buf_is_callers or not self._buf.flags.writeable or not self._buf.flags.owndata:
+            self._buf = np.array(self._buf[: self._count], dtype=np.float32)
+            self._buf_is_callers = False
+
+    def remove_embeddings(self, ordinals) -> None:
+        """Remove rows, as ``np.delete(self.serialize(), ordinals, axis=0)`` would: integer ordinals (negative
+        ones count from the end, a repeated ordinal removes one row, order does not matter) or a boolean mask of
+        one entry per row; IndexError for an ordinal out of range, with nothing removed.  The surviving rows keep their order (row r becomes row r - #{removed < r}).
+        The device copy is compacted on the device (``tav_remove_rows``), not re-uploaded.  Row masks and
+        cached predicate masks are dropped: ordinals change meaning."""
+        if self._device_only_rows:
+            raise RuntimeError("this VectorBase wraps a device tensor; rows cannot be removed from it")
+        n = self._count
+        removed = removal_ordinals(ordinals, n)
+        if removed.size == 0:
+            return
+        if self._device_in_sync():
+            on_device = np.ascontiguousarray(removed[removed < self._ix_rows])
+            if len(on_device):
+                _capi.check(_capi.load().tav_remove_rows(self._ix, on_device.ctypes.data_as(C.c_void_p),
+                                                         len(on_device), None))
+                self._ix_rows -= len(on_device)
+        first = int(removed[0])
+        keep = np.ones(n - first, dtype=bool)
+        keep[removed - first] = False
+        self._own_buffer()
+        tail = self._buf[first:n][keep]  # a copy: the rows move down within the same buffer
+        self._buf[first : first + len(tail)] = tail
+        self._count = n - len(removed)
+        self._mask_key = None
+        self._mask_ref = None
+        self._predicate_masks.clear()
+
+    def remove_embedding_at(self, pos: int) -> None:
+        if not 0 <= pos < len(self):
+            raise IndexError(f"Index {pos} out of bounds for embedding index of size {len(self)}")
+        self.remove_embeddings([pos])
+
+    def set_embeddings_at(self, first: int, embeddings: np.ndarray) -> None:
+        """Overwrite rows [first, first + len(embeddings)) in place (float32 [n, D]); the device rows are
+        rewritten through ``tav_write_rows`` with the conversion of an append, so every lookup afterwards equals
+        one on an index built from the new rows.  IndexError when the rows are not all there."""
+        if self._device_only_rows:
+            raise RuntimeError("this VectorBase wraps a device tensor; its rows cannot be overwritten")
+        rows = np.ascontiguousarray(embeddings, dtype=np.float32)
+        if rows.ndim != 2:
+            raise ValueError(f"Expected 2D embeddings array, got {rows.ndim}D")
+        self._check_width(rows.shape[1])
+        n = len(rows)
+        if first < 0 or first + n > self._count:
+            raise IndexError(
+                f"Index {first if first < 0 or n == 0 else first + n - 1} out of bounds for embedding index of "
+                f"size {len(self)}"
+            )
+        if n == 0:
+            return
+        if self._device_in_sync() and first < self._ix_rows:
+            m = min(n, self._ix_rows - first)
+            _capi.check(_capi.load().tav_write_rows(self._ix, first, rows.ctypes.data_as(C.c_void_p), m,
+                                                    self._embedding_size, _capi.TAV_F32, 0, None))
+        self._own_buffer()
+        self._buf[first : first + n] = rows
+
+    def set_embedding_at(self, pos: int, embedding) -> None:
+        row = np.asarray(embedding, dtype=np.float32)
+        if row.ndim != 1:
+            raise ValueError(f"Expected 1D embedding, got {row.ndim}D")
+        self._check_width(len(row))
+        if not 0 <= pos < len(self):
+            raise IndexError(f"Index {pos} out of bounds for embedding index of size {len(self)}")
+        self.set_embeddings_at(pos, row.reshape(1, -1))
 
     # ------------------------------------------------------------------ device plumbing
     def _drop_device(self) -> None:
