@@ -93,7 +93,13 @@ enum tav_search_flags {
     /* Do not use the single-launch form of the row scan (one host query, host outputs: the query
      * rides in the kernel parameters and the last CTA merges); tests use it to reach the two-kernel
      * form with one query. */
-    TAV_NO_FUSED_SCAN = 128
+    TAV_NO_FUSED_SCAN = 128,
+    /* With a subset only (otherwise TAV_ERR_INVALID): items are the POSITION of the hit in `subset`
+     * (+ item_offset) instead of subset[position] (+ item_offset).  Which rows are scored, their keys and
+     * the order are unchanged.  A row-sharded subset search uses it: positions stay distinct when the
+     * subset repeats an ordinal, so the ranks' lists can be merged by position (tav_merge_topk_ordered
+     * orders 2 / 3, tav_merge_range) and decoded through the caller's list afterwards (tav_map_items). */
+    TAV_ITEMS_AS_POSITIONS = 256
 };
 
 int tav_abi_version(void);
@@ -225,6 +231,30 @@ int tav_merge_topk(int device, int n_lists, int n_queries, int k, const int64_t*
                    const float* scores, const int32_t* counts, int64_t items_stride,
                    int64_t scores_stride, int64_t counts_stride, int64_t* out_items,
                    float* out_scores, int32_t* out_counts, void* stream);
+
+/*
+ * tav_merge_topk with a choice of the order among equal scores (`order`; anything else: TAV_ERR_INVALID):
+ *   0  tav_merge_topk's: later list first, inside a list the earlier slot (higher row first);
+ *   1  earlier list first, inside a list the earlier slot: lower row first for lists in ascending row
+ *      blocks that were searched with TAV_TIES_LOW_FIRST (the predicate path);
+ *   2  the item itself, higher first;  3  the item itself, lower first.  For lists whose items are
+ *      distinct and in [0, 2^32), such as global subset positions (TAV_ITEMS_AS_POSITIONS), in any list
+ *      order.  The merged items are those keys.
+ * Same arguments, layout and limits as tav_merge_topk otherwise.
+ */
+int tav_merge_topk_ordered(int device, int n_lists, int n_queries, int k, const int64_t* items,
+                           const float* scores, const int32_t* counts, int64_t items_stride,
+                           int64_t scores_stride, int64_t counts_stride, int order, int64_t* out_items,
+                           float* out_scores, int32_t* out_counts, void* stream);
+
+/*
+ * Device gather, in place: items[i] = table[items[i]] for every i < n with 0 <= items[i] < table_len;
+ * other entries (the -1 padding of a [n_queries, k] result, for one) stay as they are.  `items` (int64 [n])
+ * and `table` (int64 [table_len]) are device pointers on `device`; works on [n_queries, k] and CSR results
+ * alike.  Enqueued on `stream`, no synchronisation.  n < 0, table_len < 0, or a NULL pointer that is
+ * needed: TAV_ERR_INVALID.
+ */
+int tav_map_items(int device, int64_t n, const int64_t* table, int64_t table_len, int64_t* items, void* stream);
 
 /*
  * Merge step of the row-sharded threshold search: `n_lists` per-shard CSR results of tav_range_search

@@ -11,6 +11,8 @@ the single-GPU lookup over the whole corpus on that rank's GPU, for the float32 
 float32 split form and the bf16 / fp16 tensor-core paths, and agrees with the CPU oracle.  The sharded
 threshold search (``search_range``: offsets and hits all-gathered, ``tav_merge_range``) must equal the
 single-GPU ``search_range`` bit for bit on every rank: float32 row scan, bf16 tensor cores, float32 split form.
+Filtered and subset lookups (row masks, predicates, subsets; top-k and threshold) must equal the single-GPU
+``VectorBase`` bit for bit on every rank.
 """
 import os
 import sys
@@ -116,6 +118,39 @@ def main():
         if rank == 0:
             print(f"multi-gpu ok: world={world} search_range {storage} n={n} d={d} b={b} min_score={ms} path={path} "
                   f"hits={int(want[0][-1])}", flush=True)
+    # filtered and subset lookups (row masks, predicates, subsets with duplicates and negative ordinals): equal to
+    # the single-GPU VectorBase bit for bit on every rank, over the process group whatever `exchange` says
+    for storage, n, d, b in (("float32", 50001, 96, 6), ("bfloat16", 120001, 128, 24)):
+        v, q = O.make_corpus(n, d, seed=n + 2, n_queries=b)
+        v[n // 2: n // 2 + 500] = v[:500]  # equal scores on different ranks
+        sh = ShardedVectorBase(settings, device=local, storage_dtype=storage)
+        sh.deserialize(v)
+        whole = tab.VectorBase(settings, device=local, storage_dtype=storage)
+        whole.add_embeddings(None, v)
+        rng = np.random.default_rng(n)
+        sub = np.concatenate([rng.permutation(n)[:3000], np.arange(500), n // 2 + np.arange(500), [-1, -n, 0]])
+        allowed = rng.random(n) < 0.3
+        pred = lambda i, a=allowed: bool(a[i])  # noqa: E731
+        for tl in (False, True):
+            for got, want in ((sh.search_arrays(q, 50, 0.4, subset=sub, ties_low_first=tl),
+                               whole.search_arrays(q, 50, 0.4, subset=sub, ties_low_first=tl)),
+                              (sh.search_arrays(q, 100, 0.4, allowed=allowed, ties_low_first=tl),
+                               whole.search_arrays(q, 100, 0.4, allowed=allowed, ties_low_first=tl)),
+                              (sh.search_range(q, 0.6, ties_low_first=tl, subset=sub),
+                               whole.search_range(q, 0.6, subset=sub, ties_low_first=tl)),
+                              (sh.search_range(q, 0.6, ties_low_first=tl, allowed=allowed),
+                               whole.search_range(q, 0.6, allowed=allowed, ties_low_first=tl))):
+                for g, w in zip(got, want):
+                    np.testing.assert_array_equal(g.view(np.uint32) if g.dtype == np.float32 else g,
+                                                  w.view(np.uint32) if w.dtype == np.float32 else w)
+        for i in range(min(b, 4)):
+            assert sh.fuzzy_lookup_embedding(q[i], 10, 0.3, predicate=pred) == \
+                whole.fuzzy_lookup_embedding(q[i], 10, 0.3, predicate=pred)
+            assert sh.fuzzy_lookup_embedding_in_subset(q[i], sub.tolist(), 20, 0.3) == \
+                whole.fuzzy_lookup_embedding_in_subset(q[i], sub.tolist(), 20, 0.3)
+        dist.barrier()
+        if rank == 0:
+            print(f"multi-gpu ok: world={world} filtered and subset lookups {storage} n={n} d={d} b={b}", flush=True)
     dist.destroy_process_group()
 
 

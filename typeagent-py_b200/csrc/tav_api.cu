@@ -622,7 +622,7 @@ static int ensure_scan_counters(tav_index* ix, cudaStream_t s) {
 static int scan_search(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq_total, int k, float floor_score,
                        const int64_t* d_subset, int64_t n_scan, int64_t item_offset, int64_t* d_items,
                        float* d_scores, int32_t* d_counts, const uint32_t* d_mask, int ties_low, cudaStream_t s,
-                       bool allow_fuse = true) {
+                       bool allow_fuse = true, int positions = 0) {
     const int pass_k = std::min(k, kPassK);
     int qb = scan_max_queries(ix->dim, pass_k);
     if (qb < 1) {
@@ -668,6 +668,7 @@ static int scan_search(tav_index* ix, TimedSearch* ts, bool timing, const float*
             a.grid = grid;
             a.row_mask = d_mask;
             a.ties_low = ties_low;
+            a.items_as_positions = positions;
             if (fuse) {
                 a.fused = 1;
                 a.fused_ticket = d_count + 8;
@@ -696,7 +697,7 @@ static int scan_search(tav_index* ix, TimedSearch* ts, bool timing, const float*
             sel.k = kk;
             sel.out_stride = k;
             sel.out_offset = pass * pass_k;
-            sel.subset = d_subset;
+            sel.subset = positions ? nullptr : d_subset;  // items = the position itself
             sel.item_offset = item_offset;
             sel.out_items = d_items + static_cast<size_t>(q0) * k;
             sel.out_scores = d_scores + static_cast<size_t>(q0) * k;
@@ -1022,7 +1023,8 @@ static int range_sort(tav_index* ix, TimedSearch* ts, bool timing, std::vector<S
 // overflowed queries get exactly one more scan into regions of that size.
 static int range_collect_scan(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
                               const int64_t* d_subset, int64_t n_scan, int64_t item_offset, const uint32_t* d_mask,
-                              int ties_low, int64_t expected_hits, std::vector<int64_t>& offsets, cudaStream_t s) {
+                              int ties_low, int64_t expected_hits, std::vector<int64_t>& offsets, cudaStream_t s,
+                              int positions = 0) {
     const int64_t per = range_per_query(expected_hits, nq, n_scan);
     if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(nq) * per * sizeof(uint64_t), "the hit regions")) return rc;
     if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(nq) * sizeof(uint32_t), "the hit counters")) return rc;
@@ -1072,7 +1074,7 @@ static int range_collect_scan(tav_index* ix, TimedSearch* ts, bool timing, const
         segs[q].out = offsets[q];
         segs[q].n = cnt[q];
     }
-    return range_sort(ix, ts, timing, segs, offsets[nq], d_subset, item_offset, ties_low, s);
+    return range_sort(ix, ts, timing, segs, offsets[nq], positions ? nullptr : d_subset, item_offset, ties_low, s);
 }
 
 constexpr int kRangeUseScan = 1;  // range_collect_mma: the tensor-core form cannot serve this search
@@ -1213,7 +1215,8 @@ static int range_collect_mma(tav_index* ix, TimedSearch* ts, bool timing, const 
 // (offsets[nq + 1], host): collected by the tensor cores (use_mma) or the row scan, then the segmented sort.
 static int range_core(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
                       const int64_t* d_subset, int64_t n_scan, int64_t item_offset, const uint32_t* d_mask,
-                      int ties_low, int64_t expected_hits, bool use_mma, std::vector<int64_t>& offsets, cudaStream_t s) {
+                      int ties_low, int64_t expected_hits, bool use_mma, std::vector<int64_t>& offsets, cudaStream_t s,
+                      int positions = 0) {
     if (use_mma) {
         const int rc = range_collect_mma(ix, ts, timing, d_queries, nq, floor, item_offset, d_mask, ties_low,
                                          expected_hits, offsets, s);
@@ -1221,7 +1224,7 @@ static int range_core(tav_index* ix, TimedSearch* ts, bool timing, const float* 
         ts->path = 1;  // a value beyond the fp16 range: the exact row scan serves the search
     }
     return range_collect_scan(ix, ts, timing, d_queries, nq, floor, d_subset, n_scan, item_offset, d_mask, ties_low,
-                              expected_hits, offsets, s);
+                              expected_hits, offsets, s, positions);
 }
 
 // ---- removal and overwrite (tav_remove_rows, tav_write_rows) -----------------------------------------------
@@ -1431,6 +1434,10 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         set_error("tav_search: subset / subset_len mismatch");
         return TAV_ERR_INVALID;
     }
+    if ((flags & TAV_ITEMS_AS_POSITIONS) && !subset) {
+        set_error("tav_search: TAV_ITEMS_AS_POSITIONS needs a subset");
+        return TAV_ERR_INVALID;
+    }
     if (n_queries == 0) return TAV_OK;
     std::lock_guard<std::mutex> lock(ix->mu);
     if (int rc = set_device(ix)) return rc;
@@ -1451,6 +1458,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         d_mask = static_cast<const uint32_t*>(ix->row_mask.p);
     }
     const int ties_low = (flags & TAV_TIES_LOW_FIRST) ? 1 : 0;
+    const int positions = (flags & TAV_ITEMS_AS_POSITIONS) && TAV_SHARDED_FILTER_MUTANT != 3 ? 1 : 0;
 
     int64_t* d_items = out_items;
     float* d_scores = out_scores;
@@ -1527,7 +1535,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         std::vector<int64_t> offsets;
         ix->range_total = 0;
         if (int rc = range_core(ix, ts, timing, d_q, n_queries, min_score, d_sub, n_scan, item_offset, d_mask, ties_low,
-                                static_cast<int64_t>(n_queries) * n_scan, false, offsets, s))
+                                static_cast<int64_t>(n_queries) * n_scan, false, offsets, s, positions))
             return rc;
         if (timing) {
             TAV_CUDA(ev_record(ts->total[1], s));
@@ -1603,6 +1611,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         a.row_mask = d_mask;
         a.ties_low = ties_low;
         a.subset_in_params = subset ? 1 : 0;
+        a.items_as_positions = positions;
         a.fused = 1;
         a.fused_ticket = d_count + 8;
         a.item_offset = item_offset;
@@ -1827,7 +1836,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     } else {
         ts->path = 1;
         int rc = scan_search(ix, ts, timing, d_queries, n_queries, k, min_score, d_subset, n_scan, item_offset,
-                             d_items, d_scores, d_counts, d_mask, ties_low, s, !(flags & TAV_NO_FUSED_SCAN));
+                             d_items, d_scores, d_counts, d_mask, ties_low, s, !(flags & TAV_NO_FUSED_SCAN), positions);
         if (rc != TAV_OK) return rc;
     }
     if (timing) {
@@ -1877,6 +1886,10 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
     }
     if (flags & TAV_DEFER_RETRY) {
         set_error("tav_range_search: TAV_DEFER_RETRY is not available for threshold searches");
+        return TAV_ERR_INVALID;
+    }
+    if ((flags & TAV_ITEMS_AS_POSITIONS) && !subset) {
+        set_error("tav_range_search: TAV_ITEMS_AS_POSITIONS needs a subset");
         return TAV_ERR_INVALID;
     }
     std::lock_guard<std::mutex> lock(ix->mu);
@@ -1944,7 +1957,8 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
     if (int rc = stage_inputs(ix, ts, timing, queries, n_queries, q_dev, false, subset, subset_len, &d_queries, &d_subset, s))
         return rc;
     if (int rc = range_core(ix, ts, timing, d_queries, n_queries, min_score, d_subset, n_scan, item_offset, d_mask,
-                            (flags & TAV_TIES_LOW_FIRST) ? 1 : 0, expected_hits, use_mma, offsets, s))
+                            (flags & TAV_TIES_LOW_FIRST) ? 1 : 0, expected_hits, use_mma, offsets, s,
+                            (flags & TAV_ITEMS_AS_POSITIONS) && TAV_SHARDED_FILTER_MUTANT != 3 ? 1 : 0))
         return rc;
     if (timing) {
         TAV_CUDA(ev_record(ts->total[1], s));
@@ -2046,6 +2060,42 @@ int tav_merge_topk(int device, int n_lists, int n_queries, int k, const int64_t*
     TAV_CUDA(launch_merge(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride,
                           counts_stride, out_items, out_scores, out_counts,
                           static_cast<cudaStream_t>(stream)));
+    return TAV_OK;
+}
+
+int tav_merge_topk_ordered(int device, int n_lists, int n_queries, int k, const int64_t* items,
+                           const float* scores, const int32_t* counts, int64_t items_stride,
+                           int64_t scores_stride, int64_t counts_stride, int order, int64_t* out_items,
+                           float* out_scores, int32_t* out_counts, void* stream) {
+    if (n_lists < 1 || n_queries < 0 || k < 1 || !items || !scores || !counts || !out_items ||
+        !out_scores || !out_counts || items_stride < 0 || scores_stride < 0 || counts_stride < 0) {
+        set_error("tav_merge_topk_ordered: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    if (order < 0 || order > 3) {
+        set_error("tav_merge_topk_ordered: order %d is not 0, 1, 2 or 3", order);
+        return TAV_ERR_INVALID;
+    }
+    if (static_cast<int64_t>(n_lists) * k > 0x7FFFFFFFll || k > kPassK * 4) {
+        set_error("tav_merge_topk_ordered: n_lists * k too large");
+        return TAV_ERR_INVALID;
+    }
+    if (n_queries == 0) return TAV_OK;
+    TAV_CUDA(cudaSetDevice(device));
+    TAV_CUDA(launch_merge_ordered(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride,
+                                  counts_stride, order, out_items, out_scores, out_counts,
+                                  static_cast<cudaStream_t>(stream)));
+    return TAV_OK;
+}
+
+int tav_map_items(int device, int64_t n, const int64_t* table, int64_t table_len, int64_t* items, void* stream) {
+    if (n < 0 || table_len < 0 || (n > 0 && !items) || (n > 0 && table_len > 0 && !table)) {
+        set_error("tav_map_items: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    if (n == 0 || table_len == 0) return TAV_OK;
+    TAV_CUDA(cudaSetDevice(device));
+    TAV_CUDA(launch_map_items(n, table, table_len, items, static_cast<cudaStream_t>(stream)));
     return TAV_OK;
 }
 

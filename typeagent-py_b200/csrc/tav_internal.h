@@ -43,6 +43,7 @@ struct ScanArgs {
     // collect mode (launch_scan_collect): query q's keys go to cand_keys + q * collect_stride; cand_count[q]
     // (zero on entry) counts every admitted row, also those beyond collect_stride, which are not stored
     int64_t collect_stride;
+    int items_as_positions;   // single-launch form: items = the subset position (TAV_ITEMS_AS_POSITIONS)
 };
 constexpr int kFusedSelectMax = 8192;   // survivors the last CTA of the single-launch form can merge
 constexpr int kFusedSelOut = 1024;      // ... of which it sorts at most this many after the histogram selection
@@ -123,6 +124,21 @@ cudaError_t launch_merge(int n_lists, int n_queries, int k, const int64_t* items
                          const float* scores, const int32_t* counts, int64_t items_stride,
                          int64_t scores_stride, int64_t counts_stride, int64_t* out_items,
                          float* out_scores, int32_t* out_counts, cudaStream_t s, const MergeSync* sync = nullptr);
+// the same merge with tav_merge_topk_ordered's `order` (0..3) among equal scores
+cudaError_t launch_merge_ordered(int n_lists, int n_queries, int k, const int64_t* items, const float* scores,
+                                 const int32_t* counts, int64_t items_stride, int64_t scores_stride,
+                                 int64_t counts_stride, int order, int64_t* out_items, float* out_scores,
+                                 int32_t* out_counts, cudaStream_t s);
+// in place: items[i] = table[items[i]] where 0 <= items[i] < table_len
+cudaError_t launch_map_items(int64_t n, const int64_t* table, int64_t table_len, int64_t* items, cudaStream_t s);
+
+// TAV_SHARDED_FILTER_MUTANT (tests only, never set by build.py): 1..3 compile one deliberate defect each, so
+// that tests/test_gpu_sharded_filter.py can show its exact checks catch it: 1 the merge's order argument
+// ignored, 2 the position key of orders 2 / 3 replaced by the list / slot key, 3 subset[pos] decoded despite
+// TAV_ITEMS_AS_POSITIONS.
+#ifndef TAV_SHARDED_FILTER_MUTANT
+#define TAV_SHARDED_FILTER_MUTANT 0
+#endif
 
 // ---- compaction after a removal (tav_compact.cu) -----------------------------------------
 // keys: device [m], keys[i] = rem[i] - i over the sorted distinct removed ordinals.  Destinations

@@ -414,7 +414,8 @@ scan_rows_kernel(const ScanArgs a, const __grid_constant__ BLOB blob) {
                 if (j < n) {
                     const uint32_t kp = key_pos(result[j]);
                     const uint32_t pos = a.ties_low ? ~kp : kp;
-                    if (kBlob && a.subset_in_params) item = blob.sub[pos];
+                    if (a.items_as_positions) item = pos;
+                    else if (kBlob && a.subset_in_params) item = blob.sub[pos];
                     else item = a.subset ? a.subset[pos] : static_cast<int64_t>(pos);
                     item += a.item_offset;
                     sc = key_score(result[j]);
@@ -659,12 +660,18 @@ cudaError_t launch_select(const SelectArgs& a, cudaStream_t s) {
 }
 
 // ---- merge of per-shard results (after the candidate all-gather) -------------------------
-// key low word = list * k + (k - 1 - j): among equal scores a later shard (higher rows) and,
+// ORDER 0: key low word = list * k + (k - 1 - j): among equal scores a later shard (higher rows) and,
 // inside a shard, an earlier slot (higher row) sorts first — the same total order as one GPU.
+// ORDER 1: ~(list * k + j): an earlier shard and an earlier slot first (lists searched ties-low-first).
+// ORDER 2 / 3: the item itself (a global subset position < 2^32), or its complement: higher / lower first;
+// the decoded item is the key's low word, the items array is only read for the keys.
+template <int ORDER>
 __global__ void __launch_bounds__(kSelectThreads)
 merge_kernel(int n_lists, int n_queries, int k, const int64_t* items, const float* scores,
              const int32_t* counts, int64_t items_stride, int64_t scores_stride,
              int64_t counts_stride, int64_t* out_items, float* out_scores, int32_t* out_counts, const MergeSync sync) {
+    constexpr bool kPosKey = ORDER >= 2 && TAV_SHARDED_FILTER_MUTANT != 2;
+    constexpr bool kLowFirst = ORDER == 1 || (ORDER == 3 && !kPosKey);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);
     __shared__ int s_cnt;
@@ -694,7 +701,16 @@ merge_kernel(int n_lists, int n_queries, int k, const int64_t* items, const floa
             const int g = static_cast<int>(i / k), j = static_cast<int>(i % k);
             if (j < counts[g * counts_stride + q]) {
                 const float sc = scores[g * scores_stride + static_cast<size_t>(q) * k + j];
-                key = make_key(sc, static_cast<uint32_t>(g * k + (k - 1 - j)));
+                uint32_t low;
+                if constexpr (kPosKey) {
+                    const uint32_t it = static_cast<uint32_t>(items[g * items_stride + static_cast<size_t>(q) * k + j]);
+                    low = ORDER == 2 ? it : ~it;
+                } else if constexpr (kLowFirst) {
+                    low = ~static_cast<uint32_t>(g * k + j);
+                } else {
+                    low = static_cast<uint32_t>(g * k + (k - 1 - j));
+                }
+                key = make_key(sc, low);
                 want = key >= s_admit;
             }
         }
@@ -708,8 +724,16 @@ merge_kernel(int n_lists, int n_queries, int k, const int64_t* items, const floa
         float sc = 0.0f;
         if (j < n) {
             const uint32_t low = key_pos(keys[j]);
-            const int g = low / k, jj = k - 1 - static_cast<int>(low % k);
-            item = items[g * items_stride + static_cast<size_t>(q) * k + jj];
+            if constexpr (kPosKey) {
+                item = static_cast<int64_t>(ORDER == 2 ? low : ~low);
+            } else if constexpr (kLowFirst) {
+                const uint32_t t = ~low;
+                const int g = t / k, jj = static_cast<int>(t % k);
+                item = items[g * items_stride + static_cast<size_t>(q) * k + jj];
+            } else {
+                const int g = low / k, jj = k - 1 - static_cast<int>(low % k);
+                item = items[g * items_stride + static_cast<size_t>(q) * k + jj];
+            }
             sc = key_score(keys[j]);
         }
         out_items[static_cast<size_t>(q) * k + j] = item;
@@ -750,13 +774,68 @@ cudaError_t launch_merge(int n_lists, int n_queries, int k, const int64_t* items
     if (counts_stride == 0) counts_stride = n_queries;
     const size_t smem = static_cast<size_t>(select_cap(k)) * sizeof(uint64_t);
     static int granted[16] = {};
-    cudaError_t e = ensure_dynamic_smem(merge_kernel, smem, granted);
+    cudaError_t e = ensure_dynamic_smem(merge_kernel<0>, smem, granted);
     if (e != cudaSuccess) return e;
     MergeSync none{};
-    merge_kernel<<<n_queries, kSelectThreads, smem, s>>>(n_lists, n_queries, k, items, scores,
-                                                         counts, items_stride, scores_stride,
-                                                         counts_stride, out_items, out_scores,
-                                                         out_counts, sync ? *sync : none);
+    merge_kernel<0><<<n_queries, kSelectThreads, smem, s>>>(n_lists, n_queries, k, items, scores,
+                                                            counts, items_stride, scores_stride,
+                                                            counts_stride, out_items, out_scores,
+                                                            out_counts, sync ? *sync : none);
+    return cudaGetLastError();
+}
+
+template <int ORDER>
+static cudaError_t launch_merge_t(int n_lists, int n_queries, int k, const int64_t* items, const float* scores,
+                                  const int32_t* counts, int64_t items_stride, int64_t scores_stride,
+                                  int64_t counts_stride, int64_t* out_items, float* out_scores, int32_t* out_counts,
+                                  cudaStream_t s) {
+    const size_t smem = static_cast<size_t>(select_cap(k)) * sizeof(uint64_t);
+    static int granted[16] = {};
+    cudaError_t e = ensure_dynamic_smem(merge_kernel<ORDER>, smem, granted);
+    if (e != cudaSuccess) return e;
+    merge_kernel<ORDER><<<n_queries, kSelectThreads, smem, s>>>(n_lists, n_queries, k, items, scores, counts,
+                                                                items_stride, scores_stride, counts_stride, out_items,
+                                                                out_scores, out_counts, MergeSync{});
+    return cudaGetLastError();
+}
+
+cudaError_t launch_merge_ordered(int n_lists, int n_queries, int k, const int64_t* items, const float* scores,
+                                 const int32_t* counts, int64_t items_stride, int64_t scores_stride,
+                                 int64_t counts_stride, int order, int64_t* out_items, float* out_scores,
+                                 int32_t* out_counts, cudaStream_t s) {
+    if (items_stride == 0) items_stride = static_cast<int64_t>(n_queries) * k;
+    if (scores_stride == 0) scores_stride = static_cast<int64_t>(n_queries) * k;
+    if (counts_stride == 0) counts_stride = n_queries;
+#if TAV_SHARDED_FILTER_MUTANT == 1
+    order = 0;
+#endif
+    switch (order) {
+        case 0: return launch_merge_t<0>(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride,
+                                         counts_stride, out_items, out_scores, out_counts, s);
+        case 1: return launch_merge_t<1>(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride,
+                                         counts_stride, out_items, out_scores, out_counts, s);
+        case 2: return launch_merge_t<2>(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride,
+                                         counts_stride, out_items, out_scores, out_counts, s);
+        case 3: return launch_merge_t<3>(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride,
+                                         counts_stride, out_items, out_scores, out_counts, s);
+    }
+    return cudaErrorInvalidValue;
+}
+
+// ---- items[i] = table[items[i]] (subset positions -> global positions -> the caller's ordinals) --------
+__global__ void __launch_bounds__(256)
+map_items_kernel(int64_t n, const int64_t* __restrict__ table, int64_t table_len, int64_t* __restrict__ items) {
+    const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+    for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const int64_t v = items[i];
+        if (v >= 0 && v < table_len) items[i] = table[v];
+    }
+}
+
+cudaError_t launch_map_items(int64_t n, const int64_t* table, int64_t table_len, int64_t* items, cudaStream_t s) {
+    if (n == 0) return cudaSuccess;
+    const int64_t blocks = std::min<int64_t>((n + 255) / 256, 132 * 8);
+    map_items_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(n, table, table_len, items);
     return cudaGetLastError();
 }
 

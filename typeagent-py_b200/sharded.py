@@ -21,6 +21,13 @@ Threshold searches (``search_range``; ``max_hits=0`` lookups and ``search_arrays
 results whose size is known only after the local searches: they exchange over the process group (offsets, then
 the hits padded to the largest rank's total) and merge with ``tav_merge_range``.
 
+Filtered and subset lookups (``predicate=``, ``fuzzy_lookup_embedding_in_subset``, ``subset=`` / ``allowed=`` /
+``ties_low_first=``) return what ``VectorBase`` returns for the whole corpus, tie order included.  They exchange
+the packed layout over the process group and merge with ``tav_merge_topk_ordered``: a row mask (a predicate is
+evaluated by each rank over its own rows only) merges low row first where the reference's predicate path does;
+a subset is searched per rank with ``TAV_ITEMS_AS_POSITIONS``, its hits mapped to positions in the caller's
+subset (``tav_map_items``), merged by position and decoded through the caller's list at the end.
+
 ``torch`` is plumbing here (process group, device buffers); the search, exchange and merge are
 libtavec kernels.  The engine is injectable so that the host logic (partitioning, packing, gather,
 offsets) is testable on CPU with the ``gloo`` backend.
@@ -29,6 +36,7 @@ offsets) is testable on CPU with the ``gloo`` backend.
 from __future__ import annotations
 
 import ctypes as C
+from array import array as _array
 
 import numpy as np
 
@@ -196,25 +204,131 @@ class CudaShardEngine:
         )
         return items, scores, counts
 
+    # ---- filtered and subset lookups (per-rank steps) --------------------------------------
+    def _packed_views(self, buf, b: int, k: int):
+        off_s, off_c, _ = packed_layout(b, k)
+        return (buf[: b * k * 8].view(self.torch.int64).view(b, k),
+                buf[off_s: off_s + b * k * 4].view(self.torch.float32).view(b, k),
+                buf[off_c: off_c + b * 4].view(self.torch.int32))
+
+    def search_rows_packed(self, queries: np.ndarray, k: int, min_score: float, item_offset: int,
+                           ties_low_first: bool, mask=None, mask_key=None, mask_owner=None):
+        """``tav_search`` of host queries over this rank's rows into a packed buffer on the device (items shifted
+        by ``item_offset``): only rows whose bit is set in ``mask`` (this block's packed words; ``mask_key`` names
+        it, so an unchanged mask is not uploaded again), equal scores lower row first with ``ties_low_first``."""
+        torch = self.torch
+        b = len(queries)
+        buf = torch.empty(packed_layout(b, k)[2], dtype=torch.uint8, device=self.device)
+        items, scores, counts = self._packed_views(buf, b, k)
+        if self.n_local() == 0:
+            counts.zero_()
+            return buf
+        base = self.base
+        q = base._check_queries(queries)
+        lib, ix = base._ensure_device()
+        flags = base._flags() | _capi.TAV_OUTPUTS_ON_DEVICE
+        if mask is not None:
+            base._use_row_mask(lib, ix, mask, mask_key, mask_owner)
+            flags |= _capi.TAV_USE_ROW_MASK
+        if ties_low_first:
+            flags |= _capi.TAV_TIES_LOW_FIRST
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        with base._single_lock:
+            _capi.check(lib.tav_search(ix, q.ctypes.data_as(C.c_void_p), b, k, C.c_float(min_score), flags, None, 0,
+                                       item_offset, C.c_void_p(items.data_ptr()), C.c_void_p(scores.data_ptr()),
+                                       C.c_void_p(counts.data_ptr()), C.c_void_p(stream)))
+        return buf
+
+    def search_subset_packed(self, queries: np.ndarray, k: int, min_score: float, local_subset: np.ndarray,
+                             positions: np.ndarray, ties_low_first: bool):
+        """This rank's share of a subset search: ``tav_search`` over ``local_subset`` (block-local ordinals) with
+        TAV_ITEMS_AS_POSITIONS, then those positions mapped through ``positions`` (where the share's entries
+        stand in the whole subset, ascending) by ``tav_map_items``.  Returns the packed buffer on the device; its
+        items are positions in the caller's subset.  Host outputs, so that one query takes the single-launch
+        form as it does on one GPU; a rank without a share hands in empty lists."""
+        torch = self.torch
+        b = len(queries)
+        off_s, off_c, total = packed_layout(b, k)
+        host = np.zeros(total, np.uint8)
+        if len(local_subset):
+            base = self.base
+            q = base._check_queries(queries)
+            sub = np.ascontiguousarray(local_subset, np.int64)
+            lib, ix = base._ensure_device()
+            flags = base._flags() | _capi.TAV_ITEMS_AS_POSITIONS
+            if ties_low_first:
+                flags |= _capi.TAV_TIES_LOW_FIRST
+            items = host[: b * k * 8].view(np.int64)
+            scores = host[off_s: off_s + b * k * 4].view(np.float32)
+            counts = host[off_c: off_c + b * 4].view(np.int32)
+            with base._single_lock:
+                _capi.check(lib.tav_search(ix, q.ctypes.data_as(C.c_void_p), b, k, C.c_float(min_score), flags,
+                                           sub.ctypes.data_as(C.c_void_p), len(sub), 0, items.ctypes.data_as(C.c_void_p),
+                                           scores.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), None))
+        buf = torch.from_numpy(host).to(self.device)
+        if len(local_subset):
+            self.map_items(buf[: b * k * 8].view(torch.int64), positions)
+        return buf
+
+    def map_items(self, items, table: np.ndarray):
+        """In place on the device: items[i] = table[items[i]] where 0 <= items[i] < len(table) (``tav_map_items``);
+        ``items`` an int64 device tensor, ``table`` host int64."""
+        torch = self.torch
+        t = torch.from_numpy(np.ascontiguousarray(table, np.int64)).to(self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        _capi.check(_capi.load().tav_map_items(self.device.index, items.numel(), C.c_void_p(t.data_ptr()), t.numel(),
+                                               C.c_void_p(items.data_ptr()), C.c_void_p(stream)))
+        return items
+
+    def merge_ordered(self, gathered, world: int, n_queries: int, k: int, order: int):
+        """``merge`` with ``tav_merge_topk_ordered``'s tie order: 0 as ``merge``, 1 lower row first, 2 / 3 the
+        item (a subset position) higher / lower first.  ``gathered``: uint8 [world, row] with one rank's packed
+        buffer at the start of each row (a row may be longer, a multiple of 8 bytes)."""
+        torch = self.torch
+        off_s, off_c, _ = packed_layout(n_queries, k)
+        total = gathered.shape[1]
+        items = torch.empty((n_queries, k), dtype=torch.int64, device=self.device)
+        scores = torch.empty((n_queries, k), dtype=torch.float32, device=self.device)
+        counts = torch.empty((n_queries,), dtype=torch.int32, device=self.device)
+        base = gathered.data_ptr()
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        _capi.check(_capi.load().tav_merge_topk_ordered(
+            self.device.index, world, n_queries, k, C.c_void_p(base), C.c_void_p(base + off_s),
+            C.c_void_p(base + off_c), total // 8, total // 4, total // 4, int(order), C.c_void_p(items.data_ptr()),
+            C.c_void_p(scores.data_ptr()), C.c_void_p(counts.data_ptr()), C.c_void_p(stream)))
+        return items, scores, counts
+
     # ---- threshold search (search_range) ---------------------------------------------------
-    def range_local(self, queries: np.ndarray, min_score: float, item_offset: int, ties_low_first: bool):
+    def range_local(self, queries: np.ndarray, min_score: float, item_offset: int, ties_low_first: bool,
+                    mask=None, mask_key=None, mask_owner=None, subset=None, positions=None):
         """``tav_range_search`` on this rank's rows (items shifted by ``item_offset``).  Returns a
         ``LocalRange``: host offsets [B + 1] now, the hits later straight into the caller's buffers.  The
-        hits wait in the index between the two calls, so the base's lookup lock is held until then."""
+        hits wait in the index between the two calls, so the base's lookup lock is held until then.
+        ``mask`` as in ``search_rows_packed``.  ``subset`` / ``positions`` as in ``search_subset_packed``: the
+        hits' items are then positions in the caller's subset, and are fetched into device buffers only."""
         base = self.base
         b = len(queries)
-        if self.n_local() == 0:
+        if self.n_local() == 0 or (subset is not None and len(subset) == 0):
             return LocalRange(np.zeros(b + 1, np.int64), None, None)
         q = base._check_queries(queries)
+        sub = None if subset is None else np.ascontiguousarray(subset, np.int64)
         base._single_lock.acquire()
         try:
             lib, ix = base._ensure_device()
             flags = base._flags() & ~_capi.TAV_NO_FUSED_SCAN
             if ties_low_first:
                 flags |= _capi.TAV_TIES_LOW_FIRST
+            if mask is not None:
+                base._use_row_mask(lib, ix, mask, mask_key, mask_owner)
+                flags |= _capi.TAV_USE_ROW_MASK
+            if sub is not None:
+                flags |= _capi.TAV_ITEMS_AS_POSITIONS
+                item_offset = 0
             offsets = np.zeros(b + 1, np.int64)
-            _capi.check(lib.tav_range_search(ix, q.ctypes.data_as(C.c_void_p), b, C.c_float(min_score), flags, None, 0,
-                                             item_offset, base._range_hint, offsets.ctypes.data_as(C.c_void_p), None))
+            _capi.check(lib.tav_range_search(ix, q.ctypes.data_as(C.c_void_p), b, C.c_float(min_score), flags,
+                                             None if sub is None else sub.ctypes.data_as(C.c_void_p),
+                                             0 if sub is None else len(sub), item_offset, base._range_hint,
+                                             offsets.ctypes.data_as(C.c_void_p), None))
             base._range_hint = int(offsets[-1])
         except BaseException:
             base._single_lock.release()
@@ -226,10 +340,14 @@ class CudaShardEngine:
             if n == 0:
                 return
             on_device = not isinstance(items, np.ndarray)
+            if sub is not None and not on_device:
+                raise ValueError("the hits of a subset threshold search are fetched into device buffers")
             ip = C.c_void_p(items.data_ptr()) if on_device else items.ctypes.data_as(C.c_void_p)
             sp = C.c_void_p(scores.data_ptr()) if on_device else scores.ctypes.data_as(C.c_void_p)
             _capi.check(lib.tav_range_fetch(ix, 0, n, ip, sp, _capi.TAV_OUTPUTS_ON_DEVICE if on_device else 0,
                                             C.c_void_p(stream) if on_device else None))
+            if sub is not None:
+                self.map_items(items[:n], positions)
 
         return LocalRange(offsets, fetch, base._single_lock)
 
@@ -276,6 +394,66 @@ def pack_range_payload(local, t_pad: int, device):
     n = int(local.offsets[-1])
     local.fetch(send[: 8 * n].view(torch.int64), send[8 * t_pad: 8 * t_pad + 4 * n].view(torch.float32))
     return send
+
+
+def subset_ordinals(subset, from_list: bool = False) -> np.ndarray:
+    """A caller's subset as int64 [m], read as ``VectorBase`` reads it: IndexError for a non-integer array
+    (``from_list``: a Python list goes through ``array('q')`` first, as ``fuzzy_lookup_embedding_in_subset``
+    takes it)."""
+    if from_list and type(subset) is list:
+        try:
+            return np.frombuffer(_array("q", subset), dtype=np.int64)
+        except (TypeError, OverflowError):
+            pass
+    sub = np.ascontiguousarray(subset)
+    if sub.size and not np.issubdtype(sub.dtype, np.integer):
+        raise IndexError("arrays used as indices must be of integer (or boolean) type")
+    return sub.astype(np.int64, copy=False).reshape(-1)
+
+
+def check_subset(sub: np.ndarray, n_rows: int) -> None:
+    """IndexError, with the library's message, for an ordinal outside [-n_rows, n_rows)."""
+    bad = (sub < -n_rows) | (sub >= n_rows)
+    if bad.any():
+        raise IndexError(f"index {int(sub[bad][0])} is out of bounds for axis 0 with size {n_rows}")
+
+
+def subset_share(sub: np.ndarray, n_rows: int, lo: int, hi: int) -> tuple[np.ndarray, np.ndarray]:
+    """The entries of a subset that fall in rows [lo, hi): their positions in the subset (ascending) and their
+    block-local ordinals.  Negative ordinals wrap with the global row count; a repeated ordinal is one entry
+    per occurrence."""
+    rows = np.where(sub < 0, sub + n_rows, sub)
+    pos = np.flatnonzero((rows >= lo) & (rows < hi)).astype(np.int64)
+    return pos, rows[pos] - lo
+
+
+def block_mask(allowed, n_rows: int, lo: int, hi: int) -> np.ndarray:
+    """Rows [lo, hi) of a row mask over n_rows rows (bool [n_rows], or packed uint32 words as
+    ``VectorBase.pack_row_mask`` makes them), packed again from bit 0: a block need not start on a word.
+    ValueError, with ``VectorBase``'s message, for a mask of the wrong length."""
+    if getattr(allowed, "dtype", None) == np.uint32:
+        words = np.ascontiguousarray(allowed)
+        if len(words) != (n_rows + 31) // 32:
+            raise ValueError(f"row mask has {len(words) * 32} bits for {n_rows} rows")
+        bits = np.unpackbits(words.view(np.uint8), bitorder="little")[lo:hi].astype(bool)
+    else:
+        if len(allowed) != n_rows:
+            raise ValueError(f"row mask has {len(allowed)} entries for {n_rows} rows")
+        bits = np.asarray(allowed, dtype=bool)[lo:hi]
+    return VectorBase.pack_row_mask(bits)
+
+
+def as_topk_arrays(offsets, hits, hit_scores, b: int, k: int):
+    """CSR threshold-search results laid out as [B, k] top-k arrays (-1 / 0 padding), as ``tav_search`` lays
+    out a search it routes to the threshold engine."""
+    counts = np.diff(offsets).astype(np.int32)
+    items = np.full((b, k), -1, np.int64)
+    scores = np.zeros((b, k), np.float32)
+    cols = np.arange(len(hits)) - np.repeat(offsets[:-1], counts)
+    rows = np.repeat(np.arange(b), counts)
+    items[rows, cols] = hits
+    scores[rows, cols] = hit_scores
+    return items, scores, counts
 
 
 class LocalRange:
@@ -328,6 +506,8 @@ class ShardedVectorBase:
         self._starts = [0] * (self.world + 1)  # global row where each rank's block starts
         self._embedding_size = 0
         self._pending: list = []  # deferred searches since the last finish(): ["group"] or (local, b, k, out) tuples
+        self._generation = 0      # bumped whenever rows are replaced or removed (part of the mask cache keys)
+        self._masks: dict = {}    # (kind, id(mask or predicate), generation, rows) -> (this block's words, owner)
 
     # ---- corpus ------------------------------------------------------------------------
     def __len__(self) -> int:
@@ -346,6 +526,7 @@ class ShardedVectorBase:
     def deserialize(self, data: np.ndarray | None) -> None:
         """Bulk load: every rank passes the same global float32 [N, D] array (or a
         memory-map of it) and keeps only its own block."""
+        self._generation += 1
         if data is None or data.ndim < 2 or len(data) == 0:
             self._engine.load_rows(None)
             self._starts = [0] * (self.world + 1)
@@ -364,6 +545,7 @@ class ShardedVectorBase:
         if len(rows) != hi - lo:
             raise ValueError(f"rank {self.rank} must hold rows [{lo}, {hi}), got {len(rows)} rows")
         self._set_bounds(bounds)
+        self._generation += 1
         self._embedding_size = rows.shape[1]
         if isinstance(rows, np.ndarray):
             self._engine.load_rows(rows)
@@ -405,6 +587,7 @@ class ShardedVectorBase:
             self._engine.remove_rows(mine)
         starts = np.asarray(self._starts, np.int64)
         self._starts = (starts - np.searchsorted(removed, starts, side="left")).tolist()
+        self._generation += 1
 
     # ---- lookups -----------------------------------------------------------------------
     def _gather_and_merge(self, local, b: int, k: int):
@@ -479,7 +662,14 @@ class ShardedVectorBase:
                 out[0].copy_(items), out[1].copy_(scores), out[2].copy_(counts)
         return total
 
-    def search_arrays(self, queries: np.ndarray, k: int, min_score: float = 0.0):
+    def search_arrays(self, queries: np.ndarray, k: int, min_score: float = 0.0, subset=None, allowed=None,
+                      ties_low_first: bool = False):
+        """SPMD batched lookup, replicated on every rank: items int64 [B, k], scores float32 [B, k], counts int32
+        [B].  ``subset``, ``allowed`` and ``ties_low_first`` as ``VectorBase.search_arrays`` takes them over the
+        whole corpus (global ordinals; ``allowed`` a bool [N] mask or its packed words), with its results and
+        errors; such lookups exchange over the process group whatever ``exchange`` says."""
+        if subset is not None or allowed is not None or ties_low_first:
+            return self._search_arrays_filtered(queries, k, min_score, subset, allowed, ties_low_first)
         q = np.ascontiguousarray(queries, dtype=np.float32)
         if q.ndim == 1:
             q = q.reshape(1, -1)
@@ -491,52 +681,211 @@ class ShardedVectorBase:
         n = len(self)
         if k >= n > RANGE_ROUTE_MIN_ROWS and hasattr(self._engine, "range_local"):
             # every passing row, as tav_search routes it on one GPU: one threshold search, laid out [B, n]
-            offsets, hits, hit_scores = self.search_range(q, min_score)
-            counts = np.diff(offsets).astype(np.int32)
-            items = np.full((len(q), n), -1, np.int64)
-            scores = np.zeros((len(q), n), np.float32)
-            cols = np.arange(len(hits)) - np.repeat(offsets[:-1], counts)
-            rows = np.repeat(np.arange(len(q)), counts)
-            items[rows, cols] = hits
-            scores[rows, cols] = hit_scores
-            return items, scores, counts
+            return as_topk_arrays(*self.search_range(q, min_score), len(q), n)
         items, scores, counts = self.search_tensors(q, k, min_score)
         return items.cpu().numpy(), scores.cpu().numpy(), counts.cpu().numpy()
 
-    def search_range(self, queries, min_score: float = 0.0, ties_low_first: bool = False):
+    # ---- filtered and subset lookups ------------------------------------------------------
+    def _check_queries(self, queries) -> np.ndarray:
+        q = np.ascontiguousarray(queries, dtype=np.float32)
+        if q.ndim == 1:
+            q = q.reshape(1, -1)
+        if q.ndim != 2 or q.shape[1] != self._embedding_size:
+            raise ValueError(f"shapes ({len(self)},{self._embedding_size}) and {tuple(np.shape(queries))} not aligned")
+        return q
+
+    def _remember(self, key, words, owner) -> None:
+        if len(self._masks) > 8:
+            self._masks.clear()
+        self._masks[key] = (words, owner)  # keeps the owner, and so its id(), alive
+
+    def _block_mask(self, allowed):
+        """(this block's packed words of ``allowed``, its cache key); errors on every rank alike."""
+        key = ("allowed", id(allowed), self._generation, len(self))
+        hit = self._masks.get(key)
+        if hit is None:
+            lo, hi = self.local_range
+            self._remember(key, block_mask(allowed, len(self), lo, hi), allowed)
+            hit = self._masks[key]
+        return hit[0], key, allowed
+
+    def _predicate_mask(self, predicate):
+        """The predicate over this rank's rows only (global ordinals [lo, hi)), packed, cached per (predicate,
+        row generation, rows).  A predicate that raises on one rank raises on every rank (one all-reduce, only
+        when the mask is built)."""
+        key = ("predicate", id(predicate), self._generation, len(self))
+        hit = self._masks.get(key)
+        if hit is None:
+            lo, hi = self.local_range
+            error, words = None, None
+            try:
+                accepted = np.fromiter((bool(predicate(i)) for i in range(lo, hi)), dtype=bool, count=hi - lo)
+                words = VectorBase.pack_row_mask(accepted)
+            except Exception as e:  # noqa: BLE001
+                error = e
+            if self._any_failed(error is not None):
+                raise error if error is not None else RuntimeError("the predicate raised on another rank")
+            self._remember(key, words, predicate)
+            hit = self._masks[key]
+        return hit[0], key, predicate
+
+    def _any_failed(self, failed: bool) -> bool:
+        if self.world == 1:
+            return failed
+        import torch
+
+        dev = self._engine.comm_device() if hasattr(self._engine, "comm_device") else torch.device("cpu")
+        flag = torch.tensor([int(failed)], dtype=torch.int64, device=dev)
+        self._dist.all_reduce(flag, group=self._group)
+        return bool(flag.item())
+
+    def _exchange_topk(self, search, b: int, k: int, order: int):
+        """The local top-k search ``search()`` (a packed buffer), the packed all-gather over the process group and
+        the merge with ``tav_merge_topk_ordered``'s ``order``.  Every rank's buffer travels with a status word
+        behind it, so that a local failure raises on every rank instead of leaving the others in the collective."""
+        import torch
+
+        error, local = None, None
+        try:
+            local = search()
+        except Exception as e:  # noqa: BLE001
+            error = e
+        if self.world == 1:
+            if error is not None:
+                raise error
+            return self._engine.merge_ordered(local.view(1, -1), 1, b, k, order)
+        total = packed_layout(b, k)[2]
+        dev = self._engine.comm_device() if hasattr(self._engine, "comm_device") else torch.device("cpu")
+        send = torch.zeros(total + 8, dtype=torch.uint8, device=dev)
+        if local is not None:
+            send[:total].copy_(local.view(-1))
+        else:
+            send[total:] = 1
+        gathered = torch.empty((self.world, total + 8), dtype=torch.uint8, device=dev)
+        self._dist.all_gather_into_tensor(gathered.view(-1), send, group=self._group)
+        if gathered[:, total:].any().item():
+            raise error if error is not None else RuntimeError("a lookup failed on another rank")
+        return self._engine.merge_ordered(gathered, self.world, b, k, order)
+
+    def _search_arrays_filtered(self, queries, k, min_score, subset, allowed, ties_low_first, mask=None):
+        """``VectorBase.search_arrays`` with a subset, a row mask (``allowed``, or ``mask`` = this block's words,
+        key, owner as ``_block_mask`` returns them) or ties low-first, checks in its order."""
+        q = self._check_queries(queries)
+        b = len(q)
+        if k < 1:
+            raise ValueError("k must be >= 1")
+        n_rows = len(self)
+        sub = None
+        if subset is not None:
+            sub = subset_ordinals(subset)
+            n_rows = len(sub)
+        k_eff = max(1, min(k, n_rows))
+        items = np.full((b, k_eff), -1, dtype=np.int64)
+        scores = np.zeros((b, k_eff), dtype=np.float32)
+        counts = np.zeros(b, dtype=np.int32)
+        floor = _as_f32_scalar(min_score)
+        # early returns and errors on replicated state only: every rank takes them together
+        if b == 0 or n_rows == 0 or len(self) == 0 or np.isnan(floor):
+            return items, scores, counts
+        if allowed is not None and sub is not None:
+            raise ValueError("allowed= and subset= cannot be combined")
+        if allowed is not None:
+            mask = self._block_mask(allowed)
+        if sub is not None:
+            check_subset(sub, len(self))
+        if k_eff >= n_rows > RANGE_ROUTE_MIN_ROWS:
+            # every passing row, as tav_search routes it on one GPU: one threshold search, laid out [B, n_rows]
+            csr = self._search_range_filtered(q, floor, ties_low_first, sub, mask)
+            return as_topk_arrays(*csr, b, k_eff)
+        lo, hi = self.local_range
+        if sub is not None:
+            positions, local_sub = subset_share(sub, len(self), lo, hi)
+            items_t, scores_t, counts_t = self._exchange_topk(
+                lambda: self._engine.search_subset_packed(q, k_eff, float(floor), local_sub, positions, ties_low_first),
+                b, k_eff, 3 if ties_low_first else 2)
+            self._engine.map_items(items_t, sub)  # subset positions -> the caller's ordinals, as given
+        else:
+            if mask is not None:
+                self.finish()  # the mask upload finishes this rank's deferred searches; their exchange is redone here
+            words, key, owner = mask if mask is not None else (None, None, None)
+            items_t, scores_t, counts_t = self._exchange_topk(
+                lambda: self._engine.search_rows_packed(q, k_eff, float(floor), lo, ties_low_first, words, key, owner),
+                b, k_eff, 1 if ties_low_first else 0)
+        return items_t.cpu().numpy(), scores_t.cpu().numpy(), counts_t.cpu().numpy()
+
+    def search_range(self, queries, min_score: float = 0.0, ties_low_first: bool = False, subset=None, allowed=None):
         """Threshold search over the whole corpus: EVERY row whose score is >= min_score, per query, as
         ``VectorBase.search_range`` returns it on one GPU — CSR numpy arrays offsets int64 [B + 1], items int64
-        [T], scores float32 [T], in the library's order — replicated on every rank.  SPMD.
+        [T], scores float32 [T], in the library's order — replicated on every rank.  SPMD.  ``subset`` (global
+        ordinals) and ``allowed`` (bool [N] or packed words) as ``VectorBase.search_range`` takes them, with its
+        errors.
 
         Each rank runs the threshold search on its rows; one all-gather carries every rank's offsets (and a
         status word, so that a rank's failure raises on every rank instead of leaving the others in the next
         collective), a second one every rank's hits, padded to the largest rank's total (after a one-word
         all-reduce that makes a failure to stage them raise on every rank); ``tav_merge_range`` merges them on
-        every rank.  The exchanges go through the process group whatever ``exchange`` says.  At most
+        every rank.  A subset search merges positions in the subset and decodes them through the caller's list
+        afterwards.  The exchanges go through the process group whatever ``exchange`` says.  At most
         ``MAX_RANGE_RANKS`` (32) ranks: larger groups get ValueError on every rank before any exchange."""
-        import torch
-
+        if subset is not None or allowed is not None:
+            q = self._check_queries(queries)
+            sub = None if subset is None else subset_ordinals(subset)
+            if allowed is not None and sub is not None:
+                raise ValueError("allowed= and subset= cannot be combined")
+            floor = _as_f32_scalar(min_score)
+            n_rows = len(self) if sub is None else len(sub)
+            if len(q) == 0 or n_rows == 0 or len(self) == 0 or np.isnan(floor):
+                return np.zeros(len(q) + 1, np.int64), np.empty(0, np.int64), np.empty(0, np.float32)
+            mask = self._block_mask(allowed) if allowed is not None else None
+            if sub is not None:
+                check_subset(sub, len(self))
+            return self._search_range_filtered(q, floor, ties_low_first, sub, mask)
         q = np.ascontiguousarray(queries, dtype=np.float32)
         if q.ndim == 1:
             q = q.reshape(1, -1)
         b = len(q)
         floor = _as_f32_scalar(min_score)
-        empty = (np.zeros(b + 1, np.int64), np.empty(0, np.int64), np.empty(0, np.float32))
         # early returns on replicated state only: every rank takes them together
         if b == 0 or len(self) == 0 or np.isnan(floor):
-            return empty
+            return np.zeros(b + 1, np.int64), np.empty(0, np.int64), np.empty(0, np.float32)
         if q.shape[1] != self._embedding_size:
             raise ValueError("query width does not match the embedding size")
+        lo, _ = self.local_range
+        return self._range_exchange(q, floor, ties_low_first,
+                                    lambda: self._engine.range_local(q, float(floor), lo, bool(ties_low_first)))
+
+    def _search_range_filtered(self, q, floor, ties_low_first, sub, mask):
+        """The threshold search of validated arguments with a subset (int64, in range), this block's mask, or
+        neither (ties low-first alone)."""
+        lo, hi = self.local_range
+        if sub is not None:
+            positions, local_sub = subset_share(sub, len(self), lo, hi)
+            return self._range_exchange(q, floor, ties_low_first, lambda: self._engine.range_local(
+                q, float(floor), lo, bool(ties_low_first), subset=local_sub, positions=positions), decode=sub)
+        if mask is None:
+            return self._range_exchange(q, floor, ties_low_first, lambda: self._engine.range_local(
+                q, float(floor), lo, bool(ties_low_first)))
+        self.finish()  # the mask upload finishes this rank's deferred searches; their exchange is redone here
+        words, key, owner = mask
+        return self._range_exchange(q, floor, ties_low_first, lambda: self._engine.range_local(
+            q, float(floor), lo, bool(ties_low_first), mask=words, mask_key=key, mask_owner=owner))
+
+    def _range_exchange(self, q, floor, ties_low_first, search, decode=None):
+        """Both exchanges and the merge of a threshold search whose local part is ``search()`` (a LocalRange);
+        ``decode``: merged items are positions in this list, replaced by its entries on the device."""
+        import torch
+
+        b = len(q)
+        empty = (np.zeros(b + 1, np.int64), np.empty(0, np.int64), np.empty(0, np.float32))
         if self.world > MAX_RANGE_RANKS:
             raise ValueError(f"search_range merges at most {MAX_RANGE_RANKS} ranks (tav_merge_range), not {self.world}")
-        lo, _ = self.local_range
         error, local = None, None
         try:
-            local = self._engine.range_local(q, float(floor), lo, bool(ties_low_first))
+            local = search()
             offsets = np.asarray(local.offsets, np.int64)
         except Exception as e:  # noqa: BLE001
             error, offsets = e, np.zeros(b + 1, np.int64)
-        if self.world == 1:
+        if self.world == 1 and decode is None:
             if error is not None:
                 raise error
             total = int(offsets[-1])
@@ -549,7 +898,7 @@ class ShardedVectorBase:
             mine = torch.from_numpy(offsets_with_status(offsets, error is not None)).to(dev)
             flag = torch.zeros(1, dtype=torch.int64, device=dev)
             offsets_all = torch.empty((self.world, b + 2), dtype=torch.int64, device=dev)
-            self._dist.all_gather_into_tensor(offsets_all.view(-1), mine, group=self._group)
+            self._all_gather(offsets_all, mine)
             host = offsets_all.cpu().numpy()
             if host[:, -1].any():
                 raise error if error is not None else RuntimeError("search_range: another rank's threshold search failed")
@@ -567,16 +916,25 @@ class ShardedVectorBase:
             except Exception as e:  # noqa: BLE001
                 stage_error = e
             flag.fill_(int(stage_error is not None))
-            self._dist.all_reduce(flag, group=self._group)
+            if self.world > 1:
+                self._dist.all_reduce(flag, group=self._group)
             if int(flag.item()):
                 raise stage_error if stage_error is not None else RuntimeError(
                     "search_range: another rank failed to stage its hits")
-            self._dist.all_gather_into_tensor(payload.view(-1), send, group=self._group)
+            self._all_gather(payload, send)
             out = self._engine.merge_range(offsets_all, payload, self.world, b, t_pad, total, bool(ties_low_first))
+            if decode is not None:
+                self._engine.map_items(out[1], decode)  # subset positions -> the caller's ordinals, as given
             return tuple(np.asarray(t.cpu().numpy() if hasattr(t, "cpu") else t) for t in out)
         finally:
             if local is not None:
                 local.release()
+
+    def _all_gather(self, out, mine) -> None:
+        if self.world == 1:
+            out.view(-1).copy_(mine.view(-1))
+        else:
+            self._dist.all_gather_into_tensor(out.view(-1), mine, group=self._group)
 
     def fuzzy_lookup_embeddings(self, embeddings, max_hits=None, min_score=None):
         if min_score is None:
@@ -594,6 +952,45 @@ class ShardedVectorBase:
         il, sl, cl = items.tolist(), scores.tolist(), counts.tolist()
         return [[ScoredInt(i, s) for i, s in zip(il[b][:c], sl[b][:c])] for b, c in enumerate(cl)]
 
-    def fuzzy_lookup_embedding(self, embedding, max_hits=None, min_score=None):
-        return self.fuzzy_lookup_embeddings(np.asarray(embedding, np.float32).reshape(1, -1),
-                                            max_hits, min_score)[0]
+    def fuzzy_lookup_embedding(self, embedding, max_hits=None, min_score=None, predicate=None):
+        """``VectorBase.fuzzy_lookup_embedding`` over the whole corpus.  With a predicate: every row at or above
+        min_score that satisfies it, equal scores lower ordinal first (the reference's stable sort), first
+        max_hits; ``max_hits=0`` returns [].  Each rank evaluates the predicate on its own rows only, once per
+        (predicate, rows) while the rows stay as they are, and the search runs with that row mask."""
+        if predicate is None:
+            return self.fuzzy_lookup_embeddings(np.asarray(embedding, np.float32).reshape(1, -1),
+                                                max_hits, min_score)[0]
+        if min_score is None:
+            min_score = 0.0
+        n = len(self)
+        if n == 0:
+            return []
+        k = VectorBase._resolve_k(max_hits, n)
+        if max_hits == 0:  # the reference's predicate path slices `[:0]` (vectorbase.py:201)
+            return []
+        mask = self._predicate_mask(predicate)
+        items, scores, counts = self._search_arrays_filtered(embedding, k, min_score, None, None, True, mask=mask)
+        c = int(counts[0])
+        return [ScoredInt(i, s_) for i, s_ in zip(items[0, :c].tolist(), scores[0, :c].tolist())]
+
+    def fuzzy_lookup_embedding_in_subset(self, embedding, ordinals_of_subset, max_hits=None, min_score=None):
+        """``VectorBase.fuzzy_lookup_embedding_in_subset`` over the whole corpus: only the given global ordinals
+        (negative ones wrap; a repeated ordinal is a separate hit), items as given, equal scores the later
+        subset position first.  IndexError on every rank, before any exchange, for an ordinal out of range or a
+        non-integer one."""
+        if min_score is None:
+            min_score = 0.0
+        if len(ordinals_of_subset) == 0 or len(self) == 0:
+            return []
+        k = VectorBase._resolve_k(max_hits, len(ordinals_of_subset))
+        q = np.asarray(embedding, dtype=np.float32)
+        if q.ndim == 2 and q.shape[0] == 1:
+            q = q.reshape(-1)
+        if q.ndim != 1 or q.shape[0] != self._embedding_size:
+            raise ValueError(f"shapes ({len(self)},{self._embedding_size}) and {tuple(np.shape(embedding))} not aligned")
+        if np.isnan(np.float32(min_score)):  # `scores >= nan` is all-false in the reference
+            return []
+        sub = subset_ordinals(ordinals_of_subset, from_list=True)
+        items, scores, counts = self._search_arrays_filtered(q, k, min_score, sub, None, False)
+        c = int(counts[0])
+        return [ScoredInt(i, s_) for i, s_ in zip(items[0, :c].tolist(), scores[0, :c].tolist())]
