@@ -99,7 +99,13 @@ enum tav_search_flags {
      * the order are unchanged.  A row-sharded subset search uses it: positions stay distinct when the
      * subset repeats an ordinal, so the ranks' lists can be merged by position (tav_merge_topk_ordered
      * orders 2 / 3, tav_merge_range) and decoded through the caller's list afterwards (tav_map_items). */
-    TAV_ITEMS_AS_POSITIONS = 256
+    TAV_ITEMS_AS_POSITIONS = 256,
+    /* Per-query row masks: query q may return only rows whose bit is set in mask q of
+     * tav_set_query_masks.  n_queries must equal the number of masks set (else TAV_ERR_INVALID); with
+     * TAV_USE_ROW_MASK or a subset: TAV_ERR_INVALID; without current masks: TAV_ERR_STATE.  Every path
+     * (row scan, tensor cores, the exact redo, the threshold search and its re-pass) gives each query
+     * exactly what a one-query search with its mask as the row mask gives. */
+    TAV_USE_QUERY_MASKS = 512
 };
 
 int tav_abi_version(void);
@@ -214,6 +220,17 @@ int tav_finish_search(tav_index* ix, void* stream, int* redone);
  * (tav_clear / tav_adopt_device / tav_remove_rows drop it; appends invalidate it) or n_rows == 0
  * clears it.  tav_write_rows keeps it. */
 int tav_set_row_mask(tav_index* ix, const uint32_t* bits, int64_t n_rows, int on_device, void* stream);
+
+/* Per-query masks for TAV_USE_QUERY_MASKS: mask q is ceil(n_rows / 32) words (the bit order of
+ * tav_set_row_mask) starting at bits + q * stride_words, in host or device memory.  n_rows must equal
+ * tav_size() and stride_words must be at least ceil(n_rows / 32).  The masks are copied into library-owned
+ * device memory, each padded to whole 256-row tiles: about n_queries * n_rows / 8 bytes.  An allocation
+ * failure gives TAV_ERR_OOM and leaves the index usable, without masks.  n_queries == 0 clears them.  Same
+ * lifecycle and ordering as the row mask: the call joins the index's call order, outstanding TAV_DEFER_RETRY
+ * searches are finished first (their exact redo reads the masks they were issued with); tav_clear,
+ * tav_adopt_device and tav_remove_rows drop the masks, appends invalidate them, tav_write_rows keeps them. */
+int tav_set_query_masks(tav_index* ix, const uint32_t* bits, int n_queries, int64_t n_rows, int64_t stride_words,
+                        int on_device, void* stream);
 
 /*
  * Merge step of the row-sharded search (SURVEY.md §8e): `n_lists` per-shard results of

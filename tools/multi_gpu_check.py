@@ -148,9 +148,21 @@ def main():
                 whole.fuzzy_lookup_embedding(q[i], 10, 0.3, predicate=pred)
             assert sh.fuzzy_lookup_embedding_in_subset(q[i], sub.tolist(), 20, 0.3) == \
                 whole.fuzzy_lookup_embedding_in_subset(q[i], sub.tolist(), 20, 0.3)
+        # per-query masks (2-D allowed=): each rank cuts its block's columns out of every query's mask
+        qmasks = rng.random((b, n)) < np.array([0.3, 0.01, 1.0, 0.001] * b)[:b, None]
+        qmasks[::2, :500] = True
+        for tl in (False, True):
+            for got, want in ((sh.search_arrays(q, 100, 0.4, allowed=qmasks, ties_low_first=tl),
+                               whole.search_arrays(q, 100, 0.4, allowed=qmasks, ties_low_first=tl)),
+                              (sh.search_range(q, 0.6, ties_low_first=tl, allowed=qmasks),
+                               whole.search_range(q, 0.6, allowed=qmasks, ties_low_first=tl))):
+                for g, w in zip(got, want):
+                    np.testing.assert_array_equal(g.view(np.uint32) if g.dtype == np.float32 else g,
+                                                  w.view(np.uint32) if w.dtype == np.float32 else w)
         dist.barrier()
         if rank == 0:
-            print(f"multi-gpu ok: world={world} filtered and subset lookups {storage} n={n} d={d} b={b}", flush=True)
+            print(f"multi-gpu ok: world={world} filtered, subset and per-query-mask lookups {storage} n={n} d={d} "
+                  f"b={b}", flush=True)
     dist.destroy_process_group()
 
 

@@ -20,6 +20,7 @@ DTYPE_NAMES = {v: k for k, v in DTYPE_CODES.items()}
 TAV_NORMALIZE = 1
 TAV_QUERIES_ON_DEVICE, TAV_OUTPUTS_ON_DEVICE, TAV_FORCE_SCAN, TAV_FORCE_MMA, TAV_DEFER_RETRY = 1, 2, 4, 8, 16
 TAV_USE_ROW_MASK, TAV_TIES_LOW_FIRST, TAV_NO_FUSED_SCAN, TAV_ITEMS_AS_POSITIONS = 32, 64, 128, 256
+TAV_USE_QUERY_MASKS = 512
 ABI_VERSION = 2
 
 TAV_ERR_INVALID, TAV_ERR_CUDA, TAV_ERR_OOM, TAV_ERR_RANGE, TAV_ERR_STATE = -1, -2, -3, -4, -5
@@ -54,6 +55,7 @@ SIGNATURES = {
     "tav_range_fetch": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "tav_finish_search": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
     "tav_set_row_mask": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
+    "tav_set_query_masks": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p]),
     "tav_fold_groups": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tav_group_handle_bytes": (C.c_int, []),

@@ -122,7 +122,9 @@ struct Pending {
     float* scores;
     int32_t* counts;
     int slot;
-    bool split, masked;
+    bool split;
+    const uint32_t* mask;  // the row mask, or query 0's per-query mask (query q's: mask + q * mask_stride)
+    int64_t mask_stride;   // 0 for the row mask
 };
 
 }  // namespace tav
@@ -187,8 +189,13 @@ struct tav_index {
     // predicate pushdown: one bit per row (tav_set_row_mask)
     DevBuf row_mask;
     int64_t row_mask_rows = 0;   // 0 = no mask set
+    // per-query masks (tav_set_query_masks): qmask_n rows of qmask_stride words, and their popcounts
+    DevBuf qmask, qmask_pop;
+    int qmask_n = 0;             // 0 = no masks set
+    int64_t qmask_rows = 0;
+    int64_t qmask_stride = 0;
     // threshold search (tav_range_search): collect regions, re-pass regions, sort scratch, CSR result
-    DevBuf range_keys, range_keys2, range_counts, range_qgather, range_tmp, range_sortws;
+    DevBuf range_keys, range_keys2, range_counts, range_qgather, range_qmap, range_tmp, range_sortws;
     DevBuf range_mmaws, range_mmaws2, range_mmaaux;  // tensor-core collection: workspaces, scratch
     DevBuf range_items, range_scores;
     int64_t range_total = 0;     // hits of the last range search held in range_items / range_scores
@@ -391,6 +398,7 @@ int tav_destroy(tav_index* ix) {
     if (ix->rows && !ix->adopted) cudaFree(ix->rows);
     for (DevBuf* b : {&ix->queries, &ix->held_queries, &ix->subset, &ix->cand_keys, &ix->cand_count, &ix->out_pack, &ix->staging,
                       &ix->mma_ws, &ix->retry, &ix->split_hi, &ix->split_lo, &ix->split_flag, &ix->row_mask,
+                      &ix->qmask, &ix->qmask_pop, &ix->range_qmap,
                       &ix->range_keys, &ix->range_keys2, &ix->range_counts, &ix->range_qgather, &ix->range_tmp,
                       &ix->range_sortws, &ix->range_items, &ix->range_scores, &ix->range_mmaws,
                       &ix->range_mmaws2, &ix->range_mmaaux, &ix->compact_keys})
@@ -424,6 +432,7 @@ int tav_clear(tav_index* ix) {
     // (the "a corpus value left the fp16 range" flag is reset where the planes are rebuilt from row 0)
     ix->split_rows = 0;
     ix->row_mask_rows = 0;
+    ix->qmask_n = 0;
     return TAV_OK;
 }
 
@@ -528,6 +537,7 @@ int tav_adopt_device(tav_index* ix, void* device_rows, int64_t n, int dim) {
     ix->rows = device_rows;
     ix->split_rows = 0;  // (the planes' overflow flag is reset where they are rebuilt from row 0)
     ix->row_mask_rows = 0;
+    ix->qmask_n = 0;
     ix->adopted = true;
     ix->size = n;
     ix->capacity = n;
@@ -598,6 +608,62 @@ int tav_set_row_mask(tav_index* ix, const uint32_t* bits, int64_t n_rows, int on
     return TAV_OK;
 }
 
+int tav_set_query_masks(tav_index* ix, const uint32_t* bits, int n_queries, int64_t n_rows, int64_t stride_words,
+                        int on_device, void* stream) {
+    if (!ix || n_queries < 0 || n_rows < 0 || (n_queries > 0 && !bits)) return TAV_ERR_INVALID;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (int rc = set_device(ix)) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;  // queued searches read the old masks
+    if (!ix->pending.empty()) {  // an outstanding search may still need the old masks for its exact redo
+        int redone = 0;
+        if (int rc = finish_pending(ix, s, &redone)) return rc;
+    }
+    if (n_queries == 0) {
+        ix->qmask_n = 0;
+        return TAV_OK;
+    }
+    const int64_t src_words = (n_rows + 31) / 32;
+    if (n_rows != ix->size || n_rows == 0) {
+        set_error("tav_set_query_masks: %lld bits per mask for an index of %lld rows", (long long)n_rows,
+                  (long long)ix->size);
+        return TAV_ERR_INVALID;
+    }
+    if (stride_words < src_words) {
+        set_error("tav_set_query_masks: stride of %lld words is below the %lld words of a mask", (long long)stride_words,
+                  (long long)src_words);
+        return TAV_ERR_INVALID;
+    }
+    // each mask padded to whole 256-row tiles, as the row mask (the tensor-core epilogue reads one word per 32 rows)
+    const int64_t words = (n_rows + 255) / 256 * 8;
+    const size_t bytes = static_cast<size_t>(n_queries) * words * sizeof(uint32_t);
+    ix->qmask_n = 0;
+    cudaError_t e = ix->qmask.ensure(bytes);
+    if (e == cudaSuccess) e = ix->qmask_pop.ensure(static_cast<size_t>(n_queries) * sizeof(uint32_t));
+    if (e != cudaSuccess) {
+        cudaGetLastError();  // no sticky error: the index stays usable
+        ix->qmask.release();
+        ix->qmask_pop.release();
+        set_error("tav_set_query_masks: cannot allocate %zu bytes for %d masks: %s", bytes, n_queries, cudaGetErrorString(e));
+        return e == cudaErrorMemoryAllocation ? TAV_ERR_OOM : TAV_ERR_CUDA;
+    }
+    TAV_CUDA(cudaMemsetAsync(ix->qmask.p, 0, bytes, s));
+    TAV_CUDA(cudaMemcpy2DAsync(ix->qmask.p, static_cast<size_t>(words) * sizeof(uint32_t), bits,
+                               static_cast<size_t>(stride_words) * sizeof(uint32_t),
+                               static_cast<size_t>(src_words) * sizeof(uint32_t), static_cast<size_t>(n_queries),
+                               on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
+    // (bits beyond n_rows are never tested: the kernels test rows < n_rows only, and the popcount ignores them)
+    TAV_CUDA(launch_mask_popcount(static_cast<const uint32_t*>(ix->qmask.p), n_queries, n_rows, words,
+                                  static_cast<uint32_t*>(ix->qmask_pop.p), s));
+    ix->qmask_n = n_queries;
+    ix->qmask_rows = n_rows;
+    ix->qmask_stride = words;
+    if (on_device) return mark_queued(ix, s);
+    TAV_CUDA(cudaStreamSynchronize(s));
+    mark_done(ix);
+    return TAV_OK;
+}
+
 }  // extern "C"
 
 static inline cudaError_t ev_record(cudaEvent_t& ev, cudaStream_t s) {
@@ -622,7 +688,7 @@ static int ensure_scan_counters(tav_index* ix, cudaStream_t s) {
 static int scan_search(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq_total, int k, float floor_score,
                        const int64_t* d_subset, int64_t n_scan, int64_t item_offset, int64_t* d_items,
                        float* d_scores, int32_t* d_counts, const uint32_t* d_mask, int ties_low, cudaStream_t s,
-                       bool allow_fuse = true, int positions = 0) {
+                       bool allow_fuse = true, int positions = 0, QueryMasks qm = QueryMasks{}) {
     const int pass_k = std::min(k, kPassK);
     int qb = scan_max_queries(ix->dim, pass_k);
     if (qb < 1) {
@@ -667,6 +733,8 @@ static int scan_search(tav_index* ix, TimedSearch* ts, bool timing, const float*
             a.cand_count = d_count;
             a.grid = grid;
             a.row_mask = d_mask;
+            if (qm.bits && nq == 1 && !qm.map) a.row_mask = qm.bits + static_cast<int64_t>(q0) * qm.stride;  // the row-mask form
+            else if (qm.bits) a.qmask = qmask_from(qm, q0);
             a.ties_low = ties_low;
             a.items_as_positions = positions;
             if (fuse) {
@@ -794,10 +862,12 @@ static int finish_pending(tav_index* ix, cudaStream_t s, int* redone) {
                                      cudaMemcpyDeviceToHost, s));
             TAV_CUDA(cudaStreamSynchronize(s));
         }
-        const uint32_t* mask = p.masked ? static_cast<const uint32_t*>(ix->row_mask.p) : nullptr;
         for (int q = 0; q < p.nq; ++q) {
             if (!host[q]) continue;
             ++n_redone;
+            // the query's own mask (the row mask: stride 0), as the row-mask form of the scan
+            const uint32_t* mask = p.mask ? p.mask + static_cast<int64_t>(TAV_QUERY_MASK_MUTANT == 2 ? 0 : q) * p.mask_stride
+                                          : nullptr;
             int rc = scan_search(ix, nullptr, false, p.queries + static_cast<size_t>(q) * ix->dim, 1, p.k, p.floor, nullptr,
                                  ix->size, p.item_offset, p.items + static_cast<size_t>(q) * p.k,
                                  p.scores + static_cast<size_t>(q) * p.k, p.counts + q, mask, 0, s);
@@ -815,6 +885,37 @@ static int finish_pending(tav_index* ix, cudaStream_t s, int* redone) {
     for (DevBuf& b : ix->held_retired) b.release();
     ix->held_retired.clear();
     if (redone) *redone = n_redone;
+    return TAV_OK;
+}
+
+// TAV_USE_QUERY_MASKS of a search of n_queries: the index's masks in *qm, or the error.  One query takes the
+// row-mask form: its mask goes to *d_mask and *qm stays empty.
+static int use_query_masks(tav_index* ix, const char* fn, int n_queries, int flags, bool has_subset, QueryMasks* qm,
+                           const uint32_t** d_mask) {
+    if (flags & TAV_USE_ROW_MASK) {
+        set_error("%s: TAV_USE_QUERY_MASKS and TAV_USE_ROW_MASK cannot be combined", fn);
+        return TAV_ERR_INVALID;
+    }
+    if (has_subset) {
+        set_error("%s: per-query masks and a subset cannot be combined", fn);
+        return TAV_ERR_INVALID;
+    }
+    if (ix->qmask_n == 0 || ix->qmask_rows != ix->size || ix->size == 0) {
+        set_error("%s: TAV_USE_QUERY_MASKS without current per-query masks (tav_set_query_masks)", fn);
+        return TAV_ERR_STATE;
+    }
+    if (n_queries != ix->qmask_n) {
+        set_error("%s: %d queries for %d per-query masks", fn, n_queries, ix->qmask_n);
+        return TAV_ERR_INVALID;
+    }
+    *qm = QueryMasks{};
+    if (n_queries == 1) {
+        *d_mask = static_cast<const uint32_t*>(ix->qmask.p);
+        return TAV_OK;
+    }
+    qm->bits = static_cast<const uint32_t*>(ix->qmask.p);
+    qm->stride = ix->qmask_stride;
+    qm->pop = static_cast<const uint32_t*>(ix->qmask_pop.p);
     return TAV_OK;
 }
 
@@ -903,7 +1004,7 @@ static int stage_inputs(tav_index* ix, TimedSearch* ts, bool timing, const float
 // collect-mode row scans of nq queries (device, contiguous): query q's keys -> keys + q * stride, counts[q]
 static int collect_scans(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
                          const int64_t* d_subset, int64_t n_scan, const uint32_t* d_mask, int ties_low,
-                         uint64_t* keys, int64_t stride, uint32_t* counts, cudaStream_t s) {
+                         uint64_t* keys, int64_t stride, uint32_t* counts, cudaStream_t s, QueryMasks qm = QueryMasks{}) {
     const int qb = scan_collect_max_queries(ix->dim);  // a smaller last block takes a smaller instantiation
     if (qb < 1) {
         set_error("threshold search: embedding size %d too large for the row-scan kernel", ix->dim);
@@ -926,6 +1027,7 @@ static int collect_scans(tav_index* ix, TimedSearch* ts, bool timing, const floa
         a.cand_count = counts + q0;
         a.grid = grid;
         a.row_mask = d_mask;
+        if (qm.bits) a.qmask = qmask_from(qm, q0);
         a.ties_low = ties_low;
         const bool timed = timing && ts->used < kMaxTimedKernels;
         if (timed) TAV_CUDA(ev_record(ts->ev[ts->used][0], s));
@@ -1018,13 +1120,25 @@ static int range_sort(tav_index* ix, TimedSearch* ts, bool timing, std::vector<S
     return TAV_OK;
 }
 
+// the masks of a re-pass over the gathered queries `over` (indexes into the search whose masks are qm)
+static int gather_mask_map(tav_index* ix, const std::vector<int>& over, const QueryMasks& qm, QueryMasks& out,
+                           cudaStream_t s) {
+    if (int rc = range_alloc(ix->range_qmap, over.size() * sizeof(int32_t), "the re-pass mask map")) return rc;
+    std::vector<int32_t> map(over.begin(), over.end());
+    // from pageable memory: consumed when the call returns
+    TAV_CUDA(cudaMemcpyAsync(ix->range_qmap.p, map.data(), map.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    out = qm;
+    out.map = TAV_QUERY_MASK_MUTANT == 3 ? nullptr : static_cast<const int32_t*>(ix->range_qmap.p);
+    return TAV_OK;
+}
+
 // Row-scan collection: one collect scan per block of queries into regions sized from `expected_hits`; the
 // counters keep counting past a region, so after the one synchronisation the totals are exact and the
 // overflowed queries get exactly one more scan into regions of that size.
 static int range_collect_scan(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
                               const int64_t* d_subset, int64_t n_scan, int64_t item_offset, const uint32_t* d_mask,
                               int ties_low, int64_t expected_hits, std::vector<int64_t>& offsets, cudaStream_t s,
-                              int positions = 0) {
+                              int positions = 0, QueryMasks qm = QueryMasks{}) {
     const int64_t per = range_per_query(expected_hits, nq, n_scan);
     if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(nq) * per * sizeof(uint64_t), "the hit regions")) return rc;
     if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(nq) * sizeof(uint32_t), "the hit counters")) return rc;
@@ -1032,7 +1146,7 @@ static int range_collect_scan(tav_index* ix, TimedSearch* ts, bool timing, const
     uint64_t* keys = static_cast<uint64_t*>(ix->range_keys.p);
     TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(nq) * sizeof(uint32_t), s));
     if (int rc = collect_scans(ix, ts, timing, d_queries, nq, floor, d_subset, n_scan, d_mask, ties_low, keys, per,
-                               d_counts, s))
+                               d_counts, s, qm))
         return rc;
 
     std::vector<uint32_t> cnt(static_cast<size_t>(nq));
@@ -1062,8 +1176,12 @@ static int range_collect_scan(tav_index* ix, TimedSearch* ts, bool timing, const
             TAV_CUDA(cudaMemcpyAsync(qg + i * qrow, reinterpret_cast<const char*>(d_queries) + over[i] * qrow, qrow,
                                      cudaMemcpyDeviceToDevice, s));
         TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(no) * sizeof(uint32_t), s));
+        QueryMasks qm2{};
+        if (qm.bits) {  // each gathered query keeps its own mask
+            if (int rc = gather_mask_map(ix, over, qm, qm2, s)) return rc;
+        }
         if (int rc = collect_scans(ix, ts, timing, reinterpret_cast<const float*>(qg), no, floor, d_subset, n_scan,
-                                   d_mask, ties_low, keys2, over_max, d_counts, s))
+                                   d_mask, ties_low, keys2, over_max, d_counts, s, qm2))
             return rc;
     }
     std::vector<SortSeg> segs(static_cast<size_t>(nq));
@@ -1086,7 +1204,7 @@ constexpr int kRangeUseScan = 1;  // range_collect_mma: the tensor-core form can
 // a value beyond the fp16 range (the exact row scan then serves the search, as it does for top-k searches).
 static int range_collect_mma(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
                              int64_t item_offset, const uint32_t* d_mask, int ties_low, int64_t expected_hits,
-                             std::vector<int64_t>& offsets, cudaStream_t s) {
+                             std::vector<int64_t>& offsets, cudaStream_t s, QueryMasks qm) {
     const bool split = ix->dtype == TAV_F32;
     if (split) {
         const int rc = ensure_split_planes(ix, ts, s);
@@ -1125,6 +1243,7 @@ static int range_collect_mma(tav_index* ix, TimedSearch* ts, bool timing, const 
     m.item_offset = item_offset;
     m.retry_flags = reinterpret_cast<int32_t*>(aux);
     m.row_mask = d_mask;
+    m.qmask = qm;
     int ev_used = ts->used;
     m.ev = timing ? ts->ev : nullptr;
     m.ev_kind = ts->kind;
@@ -1180,6 +1299,9 @@ static int range_collect_mma(tav_index* ix, TimedSearch* ts, bool timing, const 
         MmaArgs m2 = m;
         m2.queries = reinterpret_cast<const float*>(qg);
         m2.nq = no;
+        if (qm.bits) {  // each gathered query keeps its own mask
+            if (int rc = gather_mask_map(ix, over, qm, m2.qmask, s)) return rc;
+        }
         const MmaCollect c2 = mma_collect_plan(m2, c.per_chunk, over_seg);
         if (c2.n_seg != c.n_seg || c2.cap_seg < over_seg) {
             set_error("threshold search: tensor-core re-pass plan mismatch");
@@ -1216,15 +1338,15 @@ static int range_collect_mma(tav_index* ix, TimedSearch* ts, bool timing, const 
 static int range_core(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
                       const int64_t* d_subset, int64_t n_scan, int64_t item_offset, const uint32_t* d_mask,
                       int ties_low, int64_t expected_hits, bool use_mma, std::vector<int64_t>& offsets, cudaStream_t s,
-                      int positions = 0) {
+                      int positions = 0, QueryMasks qm = QueryMasks{}) {
     if (use_mma) {
         const int rc = range_collect_mma(ix, ts, timing, d_queries, nq, floor, item_offset, d_mask, ties_low,
-                                         expected_hits, offsets, s);
+                                         expected_hits, offsets, s, qm);
         if (rc != kRangeUseScan) return rc;
         ts->path = 1;  // a value beyond the fp16 range: the exact row scan serves the search
     }
     return range_collect_scan(ix, ts, timing, d_queries, nq, floor, d_subset, n_scan, item_offset, d_mask, ties_low,
-                              expected_hits, offsets, s, positions);
+                              expected_hits, offsets, s, positions, qm);
 }
 
 // ---- removal and overwrite (tav_remove_rows, tav_write_rows) -----------------------------------------------
@@ -1356,6 +1478,7 @@ int tav_remove_rows(tav_index* ix, const int64_t* ordinals, int64_t n, void* str
     ix->size -= static_cast<int64_t>(rem.size());
     ix->split_rows = std::min(ix->split_rows, rem[0]);
     ix->split_recheck = true;
+    ix->qmask_n = 0;
     ix->row_mask_rows = 0;  // ordinals changed meaning (a later append can restore the old size)
     return TAV_OK;
 }
@@ -1446,7 +1569,10 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
     const size_t nk = static_cast<size_t>(n_queries) * k;
     const uint32_t* d_mask = nullptr;
-    if (flags & TAV_USE_ROW_MASK) {
+    QueryMasks qm{};
+    if (flags & TAV_USE_QUERY_MASKS) {
+        if (int rc = use_query_masks(ix, "tav_search", n_queries, flags, subset != nullptr, &qm, &d_mask)) return rc;
+    } else if (flags & TAV_USE_ROW_MASK) {
         if (ix->row_mask_rows != ix->size || ix->size == 0) {
             set_error("tav_search: TAV_USE_ROW_MASK without a current row mask (tav_set_row_mask)");
             return TAV_ERR_STATE;
@@ -1535,7 +1661,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         std::vector<int64_t> offsets;
         ix->range_total = 0;
         if (int rc = range_core(ix, ts, timing, d_q, n_queries, min_score, d_sub, n_scan, item_offset, d_mask, ties_low,
-                                static_cast<int64_t>(n_queries) * n_scan, false, offsets, s, positions))
+                                static_cast<int64_t>(n_queries) * n_scan, false, offsets, s, positions, qm))
             return rc;
         if (timing) {
             TAV_CUDA(ev_record(ts->total[1], s));
@@ -1803,6 +1929,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             m.retry_total_host = static_cast<int32_t*>(ix->retry_host.p) + 2 * slot;
             m.split_overflow_host = use_split ? static_cast<int*>(ix->retry_host.p) + 2 * slot + 1 : nullptr;
             m.row_mask = d_mask;
+            m.qmask = qmask_from(qm, q0);
             int ev_used = 0;
             const bool slab_timed = timing && q0 == 0;
             m.ev = slab_timed ? ts->ev : nullptr;
@@ -1822,7 +1949,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             if (slab_timed) ts->used = ev_used;
             ts->launches += launches;
             Pending p{m.queries, nq, k, min_score, item_offset, m.out_items, m.out_scores, m.out_counts, slot,
-                      use_split, d_mask != nullptr};
+                      use_split, m.qmask.bits ? m.qmask.bits : d_mask, m.qmask.bits ? m.qmask.stride : 0};
             ix->pending.push_back(p);
             ix->held_used = std::max(ix->held_used, held_end);  // (a finish_pending above may have reset it)
         }
@@ -1836,7 +1963,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     } else {
         ts->path = 1;
         int rc = scan_search(ix, ts, timing, d_queries, n_queries, k, min_score, d_subset, n_scan, item_offset,
-                             d_items, d_scores, d_counts, d_mask, ties_low, s, !(flags & TAV_NO_FUSED_SCAN), positions);
+                             d_items, d_scores, d_counts, d_mask, ties_low, s, !(flags & TAV_NO_FUSED_SCAN), positions, qm);
         if (rc != TAV_OK) return rc;
     }
     if (timing) {
@@ -1909,7 +2036,10 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
         return mark_queued(ix, s);  // the sort after the last synchronisation may still run
     };
     const uint32_t* d_mask = nullptr;
-    if (flags & TAV_USE_ROW_MASK) {
+    QueryMasks qm{};
+    if (flags & TAV_USE_QUERY_MASKS) {
+        if (int rc = use_query_masks(ix, "tav_range_search", n_queries, flags, subset != nullptr, &qm, &d_mask)) return rc;
+    } else if (flags & TAV_USE_ROW_MASK) {
         if (ix->row_mask_rows != ix->size || ix->size == 0) {
             set_error("tav_range_search: TAV_USE_ROW_MASK without a current row mask (tav_set_row_mask)");
             return TAV_ERR_STATE;
@@ -1958,7 +2088,7 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
         return rc;
     if (int rc = range_core(ix, ts, timing, d_queries, n_queries, min_score, d_subset, n_scan, item_offset, d_mask,
                             (flags & TAV_TIES_LOW_FIRST) ? 1 : 0, expected_hits, use_mma, offsets, s,
-                            (flags & TAV_ITEMS_AS_POSITIONS) && TAV_SHARDED_FILTER_MUTANT != 3 ? 1 : 0))
+                            (flags & TAV_ITEMS_AS_POSITIONS) && TAV_SHARDED_FILTER_MUTANT != 3 ? 1 : 0, qm))
         return rc;
     if (timing) {
         TAV_CUDA(ev_record(ts->total[1], s));

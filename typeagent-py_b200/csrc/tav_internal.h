@@ -10,6 +10,37 @@ namespace tav {
 
 struct MergeSync;  // tav_common.cuh
 
+// Per-query row masks (TAV_USE_QUERY_MASKS): query q of a launch may return row r when bit r of mask row
+// m = (map ? map[q] : q) is set, that row being `stride` words at bits + m * stride (whole 256-row tiles).
+// `map` serves a re-pass over gathered queries: each keeps the mask it was issued with.
+struct QueryMasks {
+    const uint32_t* bits = nullptr;  // device, nullptr = no per-query masks
+    int64_t stride = 0;              // words per mask row (a multiple of 8)
+    const int32_t* map = nullptr;    // device [nq], or nullptr = identity
+    const uint32_t* pop = nullptr;   // device: allowed rows per mask row (indexed like the rows), or nullptr
+};
+// masks of the queries [q0, ...) of a launch
+inline QueryMasks qmask_from(QueryMasks m, int q0) {
+    if (m.map) m.map += q0;
+    else if (m.bits) {
+        m.bits += static_cast<int64_t>(q0) * m.stride;
+        if (m.pop) m.pop += q0;
+    }
+    return m;
+}
+
+// TAV_QUERY_MASK_MUTANT (tests only, never set by build.py): 1..3 compile one deliberate defect each, so that
+// tests/test_gpu_query_masks.py can show its exact checks catch it: 1 the tensor-core MAIN epilogue tests the
+// other query's (h ^ 1) mask, 2 the exact redo of a flagged query uses mask 0, 3 the threshold search's
+// re-pass over gathered queries drops their mask map.
+#ifndef TAV_QUERY_MASK_MUTANT
+#define TAV_QUERY_MASK_MUTANT 0
+#endif
+
+// allowed rows (set bits below n_rows) of each of n_masks mask rows, `stride` words apart -> pop[n_masks]
+cudaError_t launch_mask_popcount(const uint32_t* bits, int n_masks, int64_t n_rows, int64_t stride, uint32_t* pop,
+                                 cudaStream_t s);
+
 // ---- row-scan path (tav_scan.cu) -------------------------------------------------------
 struct ScanArgs {
     const void* corpus;       // [n_corpus, dim] storage dtype, row-major dense
@@ -44,6 +75,7 @@ struct ScanArgs {
     // (zero on entry) counts every admitted row, also those beyond collect_stride, which are not stored
     int64_t collect_stride;
     int items_as_positions;   // single-launch form: items = the subset position (TAV_ITEMS_AS_POSITIONS)
+    QueryMasks qmask;         // per-query masks of queries [0, nq) of this pass (instead of row_mask; no subset)
 };
 constexpr int kFusedSelectMax = 8192;   // survivors the last CTA of the single-launch form can merge
 constexpr int kFusedSelOut = 1024;      // ... of which it sorts at most this many after the histogram selection
@@ -189,6 +221,7 @@ struct MmaArgs {
     int ev_max;
     int* ev_used;
     int ev_main_only;      // 1: record events only around the dominant (MAIN) kernel
+    QueryMasks qmask;      // optional per-query masks of queries [0, nq) (instead of row_mask)
 };
 constexpr int kMmaMaxQueries = 32768;  // queries per launch_mma_search call (256 chunks of 128; callers slab)
 size_t mma_workspace_bytes(const MmaArgs& a);

@@ -46,6 +46,8 @@
 // Optional row mask (predicate / post-filter pushdown, reference: aitools/vectorbase.py:191-201,
 // storage/sqlite/messageindex.py:296-326): one bit per corpus row; masked-out rows are dropped
 // in the epilogue (and ignored by the sampler, so the threshold adapts to the mask's density).
+// Per-query masks (kSampleQ / kMainQ): the same, with each query's own mask; a query whose mask allows at most
+// pop_exact rows is admitted at the min_score floor, so a sparse mask does not starve it into the exact redo.
 //
 // Algorithmic bytes per search: N*D*2 (corpus, read once) + queries + hits.
 
@@ -80,7 +82,8 @@ constexpr size_t kTileSmem = 192 * 1024;            // the stage ring: 4 x (16 +
 constexpr size_t kScratchBytes = 2 * kBM * kSampleTop * sizeof(float);  // the sampler tail's exchange of partial top-8 lists
 constexpr size_t kSmemBytes = 1024 + kTileSmem + 256 + kScratchBytes;
 
-enum Mode { kSample = 0, kMain = 1, kDump = 2 };
+// kSampleQ / kMainQ: kSample / kMain with per-query masks (KernelArgs::qmask)
+enum Mode { kSample = 0, kMain = 1, kDump = 2, kSampleQ = 3, kMainQ = 4 };
 
 struct KernelArgs {
     int64_t n_rows;
@@ -106,6 +109,8 @@ struct KernelArgs {
     uint32_t cap_seg;
     const uint32_t* row_mask;  // optional: bit r set = row r may be returned
     float* dump;           // DUMP: [nq, n_rows] raw dots
+    QueryMasks qmask;      // kSampleQ / kMainQ: per-query masks (bits padded to whole tiles)
+    uint32_t pop_exact;    // kSampleQ: a query whose mask allows at most this many rows is admitted at the floor
 };
 
 __device__ __forceinline__ void insert_top(float (&top)[kSampleTop], float x) {
@@ -236,6 +241,9 @@ __global__ void __launch_bounds__(kMmaThreads, 1)
 mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c,
                 const __grid_constant__ CUtensorMap map_q_lo, const __grid_constant__ CUtensorMap map_c_lo,
                 const KernelArgs a) {
+    constexpr bool kQM = MODE == kSampleQ || MODE == kMainQ;   // per-query masks
+    constexpr bool kIsSample = MODE == kSample || MODE == kSampleQ;
+    constexpr bool kIsMain = MODE == kMain || MODE == kMainQ;
     constexpr int kTileN = SPLIT ? kTileRowsSplit : kTileRows;  // corpus rows per tile
     constexpr int kNacc = kTileN / 2;                          // accumulator registers per thread
     constexpr int kBBytes = kTileN * kBK * 2;
@@ -268,6 +276,16 @@ mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         if (SPLIT) {
             ptx::prefetch_tensormap(&map_q_lo);
             ptx::prefetch_tensormap(&map_c_lo);
+        }
+    }
+    // per-query masks: the mask row of each query of this unit's chunk, in the sampler tail's scratch (unused
+    // until the tail), so that the epilogue keeps no register for it (padding queries: nullptr, nothing read)
+    const uint32_t** s_qrow = reinterpret_cast<const uint32_t**>(scratch);
+    if constexpr (kQM) {
+        if (threadIdx.x < kBM) {
+            const int q = (unit % a.nqc) * kBM + threadIdx.x;
+            s_qrow[threadIdx.x] =
+                q < a.nq ? a.qmask.bits + static_cast<int64_t>(a.qmask.map ? a.qmask.map[q] : q) * a.qmask.stride : nullptr;
         }
     }
     __syncthreads();
@@ -314,7 +332,7 @@ mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             my_cand[h] = a.cand + (static_cast<size_t>(my_q[h]) * a.n_seg + seg) * a.cap_seg;
-            tau[h] = (MODE == kMain && my_q[h] < a.nq) ? a.thr[my_q[h]] : INFINITY;
+            tau[h] = (kIsMain && my_q[h] < a.nq) ? a.thr[my_q[h]] : INFINITY;
         }
         // A: this warpgroup's 64 query rows (8 swizzle groups of 1024 B in); B: the corpus slice
         const uint32_t a_off = static_cast<uint32_t>(wg) * 64 * 128;
@@ -383,15 +401,18 @@ mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
                             if (col < ncols) out[col] = acc[acc_index(j, h, e)];
                         }
                 }
-            } else if (MODE == kSample) {
+            } else if (kIsSample) {
                 // branch-free: sample tiles are full tiles, every column is a real row
                 const int bpt = (kTileN / 128) * a.sample_gph;  // blocks per tile
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     float* dst = a.sample_max + static_cast<size_t>(t) * bpt * a.nq_pad + my_q[h];
-                    if (a.sample_gph == 16) sample_blocks<1>(acc, h, t4, a.row_mask, row0, dst, a.nq_pad);
-                    else if (a.sample_gph == 4) sample_blocks<4>(acc, h, t4, a.row_mask, row0, dst, a.nq_pad);
-                    else sample_blocks<16>(acc, h, t4, a.row_mask, row0, dst, a.nq_pad);
+                    const uint32_t* mask = a.row_mask;
+                    if constexpr (kQM)  // each query's own rows: its threshold adapts to its mask
+                        mask = s_qrow[q_local + 8 * h];
+                    if (a.sample_gph == 16) sample_blocks<1>(acc, h, t4, mask, row0, dst, a.nq_pad);
+                    else if (a.sample_gph == 4) sample_blocks<4>(acc, h, t4, mask, row0, dst, a.nq_pad);
+                    else sample_blocks<16>(acc, h, t4, mask, row0, dst, a.nq_pad);
                 }
             } else {
                 // MAIN: group-wise screen and private-segment append (admit_group)
@@ -401,21 +422,27 @@ mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
                     if (nvalid <= 0) break;
                     const uint32_t rbase = static_cast<uint32_t>(row0 + 32 * g);
                     uint32_t amask = nvalid >= 32 ? 0xFFFFFFFFu : ((1u << nvalid) - 1u);
-                    if (a.row_mask) amask &= a.row_mask[rbase >> 5];
+                    if (!kQM && a.row_mask) amask &= a.row_mask[rbase >> 5];
 #pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        admit_group(acc, g, h, t4, tau[h], rbase, amask, my_cand[h], n_admitted[h], a.cap_seg);
+                    for (int h = 0; h < 2; ++h) {
+                        uint32_t am = amask;
+                        if constexpr (kQM) {  // the query's own mask word of these 32 rows
+                            const uint32_t* qr = s_qrow[q_local + 8 * (TAV_QUERY_MASK_MUTANT == 1 ? h ^ 1 : h)];
+                            am = qr ? am & qr[rbase >> 5] : 0u;
+                        }
+                        admit_group(acc, g, h, t4, tau[h], rbase, am, my_cand[h], n_admitted[h], a.cap_seg);
+                    }
                 }
             }
         }
-        if (MODE == kSample) __threadfence();  // block maxima visible device-wide before the unit signs off
-        if (MODE == kMain && unit / a.nqc < n_units / a.nqc) {
+        if (kIsSample) __threadfence();  // block maxima visible device-wide before the unit signs off
+        if (kIsMain && unit / a.nqc < n_units / a.nqc) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) a.cand_count[static_cast<size_t>(my_q[h]) * a.n_seg + seg] = n_admitted[h];
         }
     }
 
-    if (MODE == kSample) {
+    if (kIsSample) {
         // ---- sampler tail: the last unit of a query chunk turns block maxima into thresholds ----
         __syncthreads();
         const int upc = n_units / a.nqc;
@@ -469,6 +496,11 @@ mma_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
                     if (sampled > -INFINITY) {
                         // bottom of the float32 score class of the sampled dot: rows below it score strictly less
                         thr = fmaxf(dot_floor_for_score(score_from_dot(sampled)), floor_x);
+                    }
+                    if constexpr (kQM) {
+                        // a sparse mask: every allowed row fits the segments (or fewer than k are allowed), so the
+                        // exact floor admits them all instead of a sampled threshold that could starve the query
+                        if (a.qmask.pop && a.qmask.pop[a.qmask.map ? a.qmask.map[q] : q] <= a.pop_exact) thr = floor_x;
                     }
                     a.thr[q] = thr;
                     a.floor_x[q] = floor_x;
@@ -1069,6 +1101,8 @@ cudaError_t launch_mma_search(const MmaArgs& a, void* workspace, size_t workspac
     ka.cap_seg = p.cap_seg;
     ka.n_seg = p.n_seg;
     ka.row_mask = a.row_mask;
+    ka.qmask = a.qmask;
+    ka.pop_exact = std::max<uint32_t>(p.cap_seg, static_cast<uint32_t>(a.k));
 
     if (p.n_sample > 0) {
         // strided sample of FULL tiles; the last unit of every query chunk publishes the thresholds
@@ -1076,7 +1110,8 @@ cudaError_t launch_mma_search(const MmaArgs& a, void* workspace, size_t workspac
         ka.tile_mul = p.n_full_tiles;
         ka.tile_div = p.n_sample;
         if ((e = ev_begin_kind(1)) != cudaSuccess) return e;
-        e = launch_kernel<kSample>(maps, ka, kdt, split, p.sample_units, s);
+        e = ka.qmask.bits ? launch_kernel<kSampleQ>(maps, ka, kdt, split, p.sample_units, s)
+                          : launch_kernel<kSample>(maps, ka, kdt, split, p.sample_units, s);
         if (e != cudaSuccess) return e;
         if ((e = ev_end(1)) != cudaSuccess) return e;
         ++n_launch;
@@ -1086,7 +1121,8 @@ cudaError_t launch_mma_search(const MmaArgs& a, void* workspace, size_t workspac
     ka.tile_mul = 1;
     ka.tile_div = 1;
     if ((e = ev_begin_kind(0)) != cudaSuccess) return e;
-    e = launch_kernel<kMain>(maps, ka, kdt, split, p.main_units, s);
+    e = ka.qmask.bits ? launch_kernel<kMainQ>(maps, ka, kdt, split, p.main_units, s)
+                      : launch_kernel<kMain>(maps, ka, kdt, split, p.main_units, s);
     if (e != cudaSuccess) return e;
     if ((e = ev_end(0)) != cudaSuccess) return e;
     ++n_launch;
@@ -1153,12 +1189,14 @@ cudaError_t launch_mma_collect(const MmaArgs& a, const MmaCollect& c, void* work
     ka.cap_seg = p.cap_seg;
     ka.n_seg = p.n_seg;
     ka.row_mask = a.row_mask;
+    ka.qmask = a.qmask;
     ka.n_tiles_work = p.n_tiles;
     ka.tile_mul = 1;
     ka.tile_div = 1;
     const bool timed = a.ev && a.ev_used && *a.ev_used < a.ev_max;
     if (timed && (e = cudaEventRecord(a.ev[*a.ev_used][0], s)) != cudaSuccess) return e;
-    e = launch_kernel<kMain>(maps, ka, mma_dtype(a), a.split != 0, p.main_units, s);
+    e = ka.qmask.bits ? launch_kernel<kMainQ>(maps, ka, mma_dtype(a), a.split != 0, p.main_units, s)
+                      : launch_kernel<kMain>(maps, ka, mma_dtype(a), a.split != 0, p.main_units, s);
     if (e != cudaSuccess) return e;
     if (timed) {
         if (a.ev_kind) a.ev_kind[*a.ev_used] = 0;

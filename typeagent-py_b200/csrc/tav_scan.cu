@@ -126,14 +126,30 @@ struct alignas(16) ParamBlob {
     int32_t sub[SN > 0 ? SN : 1];
 };
 
+// the general form with per-query masks (a.qmask): a tag type, so that the other instantiations stay as they are
+struct NoBlobQM : NoBlob {};
+
 template <typename BLOB>
 struct BlobTraits {
     static constexpr bool kHas = true;
+    static constexpr bool kQMask = false;
 };
 template <>
 struct BlobTraits<NoBlob> {
     static constexpr bool kHas = false;
+    static constexpr bool kQMask = false;
 };
+template <>
+struct BlobTraits<NoBlobQM> {
+    static constexpr bool kHas = false;
+    static constexpr bool kQMask = true;
+};
+
+// bit `row` of query q's mask (q < a.nq)
+__device__ __forceinline__ bool qmask_bit(const QueryMasks& m, int q, int64_t row) {
+    const int64_t r = m.map ? m.map[q] : q;
+    return (m.bits[r * m.stride + (row >> 5)] >> (row & 31)) & 1u;
+}
 
 __device__ __forceinline__ unsigned long long global_ns() {
     unsigned long long t;
@@ -279,11 +295,19 @@ scan_rows_kernel(const ScanArgs a, const __grid_constant__ BLOB blob) {
             const int r = idx / QB, q = idx % QB;
             const int64_t pos = pos0 + r;
             bool want = (lane & (kLanesPerValue - 1)) == 0 && pos < a.n_scan && q < a.nq;
-            if (want && a.row_mask) {
+            if (!BlobTraits<BLOB>::kQMask && want && a.row_mask) {
                 int64_t row = rrow[0];
 #pragma unroll
                 for (int rr = 1; rr < kRowsPerWarp; ++rr) row = (r == rr) ? rrow[rr] : row;
                 want = (a.row_mask[row >> 5] >> (row & 31)) & 1u;
+            }
+            if constexpr (BlobTraits<BLOB>::kQMask) {
+                if (want) {  // this lane's query's own mask
+                    int64_t row = rrow[0];
+#pragma unroll
+                    for (int rr = 1; rr < kRowsPerWarp; ++rr) row = (r == rr) ? rrow[rr] : row;
+                    want = qmask_bit(a.qmask, q, row);
+                }
             }
             const float s = score_from_dot(acc[0]);
             want = want && s >= a.floor_score;  // float32 compare, NaN rejected
@@ -308,11 +332,19 @@ scan_rows_kernel(const ScanArgs a, const __grid_constant__ BLOB blob) {
             const int r = idx / QB, q = idx % QB;
             const int64_t pos = pos0 + r;
             bool allowed = true;
-            if (a.row_mask) {  // predicate pushdown (vectorbase.py:191-201): one bit per corpus row
+            if (!BlobTraits<BLOB>::kQMask && a.row_mask) {  // predicate pushdown (vectorbase.py:191-201): one bit per corpus row
                 int64_t row = rrow[0];
 #pragma unroll
                 for (int rr = 1; rr < kRowsPerWarp; ++rr) row = (r == rr) ? rrow[rr] : row;
                 allowed = (a.row_mask[row >> 5] >> (row & 31)) & 1u;
+            }
+            if constexpr (BlobTraits<BLOB>::kQMask) {
+                if (pos < a.n_scan && q < a.nq) {  // this lane's query's own mask (padding lanes read nothing)
+                    int64_t row = rrow[0];
+#pragma unroll
+                    for (int rr = 1; rr < kRowsPerWarp; ++rr) row = (r == rr) ? rrow[rr] : row;
+                    allowed = qmask_bit(a.qmask, q, row);
+                }
             }
             if (pos < a.n_scan && q < a.nq && allowed) {
                 const float s = score_from_dot(acc[0]);
@@ -471,13 +503,19 @@ static cudaError_t launch_scan_t(const ScanArgs& a, const BLOB& blob, cudaStream
     return cudaGetLastError();
 }
 
-template <typename T>
-static cudaError_t launch_scan_q(const ScanArgs& a, cudaStream_t s) {
-    const NoBlob none{};
+template <typename T, typename BLOB>
+static cudaError_t launch_scan_b(const ScanArgs& a, cudaStream_t s) {
+    const BLOB none{};
     if (a.nq <= 1) return launch_scan_t<T, 1>(a, none, s);
     if (a.nq <= 2) return launch_scan_t<T, 2>(a, none, s);
     if (a.nq <= 4) return launch_scan_t<T, 4>(a, none, s);
     return launch_scan_t<T, 8>(a, none, s);
+}
+
+template <typename T>
+static cudaError_t launch_scan_q(const ScanArgs& a, cudaStream_t s) {
+    if (a.qmask.bits) return launch_scan_b<T, NoBlobQM>(a, s);
+    return launch_scan_b<T, NoBlob>(a, s);
 }
 
 cudaError_t launch_scan(const ScanArgs& a, cudaStream_t s) {
@@ -509,25 +547,59 @@ int scan_collect_grid(int device, int dim, int nq, int64_t n_scan) {
     return static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(tiles, static_cast<int64_t>(sms) * per_sm)));
 }
 
-template <typename T, int QB>
+template <typename T, int QB, typename BLOB>
 static cudaError_t launch_collect_t(const ScanArgs& a, cudaStream_t s) {
     const size_t row_bytes = static_cast<size_t>(a.dim) * sizeof(T);
     const bool vec = (row_bytes % 16 == 0) && (reinterpret_cast<uintptr_t>(a.corpus) % 16 == 0);
     const size_t smem = collect_smem_bytes(QB, a.dim);
-    auto kern = vec ? scan_rows_kernel<T, QB, true, NoBlob, true> : scan_rows_kernel<T, QB, false, NoBlob, true>;
+    auto kern = vec ? scan_rows_kernel<T, QB, true, BLOB, true> : scan_rows_kernel<T, QB, false, BLOB, true>;
     static int granted[2][16] = {};
     cudaError_t e = ensure_dynamic_smem(kern, smem, granted[vec ? 1 : 0]);
     if (e != cudaSuccess) return e;
-    kern<<<a.grid, kScanThreads, smem, s>>>(a, NoBlob{});
+    kern<<<a.grid, kScanThreads, smem, s>>>(a, BLOB{});
     return cudaGetLastError();
+}
+
+template <typename T, typename BLOB>
+static cudaError_t launch_collect_b(const ScanArgs& a, cudaStream_t s) {
+    if (a.nq <= 1) return launch_collect_t<T, 1, BLOB>(a, s);
+    if (a.nq <= 2) return launch_collect_t<T, 2, BLOB>(a, s);
+    if (a.nq <= 4) return launch_collect_t<T, 4, BLOB>(a, s);
+    return launch_collect_t<T, 8, BLOB>(a, s);
 }
 
 template <typename T>
 static cudaError_t launch_collect_q(const ScanArgs& a, cudaStream_t s) {
-    if (a.nq <= 1) return launch_collect_t<T, 1>(a, s);
-    if (a.nq <= 2) return launch_collect_t<T, 2>(a, s);
-    if (a.nq <= 4) return launch_collect_t<T, 4>(a, s);
-    return launch_collect_t<T, 8>(a, s);
+    if (a.qmask.bits) return launch_collect_b<T, NoBlobQM>(a, s);
+    return launch_collect_b<T, NoBlob>(a, s);
+}
+
+// one CTA per mask row: the set bits of its first n_rows
+__global__ void __launch_bounds__(256)
+mask_popcount_kernel(const uint32_t* __restrict__ bits, int64_t n_rows, int64_t stride, uint32_t* pop) {
+    __shared__ uint32_t s_part[8];
+    const int tid = threadIdx.x, lane = tid & 31;
+    const uint32_t* row = bits + static_cast<int64_t>(blockIdx.x) * stride;
+    const int64_t words = (n_rows + 31) / 32;
+    const uint32_t last = (n_rows & 31) ? (1u << (n_rows & 31)) - 1u : 0xFFFFFFFFu;
+    uint32_t c = 0;
+    for (int64_t i = tid; i < words; i += 256) c += __popc(i == words - 1 ? row[i] & last : row[i]);
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) c += __shfl_xor_sync(0xFFFFFFFFu, c, off);
+    if (lane == 0) s_part[tid >> 5] = c;
+    __syncthreads();
+    if (tid == 0) {
+        uint32_t t = 0;
+        for (int w = 0; w < 8; ++w) t += s_part[w];
+        pop[blockIdx.x] = t;
+    }
+}
+
+cudaError_t launch_mask_popcount(const uint32_t* bits, int n_masks, int64_t n_rows, int64_t stride, uint32_t* pop,
+                                 cudaStream_t s) {
+    if (n_masks <= 0) return cudaSuccess;
+    mask_popcount_kernel<<<n_masks, 256, 0, s>>>(bits, n_rows, stride, pop);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_scan_collect(const ScanArgs& a, cudaStream_t s) {

@@ -227,7 +227,10 @@ class CudaShardEngine:
         q = base._check_queries(queries)
         lib, ix = base._ensure_device()
         flags = base._flags() | _capi.TAV_OUTPUTS_ON_DEVICE
-        if mask is not None:
+        if mask is not None and mask.ndim == 2:  # one mask per query (this block's columns)
+            base._use_query_masks(lib, ix, mask, b)
+            flags |= _capi.TAV_USE_QUERY_MASKS
+        elif mask is not None:
             base._use_row_mask(lib, ix, mask, mask_key, mask_owner)
             flags |= _capi.TAV_USE_ROW_MASK
         if ties_low_first:
@@ -318,7 +321,10 @@ class CudaShardEngine:
             flags = base._flags() & ~_capi.TAV_NO_FUSED_SCAN
             if ties_low_first:
                 flags |= _capi.TAV_TIES_LOW_FIRST
-            if mask is not None:
+            if mask is not None and mask.ndim == 2:  # one mask per query (this block's columns)
+                base._use_query_masks(lib, ix, mask, b)
+                flags |= _capi.TAV_USE_QUERY_MASKS
+            elif mask is not None:
                 base._use_row_mask(lib, ix, mask, mask_key, mask_owner)
                 flags |= _capi.TAV_USE_ROW_MASK
             if sub is not None:
@@ -427,10 +433,28 @@ def subset_share(sub: np.ndarray, n_rows: int, lo: int, hi: int) -> tuple[np.nda
     return pos, rows[pos] - lo
 
 
-def block_mask(allowed, n_rows: int, lo: int, hi: int) -> np.ndarray:
+def block_mask(allowed, n_rows: int, lo: int, hi: int, n_queries: int | None = None) -> np.ndarray:
     """Rows [lo, hi) of a row mask over n_rows rows (bool [n_rows], or packed uint32 words as
     ``VectorBase.pack_row_mask`` makes them), packed again from bit 0: a block need not start on a word.
-    ValueError, with ``VectorBase``'s message, for a mask of the wrong length."""
+    A 2-D mask (one per query: bool [B, n_rows] or packed words [B, ceil(n_rows / 32)]) gives each query's
+    columns [lo, hi), packed per query as ``VectorBase.pack_query_masks`` does.  ValueError, with
+    ``VectorBase``'s message, for a mask of the wrong length, or (``n_queries``) the wrong number of masks."""
+    if np.ndim(allowed) == 2:
+        shape = np.shape(allowed)
+        if n_queries is not None and shape[0] != n_queries:
+            raise ValueError(f"query masks have {shape[0]} rows for {n_queries} queries")
+        if getattr(allowed, "dtype", None) == np.uint32:
+            if shape[1] != (n_rows + 31) // 32:
+                raise ValueError(f"query masks have {shape[1] * 32} bits for {n_rows} rows")
+            words = np.ascontiguousarray(allowed)
+            bits = np.unpackbits(words.view(np.uint8), axis=1, bitorder="little")[:, lo:hi].astype(bool)
+        else:
+            if shape[1] != n_rows:
+                raise ValueError(f"query masks have {shape[1]} entries for {n_rows} rows")
+            bits = np.asarray(allowed, dtype=bool)[:, lo:hi]
+        return VectorBase.pack_query_masks(bits)
+    if np.ndim(allowed) != 1:
+        raise ValueError(f"allowed= must be one row mask (1-D) or one mask per query (2-D), not {np.ndim(allowed)}-D")
     if getattr(allowed, "dtype", None) == np.uint32:
         words = np.ascontiguousarray(allowed)
         if len(words) != (n_rows + 31) // 32:
@@ -666,7 +690,8 @@ class ShardedVectorBase:
                       ties_low_first: bool = False):
         """SPMD batched lookup, replicated on every rank: items int64 [B, k], scores float32 [B, k], counts int32
         [B].  ``subset``, ``allowed`` and ``ties_low_first`` as ``VectorBase.search_arrays`` takes them over the
-        whole corpus (global ordinals; ``allowed`` a bool [N] mask or its packed words), with its results and
+        whole corpus (global ordinals; ``allowed`` a bool [N] mask or its packed words, or one mask per query: bool
+        [B, N] or packed words [B, ceil(N / 32)]), with its results and
         errors; such lookups exchange over the process group whatever ``exchange`` says."""
         if subset is not None or allowed is not None or ties_low_first:
             return self._search_arrays_filtered(queries, k, min_score, subset, allowed, ties_low_first)
@@ -699,8 +724,11 @@ class ShardedVectorBase:
             self._masks.clear()
         self._masks[key] = (words, owner)  # keeps the owner, and so its id(), alive
 
-    def _block_mask(self, allowed):
-        """(this block's packed words of ``allowed``, its cache key); errors on every rank alike."""
+    def _block_mask(self, allowed, n_queries: int):
+        """(this block's packed words of ``allowed``, its cache key); errors on every rank alike.  A 2-D
+        ``allowed`` (one mask per query) must have ``n_queries`` rows; it is checked on every call."""
+        if np.ndim(allowed) == 2 and np.shape(allowed)[0] != n_queries:
+            raise ValueError(f"query masks have {np.shape(allowed)[0]} rows for {n_queries} queries")
         key = ("allowed", id(allowed), self._generation, len(self))
         hit = self._masks.get(key)
         if hit is None:
@@ -790,7 +818,7 @@ class ShardedVectorBase:
         if allowed is not None and sub is not None:
             raise ValueError("allowed= and subset= cannot be combined")
         if allowed is not None:
-            mask = self._block_mask(allowed)
+            mask = self._block_mask(allowed, b)
         if sub is not None:
             check_subset(sub, len(self))
         if k_eff >= n_rows > RANGE_ROUTE_MIN_ROWS:
@@ -817,7 +845,8 @@ class ShardedVectorBase:
         """Threshold search over the whole corpus: EVERY row whose score is >= min_score, per query, as
         ``VectorBase.search_range`` returns it on one GPU — CSR numpy arrays offsets int64 [B + 1], items int64
         [T], scores float32 [T], in the library's order — replicated on every rank.  SPMD.  ``subset`` (global
-        ordinals) and ``allowed`` (bool [N] or packed words) as ``VectorBase.search_range`` takes them, with its
+        ordinals) and ``allowed`` (bool [N] or packed words, or 2-D: one mask per query) as ``VectorBase.search_range``
+        takes them, with its
         errors.
 
         Each rank runs the threshold search on its rows; one all-gather carries every rank's offsets (and a
@@ -836,7 +865,7 @@ class ShardedVectorBase:
             n_rows = len(self) if sub is None else len(sub)
             if len(q) == 0 or n_rows == 0 or len(self) == 0 or np.isnan(floor):
                 return np.zeros(len(q) + 1, np.int64), np.empty(0, np.int64), np.empty(0, np.float32)
-            mask = self._block_mask(allowed) if allowed is not None else None
+            mask = self._block_mask(allowed, len(q)) if allowed is not None else None
             if sub is not None:
                 check_subset(sub, len(self))
             return self._search_range_filtered(q, floor, ties_low_first, sub, mask)

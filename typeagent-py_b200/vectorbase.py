@@ -159,6 +159,8 @@ class VectorBase:
         self._pending: list = []             # tensors of deferred device searches, kept alive until finish_search()
         self._mask_key = None                # identity of the row mask currently on the device
         self._mask_ref = None                # ... and the object(s) that identity belongs to (so id() cannot be recycled)
+        self._qmask_key = None               # identity of the per-query masks currently on the device
+        self._qmask_ref = None               # ... and the mask object itself (so its id() cannot be recycled)
         self._predicate_masks: dict = {}     # (id(predicate), generation, n) -> packed bitmask
         self._range_hint = 0                 # hits of the last search_range: the next one's capacity hint
         self.clear()
@@ -347,6 +349,8 @@ class VectorBase:
         self._count = n - len(removed)
         self._mask_key = None
         self._mask_ref = None
+        self._qmask_key = None
+        self._qmask_ref = None
         self._predicate_masks.clear()
 
     def remove_embedding_at(self, pos: int) -> None:
@@ -421,8 +425,10 @@ class VectorBase:
             self._ix_rows = 0
             self._ix_generation = self._generation
             self._mask_key = None
+            self._qmask_key = None
         if self._ix_rows < self._count:
             self._mask_key = None
+            self._qmask_key = None
             fresh = np.ascontiguousarray(self._buf[self._ix_rows : self._count])
             _capi.check(
                 lib.tav_append(self._ix, fresh.ctypes.data_as(C.c_void_p), len(fresh),
@@ -474,6 +480,59 @@ class VectorBase:
         self._mask_key = key
         self._mask_ref = (allowed, owner)
 
+    @staticmethod
+    def pack_query_masks(allowed) -> np.ndarray:
+        """bool [B, N] -> little-endian bit-packed uint32 words [B, ceil(N / 32)] (row b: query b's mask, in the
+        bit order of ``pack_row_mask``)."""
+        bits = np.packbits(np.asarray(allowed, dtype=bool), axis=1, bitorder="little")
+        pad = (-bits.shape[1]) % 4
+        if pad:
+            bits = np.concatenate([bits, np.zeros((len(bits), pad), np.uint8)], axis=1)
+        return np.ascontiguousarray(bits).view(np.uint32)
+
+    @staticmethod
+    def _is_query_masks(allowed) -> bool:
+        """A 2-D ``allowed=``: one mask per query."""
+        return allowed is not None and len(getattr(allowed, "shape", np.shape(allowed))) == 2
+
+    def _use_query_masks(self, lib, ix, allowed, n_queries: int, stream=None) -> None:
+        """Upload a 2-D ``allowed`` (bool [B, N], packed uint32 [B, ceil(N / 32)], or an int32 CUDA tensor of
+        those words, copied on ``stream``) unless it is the set already on the device.  Like the row mask, the
+        masks are treated as immutable: identity + row generation + rows is the key."""
+        n = len(self)
+        words_per = (n + 31) // 32
+        shape = tuple(getattr(allowed, "shape", np.shape(allowed)))
+        if shape[0] != n_queries:
+            raise ValueError(f"query masks have {shape[0]} rows for {n_queries} queries")
+        key = (id(allowed), self._generation, n)
+        if self._qmask_key == key:
+            return
+        self._qmask_key = None
+        if getattr(allowed, "is_cuda", False):
+            import torch
+
+            if not (allowed.dtype == torch.int32 and allowed.is_contiguous()):
+                raise ValueError("device query masks must be a contiguous int32 CUDA tensor of packed words")
+            if allowed.device.index != self._device:
+                raise ValueError(f"device query masks are on cuda:{allowed.device.index}, the index on cuda:{self._device}")
+            if shape[1] != words_per:
+                raise ValueError(f"query masks have {shape[1] * 32} bits for {n} rows")
+            _capi.check(lib.tav_set_query_masks(ix, C.c_void_p(allowed.data_ptr()), n_queries, n, words_per, 1,
+                                                C.c_void_p(stream)))
+        else:
+            if getattr(allowed, "dtype", None) == np.uint32:
+                if shape[1] != words_per:
+                    raise ValueError(f"query masks have {shape[1] * 32} bits for {n} rows")
+                words = np.ascontiguousarray(allowed)
+            else:
+                if shape[1] != n:
+                    raise ValueError(f"query masks have {shape[1]} entries for {n} rows")
+                words = self.pack_query_masks(allowed)
+            _capi.check(lib.tav_set_query_masks(ix, words.ctypes.data_as(C.c_void_p), n_queries, n, words_per, 0,
+                                                None))
+        self._qmask_key = key
+        self._qmask_ref = allowed
+
     def _check_queries(self, queries) -> np.ndarray:
         q = np.ascontiguousarray(queries, dtype=np.float32)
         if q.ndim == 1:
@@ -500,8 +559,9 @@ class VectorBase:
         counts int32 [B] (entries beyond counts[b] are padding: item -1, score 0).  `k` is
         clamped to the number of rows searched.  ``out`` may supply preallocated (e.g. pinned)
         C-contiguous result arrays of exactly those shapes and dtypes.  ``allowed`` (bool [N] or
-        bit-packed uint32) restricts the lookup to rows whose bit is set, inside the kernels;
-        ``ties_low_first`` orders exactly equal scores by ascending ordinal (row-scan path)."""
+        bit-packed uint32) restricts the lookup to rows whose bit is set, inside the kernels; a 2-D ``allowed``
+        (bool [B, N] or bit-packed uint32 [B, ceil(N / 32)]) gives every query its own mask, in one batched
+        search; ``ties_low_first`` orders exactly equal scores by ascending ordinal (row-scan path)."""
         q = self._check_queries(queries)
         b = len(q)
         if k < 1:
@@ -535,8 +595,12 @@ class VectorBase:
         if allowed is not None:
             if sub is not None:
                 raise ValueError("allowed= and subset= cannot be combined")
-            self._use_row_mask(lib, ix, allowed, _mask_key, _mask_owner)
-            flags |= _capi.TAV_USE_ROW_MASK
+            if self._is_query_masks(allowed):
+                self._use_query_masks(lib, ix, allowed, b)
+                flags |= _capi.TAV_USE_QUERY_MASKS
+            else:
+                self._use_row_mask(lib, ix, allowed, _mask_key, _mask_owner)
+                flags |= _capi.TAV_USE_ROW_MASK
         if ties_low_first:
             flags |= _capi.TAV_TIES_LOW_FIRST
         with self._single_lock:
@@ -563,7 +627,7 @@ class VectorBase:
         the rows.  Returns CSR arrays: offsets int64 [B + 1], items int64 [T], scores float32 [T];
         query b's hits are items[offsets[b]:offsets[b + 1]], in the library's order (score descending,
         equal scores higher ordinal first, or lower first with ``ties_low_first``).  ``subset`` and
-        ``allowed`` as in ``search_arrays``.  Batches run on the tensor cores (16-bit storage, or float32
+        ``allowed`` (1-D, or 2-D: one mask per query) as in ``search_arrays``.  Batches run on the tensor cores (16-bit storage, or float32
         through its fp16 planes), like ``search_arrays``.  The previous call's total sizes the device buffers."""
         q = self._check_queries(queries)
         b = len(q)
@@ -590,7 +654,10 @@ class VectorBase:
         b = len(q)
         lib, ix = self._ensure_device()
         flags = self._flags() & ~_capi.TAV_NO_FUSED_SCAN
-        if allowed is not None:
+        if self._is_query_masks(allowed):
+            self._use_query_masks(lib, ix, allowed, b)
+            flags |= _capi.TAV_USE_QUERY_MASKS
+        elif allowed is not None:
             self._use_row_mask(lib, ix, allowed)
             flags |= _capi.TAV_USE_ROW_MASK
         if ties_low_first:
@@ -883,7 +950,8 @@ class VectorBase:
         the device.  The tensor-core path normally ends with one host synchronisation (did any
         query need the exact fallback?); with ``defer_check=True`` the call is fully
         asynchronous and ``finish_search()`` must run before the results are trusted.
-        ``allowed``: row bitmask (see ``search_arrays``).  ``row_to_group``: int32 CUDA tensor [N];
+        ``allowed``: row bitmask, or one per query (see ``search_arrays``; here also a contiguous int32 CUDA
+        tensor [B, ceil(N / 32)] of packed words, copied on the current stream).  ``row_to_group``: int32 CUDA tensor [N];
         the hits are then folded on the device like the reference's chunk -> message fold
         (storage/memory/messageindex.py:185-207): first hit per group, items = group ordinals."""
         import torch
@@ -906,7 +974,10 @@ class VectorBase:
         flags = _capi.TAV_QUERIES_ON_DEVICE | _capi.TAV_OUTPUTS_ON_DEVICE | self._flags()
         if defer_check and row_to_group is None:
             flags |= _capi.TAV_DEFER_RETRY
-        if allowed is not None:
+        if self._is_query_masks(allowed):
+            self._use_query_masks(lib, ix, allowed, b, stream)
+            flags |= _capi.TAV_USE_QUERY_MASKS
+        elif allowed is not None:
             self._use_row_mask(lib, ix, allowed)
             flags |= _capi.TAV_USE_ROW_MASK
         floor = float(np.float32(min_score))
@@ -926,7 +997,7 @@ class VectorBase:
             )
         if flags & _capi.TAV_DEFER_RETRY:
             # the library redoes flagged queries into these very buffers at finish_search(): keep them alive
-            self._pending.append((queries, items, scores, counts, stream))
+            self._pending.append((queries, items, scores, counts, stream, allowed))
         return items, scores, counts
 
     def finish_search(self) -> int:
