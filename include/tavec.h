@@ -205,6 +205,33 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
 int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items, float* out_scores,
                     int flags, void* stream);
 
+/*
+ * Per-query subsets: one batched lookup in which query q scores only its own entries
+ * ordinals[offsets[q] .. offsets[q + 1]) (the candidate re-ranking of fuzzy_lookup_embedding_in_subset,
+ * vectorbase.py:203-230, for a whole batch).  `offsets` is host int64 [n_queries + 1], starting at 0 and never
+ * decreasing, at most 2^32 - 1 in all; `ordinals` is host int64 [offsets[n_queries]].  Row q of the result equals,
+ * bit for bit, tav_search (tav_range_search) of query q alone with its entries as the subset: repeated ordinals
+ * are scored and returned once per occurrence, negative ordinals wrap like numpy and come back as given, equal
+ * scores put the later entry first (the earlier with TAV_TIES_LOW_FIRST), an empty subset, an empty corpus or a
+ * NaN min_score give no hits.  With TAV_ITEMS_AS_POSITIONS the item is the hit's flat index into `ordinals`.
+ * Other accepted flags: TAV_QUERIES_ON_DEVICE, TAV_OUTPUTS_ON_DEVICE; any other flag, malformed offsets or more
+ * than 2^32 - 1 ordinals: TAV_ERR_INVALID; an ordinal outside [-size, size): TAV_ERR_RANGE.  Every check runs on
+ * the host before any work.  One gather reads each entry's row once (the row scan's arithmetic, path 1 in
+ * tav_last_timing), and each query's hits are sorted by the threshold search's segmented sort; the number of
+ * launches does not depend on n_queries.  Both calls synchronise once, to learn the hit counts, and replace the
+ * hits of the last range search.
+ *
+ * tav_search_subsets: out_items / out_scores [n_queries, k], out_counts [n_queries]; count q is at most
+ * min(k, entries of q); the slots after it hold item -1, score 0.
+ * tav_range_search_subsets: CSR offsets out_offsets [n_queries + 1] of every hit at or above min_score;
+ * tav_range_fetch copies the hits out.
+ */
+int tav_search_subsets(tav_index* ix, const float* queries, int n_queries, int k, float min_score, int flags,
+                       const int64_t* offsets, const int64_t* ordinals, int64_t* out_items, float* out_scores,
+                       int32_t* out_counts, void* stream);
+int tav_range_search_subsets(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
+                             const int64_t* offsets, const int64_t* ordinals, int64_t* out_offsets, void* stream);
+
 /* Completes EVERY outstanding TAV_DEFER_RETRY search of the index, whatever stream each was issued
  * on: waits until they have run (`stream` first waits for them, then is synchronised), redoes
  * each search's flagged queries exactly on `stream` into that search's own outputs and reports how many

@@ -199,6 +199,8 @@ struct tav_index {
     DevBuf range_mmaws, range_mmaws2, range_mmaaux;  // tensor-core collection: workspaces, scratch
     DevBuf range_items, range_scores;
     int64_t range_total = 0;     // hits of the last range search held in range_items / range_scores
+    // per-query subsets: device [offsets | work-item starts | CSR offsets of the hits], each n_queries + 1
+    DevBuf subsets_meta;
 
     // call order on the device (join_stream / mark_queued / wait_queued): ev_last marks the end of the work
     // of the calls so far while `outstanding`; last_stream is ordered after it
@@ -401,7 +403,7 @@ int tav_destroy(tav_index* ix) {
                       &ix->qmask, &ix->qmask_pop, &ix->range_qmap,
                       &ix->range_keys, &ix->range_keys2, &ix->range_counts, &ix->range_qgather, &ix->range_tmp,
                       &ix->range_sortws, &ix->range_items, &ix->range_scores, &ix->range_mmaws,
-                      &ix->range_mmaws2, &ix->range_mmaaux, &ix->compact_keys})
+                      &ix->range_mmaws2, &ix->range_mmaaux, &ix->compact_keys, &ix->subsets_meta})
         b->release();
     for (DevBuf& b : ix->held_retired) b.release();
     if (ix->ev_last) cudaEventDestroy(ix->ev_last);
@@ -2124,6 +2126,251 @@ int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items,
     TAV_CUDA(cudaStreamSynchronize(s));
     mark_done(ix);
     return TAV_OK;
+}
+
+}  // extern "C"
+
+// ---- per-query subsets (tav_search_subsets, tav_range_search_subsets) ------------------------------------
+constexpr int kSubsetsFlags = TAV_QUERIES_ON_DEVICE | TAV_OUTPUTS_ON_DEVICE | TAV_TIES_LOW_FIRST | TAV_ITEMS_AS_POSITIONS;
+
+// the argument checks of both entry points that need no index state
+static int check_subsets(const char* fn, int n_queries, int flags, const int64_t* offsets, const int64_t* ordinals) {
+    if (flags & ~kSubsetsFlags) {
+        set_error("%s: flags 0x%x are not available with per-query subsets", fn, flags & ~kSubsetsFlags);
+        return TAV_ERR_INVALID;
+    }
+    if (!offsets || offsets[0] != 0) {
+        set_error("%s: offsets must be n_queries + 1 values starting at 0", fn);
+        return TAV_ERR_INVALID;
+    }
+    for (int q = 0; q < n_queries; ++q)
+        if (offsets[q + 1] < offsets[q]) {
+            set_error("%s: offsets decrease at query %d", fn, q);
+            return TAV_ERR_INVALID;
+        }
+    if (offsets[n_queries] > 0xFFFFFFFFll) {  // flat positions live in the low word of a key
+        set_error("%s: %lld ordinals; at most 2^32 - 1 per call", fn, (long long)offsets[n_queries]);
+        return TAV_ERR_INVALID;
+    }
+    if (offsets[n_queries] > 0 && !ordinals) {
+        set_error("%s: ordinals is NULL", fn);
+        return TAV_ERR_INVALID;
+    }
+    return TAV_OK;
+}
+
+static int check_subset_ordinals(const tav_index* ix, const int64_t* ordinals, int64_t n) {
+    for (int64_t i = 0; i < n; ++i)
+        if (ordinals[i] < -ix->size || ordinals[i] >= ix->size) {
+            set_error("index %lld is out of bounds for axis 0 with size %lld", (long long)ordinals[i],
+                      (long long)ix->size);
+            return TAV_ERR_RANGE;
+        }
+    return TAV_OK;
+}
+
+// Every entry of every query's subset scored in one gather, each query's admitted keys sorted: the hits in CSR
+// order in ix->range_items / range_scores, csr[nq + 1] on the host.  Synchronises once, to learn the counts.
+static int subsets_core(tav_index* ix, TimedSearch* ts, bool timing, const float* queries, int nq, bool q_dev,
+                        float floor, int ties_low, int positions, const int64_t* offsets, const int64_t* ordinals,
+                        std::vector<int64_t>& csr, cudaStream_t s) {
+    if (scan_collect_max_queries(ix->dim) < 1) {  // one query row in shared memory, as the row scan stages it
+        set_error("per-query subsets: embedding size %d too large for the row-scan kernel", ix->dim);
+        return TAV_ERR_INVALID;
+    }
+    const int64_t total = offsets[nq];
+#if TAV_SUBSETS_MUTANT == 2
+    std::vector<int64_t> wrapped(ordinals, ordinals + total);
+    for (int64_t& o : wrapped)
+        if (o < 0) o += ix->size;
+    ordinals = wrapped.data();
+#endif
+    const float* d_queries = nullptr;
+    const int64_t* d_ordinals = nullptr;
+    if (int rc = stage_inputs(ix, ts, timing, queries, nq, q_dev, false, ordinals, total, &d_queries, &d_ordinals, s))
+        return rc;
+    // device [offsets | work0 | csr]: query q's work items (tiles of its entries) are [work0[q], work0[q + 1])
+    const size_t n1 = static_cast<size_t>(nq) + 1;
+    std::vector<int64_t> meta(2 * n1);
+    memcpy(meta.data(), offsets, n1 * sizeof(int64_t));
+    int64_t* work0 = meta.data() + n1;
+    work0[0] = 0;
+    for (int q = 0; q < nq; ++q) work0[q + 1] = work0[q] + (offsets[q + 1] - offsets[q] + kSubsetTile - 1) / kSubsetTile;
+    if (int rc = range_alloc(ix->subsets_meta, 3 * n1 * sizeof(int64_t), "the subset offsets")) return rc;
+    int64_t* d_meta = static_cast<int64_t*>(ix->subsets_meta.p);
+    // from pageable memory: consumed when the call returns
+    TAV_CUDA(cudaMemcpyAsync(d_meta, meta.data(), meta.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(total) * sizeof(uint64_t), "the hit regions")) return rc;
+    if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(nq) * sizeof(uint32_t), "the hit counters")) return rc;
+    uint32_t* d_counts = static_cast<uint32_t*>(ix->range_counts.p);
+    uint64_t* keys = static_cast<uint64_t*>(ix->range_keys.p);
+    TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(nq) * sizeof(uint32_t), s));
+
+    SubsetArgs a{};
+    a.corpus = ix->rows;
+    a.dtype = ix->dtype;
+    a.n_corpus = ix->size;
+    a.dim = ix->dim;
+    a.queries = d_queries;
+    a.nq = nq;
+    a.ordinals = d_ordinals;
+    a.offsets = d_meta;
+    a.work0 = d_meta + n1;
+    a.n_work = work0[nq];
+    a.floor_score = floor;
+    a.ties_low = ties_low;
+    a.keys = keys;
+    a.counts = d_counts;
+    const bool timed = timing && ts->used < kMaxTimedKernels;
+    if (timed) TAV_CUDA(ev_record(ts->ev[ts->used][0], s));
+    TAV_CUDA(launch_subset_gather(a, s));
+    if (timed) {
+        ts->kind[ts->used] = 0;
+        TAV_CUDA(ev_record(ts->ev[ts->used++][1], s));
+    }
+    ts->launches += 1;
+
+    std::vector<uint32_t> cnt(static_cast<size_t>(nq));
+    TAV_CUDA(cudaMemcpyAsync(cnt.data(), d_counts, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaStreamSynchronize(s));
+    csr.assign(n1, 0);
+    std::vector<SortSeg> segs(static_cast<size_t>(nq));
+    for (int q = 0; q < nq; ++q) {
+        csr[q + 1] = csr[q] + cnt[q];
+        segs[q].keys = keys + offsets[q];
+        segs[q].out = csr[q];
+        segs[q].n = cnt[q];
+    }
+    return range_sort(ix, ts, timing, segs, csr[nq], positions ? nullptr : d_ordinals, 0, ties_low, s);
+}
+
+// the timing record of a subsets call
+static TimedSearch* begin_subsets_timing(tav_index* ix) {
+    ix->last_first_slot = -1;
+    ix->last_n_slots = 0;
+    TimedSearch* ts = cur_timed(ix);
+    if (!ts) ts = &ix->untimed;
+    ts->used = 0;
+    ts->launches = 0;
+    ts->path = 1;
+    ts->valid = false;
+    return ts;
+}
+
+extern "C" {
+
+int tav_search_subsets(tav_index* ix, const float* queries, int n_queries, int k, float min_score, int flags,
+                       const int64_t* offsets, const int64_t* ordinals, int64_t* out_items, float* out_scores,
+                       int32_t* out_counts, void* stream) {
+    if (!ix || n_queries < 0 || k < 1 || (n_queries > 0 && (!queries || !out_items || !out_scores || !out_counts))) {
+        set_error("tav_search_subsets: invalid argument (k must be >= 1)");
+        return TAV_ERR_INVALID;
+    }
+    if (int rc = check_subsets("tav_search_subsets", n_queries, flags, offsets, ordinals)) return rc;
+    if (n_queries == 0) return TAV_OK;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (int rc = set_device(ix)) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;
+    const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
+    const size_t nk = static_cast<size_t>(n_queries) * k;
+    const int64_t total = offsets[n_queries];
+    // no entries, no rows or a NaN min_score: no hits (as tav_search, before the ordinals are looked at)
+    if (total == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score) {
+        if (o_dev) {
+            TAV_CUDA(cudaMemsetAsync(out_items, 0xFF, nk * sizeof(int64_t), s));
+            TAV_CUDA(cudaMemsetAsync(out_scores, 0, nk * sizeof(float), s));
+            TAV_CUDA(cudaMemsetAsync(out_counts, 0, static_cast<size_t>(n_queries) * sizeof(int32_t), s));
+            return mark_queued(ix, s);
+        }
+        std::fill(out_items, out_items + nk, int64_t(-1));
+        std::fill(out_scores, out_scores + nk, 0.0f);
+        std::fill(out_counts, out_counts + n_queries, 0);
+        return TAV_OK;
+    }
+    if (int rc = check_subset_ordinals(ix, ordinals, total)) return rc;
+    TimedSearch* ts = begin_subsets_timing(ix);
+    const bool timing = ts != &ix->untimed;
+    const int ties_low = (flags & TAV_TIES_LOW_FIRST) && TAV_SUBSETS_MUTANT != 3 ? 1 : 0;
+    std::vector<int64_t> csr;
+    ix->range_total = 0;  // the hits land in the threshold search's buffers
+    if (int rc = subsets_core(ix, ts, timing, queries, n_queries, q_dev, min_score, ties_low,
+                              (flags & TAV_ITEMS_AS_POSITIONS) ? 1 : 0, offsets, ordinals, csr, s))
+        return rc;
+    ix->range_total = csr[n_queries];
+    const size_t n1 = static_cast<size_t>(n_queries) + 1;
+    int64_t* d_csr = static_cast<int64_t*>(ix->subsets_meta.p) + 2 * n1;
+    // from pageable memory: consumed when the call returns
+    TAV_CUDA(cudaMemcpyAsync(d_csr, csr.data(), n1 * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    int64_t* d_items = out_items;
+    float* d_scores = out_scores;
+    int32_t* d_counts = out_counts;
+    const size_t off_scores = nk * sizeof(int64_t);
+    const size_t off_counts = off_scores + ((nk * sizeof(float) + 7) & ~size_t(7));
+    if (!o_dev) {
+        TAV_CUDA(ix->out_pack.ensure(off_counts + static_cast<size_t>(n_queries) * sizeof(int32_t)));
+        char* base = static_cast<char*>(ix->out_pack.p);
+        d_items = reinterpret_cast<int64_t*>(base);
+        d_scores = reinterpret_cast<float*>(base + off_scores);
+        d_counts = reinterpret_cast<int32_t*>(base + off_counts);
+    }
+    TAV_CUDA(launch_subset_topk_layout(n_queries, k, d_csr, static_cast<const int64_t*>(ix->range_items.p),
+                                       static_cast<const float*>(ix->range_scores.p), d_items, d_scores, d_counts, s));
+    ts->launches += 1;
+    if (timing) {
+        TAV_CUDA(ev_record(ts->total[1], s));
+        ++ix->search_seq;
+    }
+    ts->valid = true;
+    if (o_dev) return mark_queued(ix, s);
+    TAV_CUDA(cudaMemcpyAsync(out_items, d_items, nk * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaMemcpyAsync(out_scores, d_scores, nk * sizeof(float), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaMemcpyAsync(out_counts, d_counts, static_cast<size_t>(n_queries) * sizeof(int32_t),
+                             cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaStreamSynchronize(s));
+    mark_done(ix);
+    return TAV_OK;
+}
+
+int tav_range_search_subsets(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
+                             const int64_t* offsets, const int64_t* ordinals, int64_t* out_offsets, void* stream) {
+    if (!ix || n_queries < 0 || !out_offsets || (n_queries > 0 && !queries)) {
+        set_error("tav_range_search_subsets: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    if (int rc = check_subsets("tav_range_search_subsets", n_queries, flags, offsets, ordinals)) return rc;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (int rc = set_device(ix)) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = join_stream(ix, s)) return rc;  // (also: a queued tav_range_fetch reads the hits replaced here)
+    const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
+    const int64_t total = offsets[n_queries];
+    const bool none = n_queries == 0 || total == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score;
+    if (!none)
+        if (int rc = check_subset_ordinals(ix, ordinals, total)) return rc;
+    std::vector<int64_t> csr(static_cast<size_t>(n_queries) + 1, 0);
+    ix->range_total = 0;
+    if (!none) {
+        TimedSearch* ts = begin_subsets_timing(ix);
+        const bool timing = ts != &ix->untimed;
+        if (int rc = subsets_core(ix, ts, timing, queries, n_queries, q_dev, min_score,
+                                  (flags & TAV_TIES_LOW_FIRST) && TAV_SUBSETS_MUTANT != 3 ? 1 : 0,
+                                  (flags & TAV_ITEMS_AS_POSITIONS) ? 1 : 0, offsets, ordinals, csr, s))
+            return rc;
+        if (timing) {
+            TAV_CUDA(ev_record(ts->total[1], s));
+            ++ix->search_seq;
+        }
+        ts->valid = true;
+        ix->range_total = csr[n_queries];
+    }
+    const size_t bytes = csr.size() * sizeof(int64_t);
+    if (o_dev) {  // from pageable memory: consumed when the call returns
+        TAV_CUDA(cudaMemcpyAsync(out_offsets, csr.data(), bytes, cudaMemcpyHostToDevice, s));
+    } else {
+        memcpy(out_offsets, csr.data(), bytes);
+    }
+    return mark_queued(ix, s);  // the sort after the synchronisation may still run
 }
 
 int tav_mma_scores(tav_index* ix, const float* queries, int n_queries, int flags, float* out_device,

@@ -94,6 +94,41 @@ int scan_collect_max_queries(int dim);          // queries one collect-mode pass
 int scan_collect_grid(int device, int dim, int nq, int64_t n_scan);
 cudaError_t launch_scan_collect(const ScanArgs& a, cudaStream_t s);
 
+// ---- per-query subsets (tav_search_subsets / tav_range_search_subsets, tav_scan.cu) ------
+// Query q scores the entries [offsets[q], offsets[q + 1]) of one flat ordinal list.  The work is a flat space of
+// (query, tile of kSubsetTile entries) items: query q's tiles are [work0[q], work0[q + 1]).  Every admitted
+// entry j appends the key (score, j, or ~j with ties_low) to keys + offsets[q] through counts[q]: a query
+// admits at most its own entries, so its region never overflows.
+constexpr int kSubsetTile = 256;
+struct SubsetArgs {
+    const void* corpus;       // [n_corpus, dim] storage dtype
+    int dtype;
+    int64_t n_corpus;
+    int dim;
+    const float* queries;     // device float32 [nq, dim]
+    int nq;
+    const int64_t* ordinals;  // device [offsets[nq]], validated, numpy-style negatives
+    const int64_t* offsets;   // device [nq + 1]
+    const int64_t* work0;     // device [nq + 1]
+    int64_t n_work;
+    float floor_score;
+    int ties_low;
+    uint64_t* keys;           // [offsets[nq]]
+    uint32_t* counts;         // [nq], zero on entry
+};
+cudaError_t launch_subset_gather(const SubsetArgs& a, cudaStream_t s);
+// [nq, k] layout of sorted CSR hits: the first min(k, count) of each query, -1 / 0 padding after them
+cudaError_t launch_subset_topk_layout(int nq, int k, const int64_t* csr_offsets, const int64_t* hits,
+                                      const float* hit_scores, int64_t* out_items, float* out_scores,
+                                      int32_t* out_counts, cudaStream_t s);
+
+// TAV_SUBSETS_MUTANT (tests only, never set by build.py): 1..3 compile one deliberate defect each, so that
+// tests/test_gpu_subsets.py can show its exact checks catch it: 1 a query's later tiles start one entry late
+// when its length is not a multiple of the tile, 2 negative ordinals come back wrapped, 3 ties-low ignored.
+#ifndef TAV_SUBSETS_MUTANT
+#define TAV_SUBSETS_MUTANT 0
+#endif
+
 // ---- segmented sort of the threshold search's keys (tav_sort.cu) -----------------------
 // One segment per query: n keys (unsorted, unique) at `keys`; sorted descending and decoded into
 // out_items / out_scores [out, out + n).  Segments above kSmallSortMax keys also need `tmp` (n keys of

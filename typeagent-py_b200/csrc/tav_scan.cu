@@ -611,6 +611,166 @@ cudaError_t launch_scan_collect(const ScanArgs& a, cudaStream_t s) {
     return cudaErrorInvalidValue;
 }
 
+// ---- per-query subsets: one gather over a batch whose queries score different rows ---------------
+// Each (query, entry) dot is computed as the row scan computes it with one query per pass (QB = 1): the same
+// lane-strided loads, fmaf order and warp_transpose_reduce<4> tree, so row b of a batch equals the one-query
+// subset search bit for bit.  A CTA walks work items (query, tile); it stages a query only when the query changes.
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kScanThreads) subset_gather_kernel(const SubsetArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    float* sq = reinterpret_cast<float*>(smem_raw);
+    __shared__ int s_q;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int dim = a.dim;
+    const T* corpus = reinterpret_cast<const T*>(a.corpus);
+    int cur = -1;
+    for (int64_t w = blockIdx.x; w < a.n_work; w += gridDim.x) {
+        __syncthreads();  // the previous item is done with s_q and sq
+        if (tid == 0) {   // the query of item w: the last q with work0[q] <= w
+            int lo = 0, hi = a.nq - 1;
+            while (lo < hi) {
+                const int mid = (lo + hi + 1) >> 1;
+                if (a.work0[mid] <= w) lo = mid;
+                else hi = mid - 1;
+            }
+            s_q = lo;
+        }
+        __syncthreads();
+        const int q = s_q;
+        if (q != cur) {  // CTA-uniform
+            for (int i = tid; i < dim; i += kScanThreads) sq[i] = a.queries[static_cast<size_t>(q) * dim + i];
+            __syncthreads();
+            cur = q;
+        }
+        const int64_t q_begin = a.offsets[q], q_end = a.offsets[q + 1];
+        int64_t begin = q_begin + (w - a.work0[q]) * kSubsetTile;
+#if TAV_SUBSETS_MUTANT == 1
+        if (w > a.work0[q] && (q_end - q_begin) % kSubsetTile != 0) ++begin;
+#endif
+        const int64_t end = min(begin + kSubsetTile, q_end);
+        uint64_t* qkeys = a.keys + q_begin;
+        for (int64_t pos0 = begin + warp * kRowsPerWarp; pos0 < end; pos0 += kRoundRows) {  // warp-uniform
+            const T* rp[kRowsPerWarp];
+#pragma unroll
+            for (int r = 0; r < kRowsPerWarp; ++r) {
+                int64_t row = 0;
+                if (pos0 + r < end) {
+                    row = a.ordinals[pos0 + r];
+                    if (row < 0) row += a.n_corpus;  // numpy-style negative ordinals
+                }
+                rp[r] = corpus + row * dim;
+            }
+            float acc[kRowsPerWarp];
+#pragma unroll
+            for (int r = 0; r < kRowsPerWarp; ++r) acc[r] = 0.0f;
+            if constexpr (VEC) {
+                constexpr int E = Vec<T>::kElems;
+                const int nvec = dim / E;
+                for (int c = lane; c < nvec; c += 32) {
+                    float f[kRowsPerWarp][E];
+#pragma unroll
+                    for (int r = 0; r < kRowsPerWarp; ++r) Vec<T>::load(rp[r] + c * E, f[r]);
+                    const float4* q4 = reinterpret_cast<const float4*>(sq + c * E);
+#pragma unroll
+                    for (int h = 0; h < E / 4; ++h) {
+                        const float4 qv = q4[h];
+#pragma unroll
+                        for (int r = 0; r < kRowsPerWarp; ++r) {
+                            float s = acc[r];
+                            s = fmaf(f[r][4 * h + 0], qv.x, s);
+                            s = fmaf(f[r][4 * h + 1], qv.y, s);
+                            s = fmaf(f[r][4 * h + 2], qv.z, s);
+                            s = fmaf(f[r][4 * h + 3], qv.w, s);
+                            acc[r] = s;
+                        }
+                    }
+                }
+            } else {
+                for (int c = lane; c < dim; c += 32) {
+                    float f[kRowsPerWarp];
+#pragma unroll
+                    for (int r = 0; r < kRowsPerWarp; ++r) f[r] = to_float(rp[r][c]);
+                    const float qv = sq[c];
+#pragma unroll
+                    for (int r = 0; r < kRowsPerWarp; ++r) acc[r] = fmaf(f[r], qv, acc[r]);
+                }
+            }
+            warp_transpose_reduce<kRowsPerWarp>(acc, lane);
+
+            // lane 8r holds entry pos0 + r; the warp's admitted keys take one atomic
+            constexpr int kLanesPerValue = 32 / kRowsPerWarp;
+            const int64_t pos = pos0 + lane / kLanesPerValue;
+            const float s = score_from_dot(acc[0]);
+            const bool want = (lane & (kLanesPerValue - 1)) == 0 && pos < end && s >= a.floor_score;  // NaN rejected
+            const unsigned m = __ballot_sync(0xFFFFFFFFu, want);
+            if (m == 0) continue;
+            const int leader = __ffs(m) - 1;
+            uint32_t base = 0;
+            if (lane == leader) base = atomicAdd(&a.counts[q], static_cast<uint32_t>(__popc(m)));
+            base = __shfl_sync(0xFFFFFFFFu, base, leader);
+            if (want) {
+                const uint32_t j = static_cast<uint32_t>(pos);  // flat index into the ordinals (< 2^32)
+                qkeys[base + __popc(m & ((1u << lane) - 1u))] = make_key(s, a.ties_low ? ~j : j);
+            }
+        }
+    }
+}
+
+template <typename T>
+static cudaError_t launch_subset_gather_t(const SubsetArgs& a, cudaStream_t s) {
+    const size_t row_bytes = static_cast<size_t>(a.dim) * sizeof(T);
+    const bool vec = (row_bytes % 16 == 0) && (reinterpret_cast<uintptr_t>(a.corpus) % 16 == 0);
+    const size_t smem = collect_smem_bytes(1, a.dim);
+    auto kern = vec ? subset_gather_kernel<T, true> : subset_gather_kernel<T, false>;
+    static int granted[2][16] = {};
+    cudaError_t e = ensure_dynamic_smem(kern, smem, granted[vec ? 1 : 0]);
+    if (e != cudaSuccess) return e;
+    // one wave of as many CTAs as fit per SM (at most 4, the row scan's occupancy); the items are grid-strided
+    int device = 0, sms = 132, per_sm = 1;
+    if ((e = cudaGetDevice(&device)) != cudaSuccess) return e;
+    if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device)) != cudaSuccess) return e;
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kScanThreads, smem)) != cudaSuccess) return e;
+    per_sm = std::max(1, std::min(per_sm, 4));
+    const int grid = static_cast<int>(std::min<int64_t>(a.n_work, static_cast<int64_t>(sms) * per_sm));
+    kern<<<grid, kScanThreads, smem, s>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_subset_gather(const SubsetArgs& a, cudaStream_t s) {
+    if (a.n_work == 0) return cudaSuccess;
+    switch (a.dtype) {
+        case TAV_F32: return launch_subset_gather_t<float>(a, s);
+        case TAV_BF16: return launch_subset_gather_t<__nv_bfloat16>(a, s);
+        case TAV_F16: return launch_subset_gather_t<__half>(a, s);
+    }
+    return cudaErrorInvalidValue;
+}
+
+// one CTA per query
+__global__ void __launch_bounds__(256)
+subset_topk_layout_kernel(int k, const int64_t* __restrict__ csr_offsets, const int64_t* __restrict__ hits,
+                          const float* __restrict__ hit_scores, int64_t* out_items, float* out_scores,
+                          int32_t* out_counts) {
+    const int q = blockIdx.x;
+    const int64_t first = csr_offsets[q];
+    const int n = static_cast<int>(min(static_cast<int64_t>(k), csr_offsets[q + 1] - first));
+    int64_t* items = out_items + static_cast<size_t>(q) * k;
+    float* scores = out_scores + static_cast<size_t>(q) * k;
+    for (int j = threadIdx.x; j < k; j += 256) {
+        items[j] = j < n ? hits[first + j] : -1;
+        scores[j] = j < n ? hit_scores[first + j] : 0.0f;
+    }
+    if (threadIdx.x == 0) out_counts[q] = n;
+}
+
+cudaError_t launch_subset_topk_layout(int nq, int k, const int64_t* csr_offsets, const int64_t* hits,
+                                      const float* hit_scores, int64_t* out_items, float* out_scores,
+                                      int32_t* out_counts, cudaStream_t s) {
+    if (nq <= 0) return cudaSuccess;
+    subset_topk_layout_kernel<<<nq, 256, 0, s>>>(k, csr_offsets, hits, hit_scores, out_items, out_scores, out_counts);
+    return cudaGetLastError();
+}
+
 // ---- single-lookup latency form: query (and a short subset) in the kernel parameters ----------
 using SmallBlob = ParamBlob<kParamQuerySmall, 0>;                   // 4 KB of parameters
 using MidBlob = ParamBlob<kParamQuerySmall, kParamSubsetSmall>;    // 8 KB

@@ -11,7 +11,7 @@ table rather than boilerplate.
 
 from __future__ import annotations
 
-from collections.abc import Callable
+from collections.abc import Callable, Sequence
 
 import numpy as np
 
@@ -115,3 +115,14 @@ class EmbeddingIndex:
     ) -> list[list[ScoredInt]]:
         """One GPU search for a [B, D] batch of query embeddings."""
         return self._vector_base.fuzzy_lookup_embeddings(embeddings, max_matches, min_score)
+
+    def get_indexes_of_nearest_in_subsets_batch(
+        self,
+        embeddings: np.ndarray,
+        ordinals_of_subsets: Sequence[Sequence[int]],
+        max_matches: int | None = None,
+        min_score: float | None = None,
+    ) -> list[list[ScoredInt]]:
+        """One GPU search in which query b of a [B, D] batch scores only ``ordinals_of_subsets[b]``."""
+        return self._vector_base.fuzzy_lookup_embeddings_in_subsets(embeddings, ordinals_of_subsets, max_matches,
+                                                                    min_score)

@@ -26,7 +26,9 @@ Filtered and subset lookups (``predicate=``, ``fuzzy_lookup_embedding_in_subset`
 the packed layout over the process group and merge with ``tav_merge_topk_ordered``: a row mask (a predicate is
 evaluated by each rank over its own rows only) merges low row first where the reference's predicate path does;
 a subset is searched per rank with ``TAV_ITEMS_AS_POSITIONS``, its hits mapped to positions in the caller's
-subset (``tav_map_items``), merged by position and decoded through the caller's list at the end.
+subset (``tav_map_items``), merged by position and decoded through the caller's list at the end.  Per-query
+subsets (``subsets=``, ``fuzzy_lookup_embeddings_in_subsets``) do the same with ``tav_search_subsets`` and the
+entries' flat positions in the caller's concatenated ordinals.
 
 ``torch`` is plumbing here (process group, device buffers); the search, exchange and merge are
 libtavec kernels.  The engine is injectable so that the host logic (partitioning, packing, gather,
@@ -41,9 +43,13 @@ from array import array as _array
 import numpy as np
 
 from . import _capi
-from .vectorbase import ScoredInt, TextEmbeddingIndexSettings, VectorBase, _as_f32_scalar, removal_ordinals
+from .vectorbase import (_DEFAULT_MAX_HITS, ScoredInt, TextEmbeddingIndexSettings, VectorBase, _as_f32_scalar,
+                         removal_ordinals)
 
 RANGE_ROUTE_MIN_ROWS = 4 * 2048  # search_arrays with k >= rows above this (4 * TAV_PASS_K) -> search_range
+# per-query subsets with a larger k are served by the threshold exchange and cut to k: the top-k merge keeps k keys
+# per query in shared memory
+SUBSETS_MERGE_MAX_K = 2048
 
 
 def shard_bounds(n_rows: int, world: int) -> list[tuple[int, int]]:
@@ -273,6 +279,37 @@ class CudaShardEngine:
             self.map_items(buf[: b * k * 8].view(torch.int64), positions)
         return buf
 
+    def search_subsets_packed(self, queries: np.ndarray, k: int, min_score: float, local_offsets: np.ndarray,
+                              local_ordinals: np.ndarray, positions: np.ndarray, ties_low_first: bool):
+        """This rank's share of a per-query subsets search: ``tav_search_subsets`` over each query's block-local
+        entries (CSR ``local_offsets`` / ``local_ordinals``) with TAV_ITEMS_AS_POSITIONS, then those flat positions
+        mapped through ``positions`` (where the share's entries stand in the caller's concatenated ordinals,
+        ascending) by ``tav_map_items``.  Returns the packed buffer on the device; its items are flat positions in
+        the caller's ordinals.  A rank without a share hands in empty lists."""
+        torch = self.torch
+        b = len(queries)
+        off_s, off_c, total = packed_layout(b, k)
+        host = np.zeros(total, np.uint8)
+        if len(local_ordinals):
+            base = self.base
+            q = base._check_queries(queries)
+            offs = np.ascontiguousarray(local_offsets, np.int64)
+            ords = np.ascontiguousarray(local_ordinals, np.int64)
+            lib, ix = base._ensure_device()
+            flags = _capi.TAV_ITEMS_AS_POSITIONS | (_capi.TAV_TIES_LOW_FIRST if ties_low_first else 0)
+            items = host[: b * k * 8].view(np.int64)
+            scores = host[off_s: off_s + b * k * 4].view(np.float32)
+            counts = host[off_c: off_c + b * 4].view(np.int32)
+            with base._single_lock:
+                _capi.check(lib.tav_search_subsets(ix, q.ctypes.data_as(C.c_void_p), b, k, C.c_float(min_score), flags,
+                                                   offs.ctypes.data_as(C.c_void_p), ords.ctypes.data_as(C.c_void_p),
+                                                   items.ctypes.data_as(C.c_void_p), scores.ctypes.data_as(C.c_void_p),
+                                                   counts.ctypes.data_as(C.c_void_p), None))
+        buf = torch.from_numpy(host).to(self.device)
+        if len(local_ordinals):
+            self.map_items(buf[: b * k * 8].view(torch.int64), positions)
+        return buf
+
     def map_items(self, items, table: np.ndarray):
         """In place on the device: items[i] = table[items[i]] where 0 <= items[i] < len(table) (``tav_map_items``);
         ``items`` an int64 device tensor, ``table`` host int64."""
@@ -303,18 +340,21 @@ class CudaShardEngine:
 
     # ---- threshold search (search_range) ---------------------------------------------------
     def range_local(self, queries: np.ndarray, min_score: float, item_offset: int, ties_low_first: bool,
-                    mask=None, mask_key=None, mask_owner=None, subset=None, positions=None):
+                    mask=None, mask_key=None, mask_owner=None, subset=None, positions=None, subsets=None):
         """``tav_range_search`` on this rank's rows (items shifted by ``item_offset``).  Returns a
         ``LocalRange``: host offsets [B + 1] now, the hits later straight into the caller's buffers.  The
         hits wait in the index between the two calls, so the base's lookup lock is held until then.
-        ``mask`` as in ``search_rows_packed``.  ``subset`` / ``positions`` as in ``search_subset_packed``: the
-        hits' items are then positions in the caller's subset, and are fetched into device buffers only."""
+        ``mask`` as in ``search_rows_packed``.  ``subset`` / ``positions`` as in ``search_subset_packed``, or
+        ``subsets`` (this block's (offsets, ordinals) CSR) / ``positions`` as in ``search_subsets_packed``: the
+        hits' items are then positions in the caller's subset(s), and are fetched into device buffers only."""
         base = self.base
         b = len(queries)
-        if self.n_local() == 0 or (subset is not None and len(subset) == 0):
+        if (self.n_local() == 0 or (subset is not None and len(subset) == 0)
+                or (subsets is not None and len(subsets[1]) == 0)):
             return LocalRange(np.zeros(b + 1, np.int64), None, None)
         q = base._check_queries(queries)
         sub = None if subset is None else np.ascontiguousarray(subset, np.int64)
+        csr = None if subsets is None else tuple(np.ascontiguousarray(a, np.int64) for a in subsets)
         base._single_lock.acquire()
         try:
             lib, ix = base._ensure_device()
@@ -331,11 +371,18 @@ class CudaShardEngine:
                 flags |= _capi.TAV_ITEMS_AS_POSITIONS
                 item_offset = 0
             offsets = np.zeros(b + 1, np.int64)
-            _capi.check(lib.tav_range_search(ix, q.ctypes.data_as(C.c_void_p), b, C.c_float(min_score), flags,
-                                             None if sub is None else sub.ctypes.data_as(C.c_void_p),
-                                             0 if sub is None else len(sub), item_offset, base._range_hint,
-                                             offsets.ctypes.data_as(C.c_void_p), None))
-            base._range_hint = int(offsets[-1])
+            if csr is not None:
+                flags = _capi.TAV_ITEMS_AS_POSITIONS | (_capi.TAV_TIES_LOW_FIRST if ties_low_first else 0)
+                _capi.check(lib.tav_range_search_subsets(ix, q.ctypes.data_as(C.c_void_p), b, C.c_float(min_score),
+                                                         flags, csr[0].ctypes.data_as(C.c_void_p),
+                                                         csr[1].ctypes.data_as(C.c_void_p),
+                                                         offsets.ctypes.data_as(C.c_void_p), None))
+            else:
+                _capi.check(lib.tav_range_search(ix, q.ctypes.data_as(C.c_void_p), b, C.c_float(min_score), flags,
+                                                 None if sub is None else sub.ctypes.data_as(C.c_void_p),
+                                                 0 if sub is None else len(sub), item_offset, base._range_hint,
+                                                 offsets.ctypes.data_as(C.c_void_p), None))
+                base._range_hint = int(offsets[-1])
         except BaseException:
             base._single_lock.release()
             raise
@@ -346,13 +393,13 @@ class CudaShardEngine:
             if n == 0:
                 return
             on_device = not isinstance(items, np.ndarray)
-            if sub is not None and not on_device:
+            if (sub is not None or csr is not None) and not on_device:
                 raise ValueError("the hits of a subset threshold search are fetched into device buffers")
             ip = C.c_void_p(items.data_ptr()) if on_device else items.ctypes.data_as(C.c_void_p)
             sp = C.c_void_p(scores.data_ptr()) if on_device else scores.ctypes.data_as(C.c_void_p)
             _capi.check(lib.tav_range_fetch(ix, 0, n, ip, sp, _capi.TAV_OUTPUTS_ON_DEVICE if on_device else 0,
                                             C.c_void_p(stream) if on_device else None))
-            if sub is not None:
+            if sub is not None or csr is not None:
                 self.map_items(items[:n], positions)
 
         return LocalRange(offsets, fetch, base._single_lock)
@@ -433,6 +480,24 @@ def subset_share(sub: np.ndarray, n_rows: int, lo: int, hi: int) -> tuple[np.nda
     return pos, rows[pos] - lo
 
 
+def check_subsets_total(total: int) -> None:
+    """ValueError when a per-query subsets lookup has 2^32 ordinals or more: their flat positions are 32-bit keys."""
+    if total >= 1 << 32:
+        raise ValueError(f"{total} ordinals in one per-query subsets lookup; at most 2^32 - 1")
+
+
+def subsets_share(offsets: np.ndarray, ordinals: np.ndarray, n_rows: int, lo: int,
+                  hi: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """The entries of per-query subsets (CSR ``offsets`` [B + 1], ``ordinals`` [T]) that fall in rows [lo, hi):
+    their flat positions in ``ordinals`` (ascending), the share as CSR offsets [B + 1] and block-local ordinals.
+    Negative ordinals wrap with the global row count; a repeated ordinal is one entry per occurrence."""
+    rows = np.where(ordinals < 0, ordinals + n_rows, ordinals)
+    inside = (rows >= lo) & (rows < hi)
+    pos = np.flatnonzero(inside).astype(np.int64)
+    before = np.concatenate([[0], np.cumsum(inside, dtype=np.int64)])
+    return pos, before[offsets], rows[pos] - lo
+
+
 def block_mask(allowed, n_rows: int, lo: int, hi: int, n_queries: int | None = None) -> np.ndarray:
     """Rows [lo, hi) of a row mask over n_rows rows (bool [n_rows], or packed uint32 words as
     ``VectorBase.pack_row_mask`` makes them), packed again from bit 0: a block need not start on a word.
@@ -469,15 +534,16 @@ def block_mask(allowed, n_rows: int, lo: int, hi: int, n_queries: int | None = N
 
 def as_topk_arrays(offsets, hits, hit_scores, b: int, k: int):
     """CSR threshold-search results laid out as [B, k] top-k arrays (-1 / 0 padding), as ``tav_search`` lays
-    out a search it routes to the threshold engine."""
-    counts = np.diff(offsets).astype(np.int32)
+    out a search it routes to the threshold engine: the first k hits of each query."""
+    per = np.diff(offsets)
     items = np.full((b, k), -1, np.int64)
     scores = np.zeros((b, k), np.float32)
-    cols = np.arange(len(hits)) - np.repeat(offsets[:-1], counts)
-    rows = np.repeat(np.arange(b), counts)
-    items[rows, cols] = hits
-    scores[rows, cols] = hit_scores
-    return items, scores, counts
+    cols = np.arange(len(hits)) - np.repeat(offsets[:-1], per)
+    rows = np.repeat(np.arange(b), per)
+    keep = cols < k
+    items[rows[keep], cols[keep]] = hits[keep]
+    scores[rows[keep], cols[keep]] = hit_scores[keep]
+    return items, scores, np.minimum(per, k).astype(np.int32)
 
 
 class LocalRange:
@@ -687,12 +753,14 @@ class ShardedVectorBase:
         return total
 
     def search_arrays(self, queries: np.ndarray, k: int, min_score: float = 0.0, subset=None, allowed=None,
-                      ties_low_first: bool = False):
+                      ties_low_first: bool = False, subsets=None):
         """SPMD batched lookup, replicated on every rank: items int64 [B, k], scores float32 [B, k], counts int32
-        [B].  ``subset``, ``allowed`` and ``ties_low_first`` as ``VectorBase.search_arrays`` takes them over the
-        whole corpus (global ordinals; ``allowed`` a bool [N] mask or its packed words, or one mask per query: bool
-        [B, N] or packed words [B, ceil(N / 32)]), with its results and
+        [B].  ``subset``, ``subsets``, ``allowed`` and ``ties_low_first`` as ``VectorBase.search_arrays`` takes
+        them over the whole corpus (global ordinals; ``allowed`` a bool [N] mask or its packed words, or one mask
+        per query: bool [B, N] or packed words [B, ceil(N / 32)]), with its results and
         errors; such lookups exchange over the process group whatever ``exchange`` says."""
+        if subsets is not None:
+            return self._search_arrays_subsets(queries, k, min_score, subsets, subset, allowed, ties_low_first)
         if subset is not None or allowed is not None or ties_low_first:
             return self._search_arrays_filtered(queries, k, min_score, subset, allowed, ties_low_first)
         q = np.ascontiguousarray(queries, dtype=np.float32)
@@ -841,7 +909,51 @@ class ShardedVectorBase:
                 b, k_eff, 1 if ties_low_first else 0)
         return items_t.cpu().numpy(), scores_t.cpu().numpy(), counts_t.cpu().numpy()
 
-    def search_range(self, queries, min_score: float = 0.0, ties_low_first: bool = False, subset=None, allowed=None):
+    def _subsets_checked(self, queries, subsets, subset, allowed):
+        """(queries, offsets, ordinals) of a per-query subsets lookup; every error is raised from replicated
+        arguments, so on every rank alike and before any exchange."""
+        q = self._check_queries(queries)
+        if subset is not None or allowed is not None:
+            raise ValueError("subsets= cannot be combined with subset= or allowed=")
+        offsets, ordinals = VectorBase._subsets_csr(subsets, len(q))
+        return q, offsets, ordinals
+
+    def _search_arrays_subsets(self, queries, k, min_score, subsets, subset, allowed, ties_low_first):
+        """``VectorBase.search_arrays(subsets=)`` over the whole corpus.  Each rank searches its share of every
+        query's subset with flat positions as items, maps them to positions in the caller's ordinals, the ranks'
+        lists are merged by position and decoded through the caller's ordinals."""
+        if k < 1:
+            raise ValueError("k must be >= 1")
+        q, offsets, ordinals = self._subsets_checked(queries, subsets, subset, allowed)
+        b = len(q)
+        longest = int(np.diff(offsets).max()) if b else 0
+        k_eff = max(1, min(k, longest))
+        floor = _as_f32_scalar(min_score)
+        if b == 0 or longest == 0 or len(self) == 0 or np.isnan(floor):
+            return np.full((b, k_eff), -1, np.int64), np.zeros((b, k_eff), np.float32), np.zeros(b, np.int32)
+        check_subset(ordinals, len(self))
+        check_subsets_total(len(ordinals))
+        if k_eff > SUBSETS_MERGE_MAX_K:
+            return as_topk_arrays(*self._search_range_subsets(q, floor, ties_low_first, offsets, ordinals), b, k_eff)
+        lo, hi = self.local_range
+        positions, local_offsets, local_ordinals = subsets_share(offsets, ordinals, len(self), lo, hi)
+        items_t, scores_t, counts_t = self._exchange_topk(
+            lambda: self._engine.search_subsets_packed(q, k_eff, float(floor), local_offsets, local_ordinals, positions,
+                                                       ties_low_first),
+            b, k_eff, 3 if ties_low_first else 2)
+        self._engine.map_items(items_t, ordinals)  # flat positions -> the caller's ordinals, as given
+        return items_t.cpu().numpy(), scores_t.cpu().numpy(), counts_t.cpu().numpy()
+
+    def _search_range_subsets(self, q, floor, ties_low_first, offsets, ordinals):
+        """The threshold search of validated per-query subsets: flat positions merged, then decoded."""
+        lo, hi = self.local_range
+        positions, local_offsets, local_ordinals = subsets_share(offsets, ordinals, len(self), lo, hi)
+        return self._range_exchange(q, floor, ties_low_first, lambda: self._engine.range_local(
+            q, float(floor), lo, bool(ties_low_first), subsets=(local_offsets, local_ordinals), positions=positions),
+            decode=ordinals)
+
+    def search_range(self, queries, min_score: float = 0.0, ties_low_first: bool = False, subset=None, allowed=None,
+                     subsets=None):
         """Threshold search over the whole corpus: EVERY row whose score is >= min_score, per query, as
         ``VectorBase.search_range`` returns it on one GPU — CSR numpy arrays offsets int64 [B + 1], items int64
         [T], scores float32 [T], in the library's order — replicated on every rank.  SPMD.  ``subset`` (global
@@ -855,7 +967,16 @@ class ShardedVectorBase:
         all-reduce that makes a failure to stage them raise on every rank); ``tav_merge_range`` merges them on
         every rank.  A subset search merges positions in the subset and decodes them through the caller's list
         afterwards.  The exchanges go through the process group whatever ``exchange`` says.  At most
-        ``MAX_RANGE_RANKS`` (32) ranks: larger groups get ValueError on every rank before any exchange."""
+        ``MAX_RANGE_RANKS`` (32) ranks: larger groups get ValueError on every rank before any exchange.
+        ``subsets`` (one integer sequence per query) as ``VectorBase.search_range`` takes it."""
+        if subsets is not None:
+            q, offsets, ordinals = self._subsets_checked(queries, subsets, subset, allowed)
+            floor = _as_f32_scalar(min_score)
+            if len(q) == 0 or len(ordinals) == 0 or len(self) == 0 or np.isnan(floor):
+                return np.zeros(len(q) + 1, np.int64), np.empty(0, np.int64), np.empty(0, np.float32)
+            check_subset(ordinals, len(self))
+            check_subsets_total(len(ordinals))
+            return self._search_range_subsets(q, floor, ties_low_first, offsets, ordinals)
         if subset is not None or allowed is not None:
             q = self._check_queries(queries)
             sub = None if subset is None else subset_ordinals(subset)
@@ -978,6 +1099,26 @@ class ShardedVectorBase:
                     for b in range(len(ol) - 1)]
         k = VectorBase._resolve_k(max_hits, len(self))
         items, scores, counts = self.search_arrays(embeddings, k, min_score)
+        il, sl, cl = items.tolist(), scores.tolist(), counts.tolist()
+        return [[ScoredInt(i, s) for i, s in zip(il[b][:c], sl[b][:c])] for b, c in enumerate(cl)]
+
+    def fuzzy_lookup_embeddings_in_subsets(self, embeddings, ordinals_of_subsets, max_hits=None, min_score=None):
+        """``VectorBase.fuzzy_lookup_embeddings_in_subsets`` over the whole corpus, SPMD: element b equals
+        ``fuzzy_lookup_embedding_in_subset(embeddings[b], ordinals_of_subsets[b], max_hits, min_score)``."""
+        if min_score is None:
+            min_score = 0.0
+        q = np.asarray(embeddings, dtype=np.float32)
+        if q.ndim != 2:
+            raise ValueError(f"Expected 2D embeddings array, got {q.ndim}D")
+        if max_hits is not None and max_hits < 0:
+            raise ValueError("max_hits must be >= 0")
+        if max_hits == 0:
+            offsets, items, scores = self.search_range(q, min_score, subsets=ordinals_of_subsets)
+            il, sl, ol = items.tolist(), scores.tolist(), offsets.tolist()
+            return [[ScoredInt(i, s) for i, s in zip(il[ol[b]:ol[b + 1]], sl[ol[b]:ol[b + 1]])]
+                    for b in range(len(q))]
+        k = _DEFAULT_MAX_HITS if max_hits is None else max_hits
+        items, scores, counts = self.search_arrays(q, k, min_score, subsets=ordinals_of_subsets)
         il, sl, cl = items.tolist(), scores.tolist(), counts.tolist()
         return [[ScoredInt(i, s) for i, s in zip(il[b][:c], sl[b][:c])] for b, c in enumerate(cl)]
 

@@ -17,6 +17,9 @@ Additions (not in the reference; all opt-in):
     one read of the rows; ``fuzzy_lookup_embeddings(max_hits=0)`` builds its lists from it;
   * ``search_arrays(..., allowed=mask)`` — predicate / post-filter pushdown as a row bitmask
     evaluated inside the kernels (vectorbase.py:191-201, storage/sqlite/messageindex.py:296-326);
+  * ``search_arrays`` / ``search_range(..., subsets=)`` and ``fuzzy_lookup_embeddings_in_subsets`` — one
+    batched lookup in which every query scores only its own candidate ordinals (the batched form of
+    ``fuzzy_lookup_embedding_in_subset``, vectorbase.py:203-230: candidate re-ranking);
   * constructor keywords ``device``, ``storage_dtype``, ``normalize``;
   * ``from_device_tensor`` / ``search_device`` — torch tensors as device-memory handles.
 
@@ -554,6 +557,7 @@ class VectorBase:
         ties_low_first: bool = False,
         _mask_key=None,
         _mask_owner=None,
+        subsets: Sequence[Sequence[int] | np.ndarray] | None = None,
     ) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
         """Batched lookup returning arrays: items int64 [B, k], scores float32 [B, k],
         counts int32 [B] (entries beyond counts[b] are padding: item -1, score 0).  `k` is
@@ -561,14 +565,22 @@ class VectorBase:
         C-contiguous result arrays of exactly those shapes and dtypes.  ``allowed`` (bool [N] or
         bit-packed uint32) restricts the lookup to rows whose bit is set, inside the kernels; a 2-D ``allowed``
         (bool [B, N] or bit-packed uint32 [B, ceil(N / 32)]) gives every query its own mask, in one batched
-        search; ``ties_low_first`` orders exactly equal scores by ascending ordinal (row-scan path)."""
+        search; ``ties_low_first`` orders exactly equal scores by ascending ordinal (row-scan path).
+        ``subsets`` (B one-dimensional integer sequences) gives every query its own subset, in one batched
+        search: row b equals the one-query search with ``subset=subsets[b]``; `k` is clamped to the longest."""
         q = self._check_queries(queries)
         b = len(q)
         if k < 1:
             raise ValueError("k must be >= 1")
         n_rows = len(self)
         sub = None
-        if subset is not None:
+        csr = None
+        if subsets is not None:
+            if subset is not None or allowed is not None:
+                raise ValueError("subsets= cannot be combined with subset= or allowed=")
+            csr = self._subsets_csr(subsets, b)
+            n_rows = int(np.diff(csr[0]).max()) if b else 0
+        elif subset is not None:
             sub = np.ascontiguousarray(subset)
             if sub.size and not np.issubdtype(sub.dtype, np.integer):
                 raise IndexError("arrays used as indices must be of integer (or boolean) type")
@@ -591,6 +603,19 @@ class VectorBase:
         if b == 0 or n_rows == 0 or len(self) == 0 or np.isnan(floor):
             return items, scores, counts
         lib, ix = self._ensure_device()
+        if csr is not None:
+            offsets, ordinals = csr
+            # the hits pass through the index's threshold-search buffers
+            with self._single_lock:
+                _capi.check(
+                    lib.tav_search_subsets(
+                        ix, q.ctypes.data_as(C.c_void_p), b, k_eff, C.c_float(float(floor)),
+                        _capi.TAV_TIES_LOW_FIRST if ties_low_first else 0, offsets.ctypes.data_as(C.c_void_p),
+                        ordinals.ctypes.data_as(C.c_void_p), items.ctypes.data_as(C.c_void_p),
+                        scores.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), None,
+                    )
+                )
+            return items, scores, counts
         flags = self._flags()
         if allowed is not None:
             if sub is not None:
@@ -622,17 +647,36 @@ class VectorBase:
         subset: Sequence[int] | np.ndarray | None = None,
         allowed: np.ndarray | None = None,
         ties_low_first: bool = False,
+        subsets: Sequence[Sequence[int] | np.ndarray] | None = None,
     ) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
         """Threshold (range) search: EVERY row whose score is >= min_score, per query, in one read of
         the rows.  Returns CSR arrays: offsets int64 [B + 1], items int64 [T], scores float32 [T];
         query b's hits are items[offsets[b]:offsets[b + 1]], in the library's order (score descending,
-        equal scores higher ordinal first, or lower first with ``ties_low_first``).  ``subset`` and
+        equal scores higher ordinal first, or lower first with ``ties_low_first``).  ``subset``, ``subsets`` and
         ``allowed`` (1-D, or 2-D: one mask per query) as in ``search_arrays``.  Batches run on the tensor cores (16-bit storage, or float32
         through its fp16 planes), like ``search_arrays``.  The previous call's total sizes the device buffers."""
         q = self._check_queries(queries)
         b = len(q)
         n_rows = len(self)
         sub = None
+        if subsets is not None:
+            if subset is not None or allowed is not None:
+                raise ValueError("subsets= cannot be combined with subset= or allowed=")
+            offsets_in, ordinals = self._subsets_csr(subsets, b)
+            offsets = np.zeros(b + 1, dtype=np.int64)
+            floor = _as_f32_scalar(min_score)
+            if b == 0 or len(ordinals) == 0 or len(self) == 0 or np.isnan(floor):
+                return offsets, np.empty(0, np.int64), np.empty(0, np.float32)
+            with self._single_lock:
+                lib, ix = self._ensure_device()
+                _capi.check(
+                    lib.tav_range_search_subsets(
+                        ix, q.ctypes.data_as(C.c_void_p), b, C.c_float(float(floor)),
+                        _capi.TAV_TIES_LOW_FIRST if ties_low_first else 0, offsets_in.ctypes.data_as(C.c_void_p),
+                        ordinals.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), None,
+                    )
+                )
+                return offsets, *self._range_fetch(lib, ix, int(offsets[-1]))
         if subset is not None:
             sub = np.ascontiguousarray(subset)
             if sub.size and not np.issubdtype(sub.dtype, np.integer):
@@ -671,13 +715,36 @@ class VectorBase:
             )
         )
         total = int(offsets[-1])
+        items, scores = self._range_fetch(lib, ix, total)
+        self._range_hint = total
+        return offsets, items, scores
+
+    @staticmethod
+    def _range_fetch(lib, ix, total: int) -> tuple[np.ndarray, np.ndarray]:
+        """The `total` hits of the index's last threshold search (the caller holds ``_single_lock``)."""
         items = np.empty(total, dtype=np.int64)
         scores = np.empty(total, dtype=np.float32)
         if total:
             _capi.check(lib.tav_range_fetch(ix, 0, total, items.ctypes.data_as(C.c_void_p),
                                             scores.ctypes.data_as(C.c_void_p), 0, None))
-        self._range_hint = total
-        return offsets, items, scores
+        return items, scores
+
+    @staticmethod
+    def _subsets_csr(subsets, n_queries: int) -> tuple[np.ndarray, np.ndarray]:
+        """B one-dimensional integer sequences -> (offsets int64 [B + 1], ordinals int64 [T]), the layout of
+        ``tav_search_subsets``; ValueError when their count is not B, IndexError for a non-integer ordinal."""
+        if len(subsets) != n_queries:
+            raise ValueError(f"{len(subsets)} subsets for {n_queries} queries")
+        parts = []
+        for s in subsets:
+            a = np.asarray(s)
+            if a.size and not np.issubdtype(a.dtype, np.integer):
+                raise IndexError("arrays used as indices must be of integer (or boolean) type")
+            parts.append(a.astype(np.int64, copy=False).reshape(-1))
+        offsets = np.zeros(n_queries + 1, dtype=np.int64)
+        np.cumsum([len(p) for p in parts], out=offsets[1:])
+        ordinals = np.concatenate(parts) if parts else np.empty(0, np.int64)
+        return offsets, np.ascontiguousarray(ordinals, dtype=np.int64)
 
     def enable_timing(self, enabled: bool = True, main_only: bool = False) -> None:
         """Record CUDA events around the kernels of subsequent lookups (see ``last_timing``);
@@ -891,6 +958,33 @@ class VectorBase:
                     for b in range(len(q))]
         items, scores, counts = self.search_arrays(q, k, min_score)
         # three bulk conversions, then plain list slices: 1.6x faster than slicing the arrays per query
+        il, sl, cl = items.tolist(), scores.tolist(), counts.tolist()
+        return [[ScoredInt(i, s) for i, s in zip(il[b][:c], sl[b][:c])] for b, c in enumerate(cl)]
+
+    def fuzzy_lookup_embeddings_in_subsets(
+        self,
+        embeddings: np.ndarray,
+        ordinals_of_subsets: Sequence[Sequence[int]],
+        max_hits: int | None = None,
+        min_score: float | None = None,
+    ) -> list[list[ScoredInt]]:
+        """One batched GPU search in which query b scores only ``ordinals_of_subsets[b]``; element b equals
+        ``fuzzy_lookup_embedding_in_subset(embeddings[b], ordinals_of_subsets[b], max_hits, min_score)``."""
+        if min_score is None:
+            min_score = 0.0
+        q = np.asarray(embeddings, dtype=np.float32)
+        if q.ndim != 2:
+            raise ValueError(f"Expected 2D embeddings array, got {q.ndim}D")
+        if max_hits is not None and max_hits < 0:
+            raise ValueError("max_hits must be >= 0")
+        if max_hits == 0:
+            # every passing entry: CSR lists from the threshold form instead of [B, longest] arrays
+            offsets, items, scores = self.search_range(q, min_score, subsets=ordinals_of_subsets)
+            il, sl, ol = items.tolist(), scores.tolist(), offsets.tolist()
+            return [[ScoredInt(i, s) for i, s in zip(il[ol[b]:ol[b + 1]], sl[ol[b]:ol[b + 1]])]
+                    for b in range(len(q))]
+        k = _DEFAULT_MAX_HITS if max_hits is None else max_hits
+        items, scores, counts = self.search_arrays(q, k, min_score, subsets=ordinals_of_subsets)
         il, sl, cl = items.tolist(), scores.tolist(), counts.tolist()
         return [[ScoredInt(i, s) for i, s in zip(il[b][:c], sl[b][:c])] for b, c in enumerate(cl)]
 
