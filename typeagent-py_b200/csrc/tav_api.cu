@@ -45,47 +45,44 @@ static inline bool dtype_ok(int dt) { return dt == TAV_F32 || dt == TAV_BF16 || 
         }                                                                                  \
     } while (0)
 
-// a grow-only device buffer
-struct DevBuf {
+// a grow-only buffer from one alloc / free pair; it owns its memory: freed when it is destroyed, moved, never copied
+template <cudaError_t (*Alloc)(void**, size_t), cudaError_t (*Free)(void*)>
+struct GrowBuf {
     void* p = nullptr;
     size_t bytes = 0;
+    GrowBuf() = default;
+    GrowBuf(GrowBuf&& o) noexcept : p(o.p), bytes(o.bytes) {
+        o.p = nullptr;
+        o.bytes = 0;
+    }
+    GrowBuf& operator=(GrowBuf&& o) noexcept {
+        if (this != &o) {
+            release();
+            p = o.p;
+            bytes = o.bytes;
+            o.p = nullptr;
+            o.bytes = 0;
+        }
+        return *this;
+    }
+    ~GrowBuf() { release(); }
     cudaError_t ensure(size_t need) {
         if (need <= bytes) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        bytes = 0;
+        release();
         size_t want = std::max(need, size_t(1) << 16);
-        cudaError_t e = cudaMalloc(&p, want);
+        cudaError_t e = Alloc(&p, want);
         if (e == cudaSuccess) bytes = want;
         return e;
     }
     void release() {
-        if (p) cudaFree(p);
+        if (p) Free(p);
         p = nullptr;
         bytes = 0;
     }
 };
-
-// a grow-only pinned host buffer (staging for truly asynchronous H2D / D2H of small payloads)
-struct PinBuf {
-    void* p = nullptr;
-    size_t bytes = 0;
-    cudaError_t ensure(size_t need) {
-        if (need <= bytes) return cudaSuccess;
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        bytes = 0;
-        size_t want = std::max(need, size_t(1) << 16);
-        cudaError_t e = cudaMallocHost(&p, want);
-        if (e == cudaSuccess) bytes = want;
-        return e;
-    }
-    void release() {
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        bytes = 0;
-    }
-};
+using DevBuf = GrowBuf<cudaMalloc, cudaFree>;
+// pinned host memory: staging for truly asynchronous H2D / D2H of small payloads
+using PinBuf = GrowBuf<cudaMallocHost, cudaFreeHost>;
 
 constexpr int kMaxTimedKernels = 12;   // event pairs per search (more kernels than that go untimed)
 constexpr int kHistory = 64;           // timed searches remembered (tav_timing_history)
@@ -104,7 +101,7 @@ constexpr uint32_t kNoScoreYet = 0xFFFFFFFFu;    // ... or this score (a NaN pat
 // CUDA events around one search (created lazily, when timing is first enabled)
 struct TimedSearch {
     cudaEvent_t total[2] = {nullptr, nullptr};
-    cudaEvent_t ev[kMaxTimedKernels][2];
+    cudaEvent_t ev[kMaxTimedKernels][2] = {};
     int kind[kMaxTimedKernels];  // 0 dominant kernel, 1 sample pass, 2 auxiliary
     int used = 0;
     int launches = 0;
@@ -258,6 +255,12 @@ static int mark_queued(tav_index* ix, cudaStream_t s) {
     return TAV_OK;
 }
 
+// entry of the calls that name a stream: the index's device, and s ordered after the earlier calls' work
+static int enter_stream(tav_index* ix, cudaStream_t s) {
+    if (int rc = set_device(ix)) return rc;
+    return join_stream(ix, s);
+}
+
 static void mark_done(tav_index* ix) { ix->outstanding = false; }
 
 // the entry points without a stream (clear, adopt, reserve): the host waits for the earlier calls' work
@@ -268,6 +271,21 @@ static int wait_queued(tav_index* ix) {
 }
 
 static int finish_pending(tav_index* ix, cudaStream_t s, int* redone);
+
+// bitmask words of n_rows rows padded to whole 256-row tiles (the tensor-core epilogue reads one word per 32 rows
+// of a tile)
+static inline int64_t mask_words(int64_t n_rows) { return (n_rows + 255) / 256 * 8; }
+
+// numpy's IndexError for ordinals outside [-size, size)
+static int check_subset_ordinals(const tav_index* ix, const int64_t* ordinals, int64_t n) {
+    for (int64_t i = 0; i < n; ++i)
+        if (ordinals[i] < -ix->size || ordinals[i] >= ix->size) {
+            set_error("index %lld is out of bounds for axis 0 with size %lld", (long long)ordinals[i],
+                      (long long)ix->size);
+            return TAV_ERR_RANGE;
+        }
+    return TAV_OK;
+}
 
 static void destroy_history(tav_index* ix) {
     if (!ix->hist) return;
@@ -398,24 +416,12 @@ int tav_destroy(tav_index* ix) {
     cudaSetDevice(ix->device);
     cudaDeviceSynchronize();  // searches may still be in flight on the caller's streams
     if (ix->rows && !ix->adopted) cudaFree(ix->rows);
-    for (DevBuf* b : {&ix->queries, &ix->held_queries, &ix->subset, &ix->cand_keys, &ix->cand_count, &ix->out_pack, &ix->staging,
-                      &ix->mma_ws, &ix->retry, &ix->split_hi, &ix->split_lo, &ix->split_flag, &ix->row_mask,
-                      &ix->qmask, &ix->qmask_pop, &ix->range_qmap,
-                      &ix->range_keys, &ix->range_keys2, &ix->range_counts, &ix->range_qgather, &ix->range_tmp,
-                      &ix->range_sortws, &ix->range_items, &ix->range_scores, &ix->range_mmaws,
-                      &ix->range_mmaws2, &ix->range_mmaaux, &ix->compact_keys, &ix->subsets_meta})
-        b->release();
-    for (DevBuf& b : ix->held_retired) b.release();
     if (ix->ev_last) cudaEventDestroy(ix->ev_last);
-    ix->pin_in.release();
-    ix->pin_out.release();
-    ix->retry_host.release();
-    for (auto& b : ix->pin_append) b.release();
     if (ix->ev_pin_in) cudaEventDestroy(ix->ev_pin_in);
     for (auto& ev : ix->ev_append)
         if (ev) cudaEventDestroy(ev);
     destroy_history(ix);
-    delete ix;
+    delete ix;  // (its buffers free themselves)
     return TAV_OK;
 }
 
@@ -499,9 +505,8 @@ int tav_append(tav_index* ix, const void* rows, int64_t n, int dim, int src_dtyp
         return TAV_ERR_INVALID;
     }
     if (n == 0) return TAV_OK;
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;
+    if (int rc = enter_stream(ix, s)) return rc;
     if (ix->size + n > ix->capacity) {
         int64_t want = std::max<int64_t>(ix->size + n, ix->capacity * 2);
         want = std::max<int64_t>(want, 1024);
@@ -560,9 +565,8 @@ int tav_read_rows(tav_index* ix, int64_t first, int64_t n, float* out_host, void
         return TAV_ERR_RANGE;
     }
     if (n == 0) return TAV_OK;
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;
+    if (int rc = enter_stream(ix, s)) return rc;
     const size_t row = static_cast<size_t>(ix->dim) * dtype_size(ix->dtype);
     const char* src = static_cast<const char*>(ix->rows) + static_cast<size_t>(first) * row;
     if (ix->dtype == TAV_F32) {
@@ -581,13 +585,10 @@ int tav_read_rows(tav_index* ix, int64_t first, int64_t n, float* out_host, void
 int tav_set_row_mask(tav_index* ix, const uint32_t* bits, int64_t n_rows, int on_device, void* stream) {
     if (!ix || n_rows < 0 || (n_rows > 0 && !bits)) return TAV_ERR_INVALID;
     std::lock_guard<std::mutex> lock(ix->mu);
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;  // queued searches read the old mask
-    if (!ix->pending.empty()) {  // an outstanding search may still need the old mask for its exact redo
-        int redone = 0;
-        if (int rc = finish_pending(ix, s, &redone)) return rc;
-    }
+    if (int rc = enter_stream(ix, s)) return rc;  // queued searches read the old mask
+    // an outstanding search may still need the old mask for its exact redo
+    if (int rc = finish_pending(ix, s, nullptr)) return rc;
     if (n_rows == 0) {
         ix->row_mask_rows = 0;
         return TAV_OK;
@@ -596,8 +597,7 @@ int tav_set_row_mask(tav_index* ix, const uint32_t* bits, int64_t n_rows, int on
         set_error("tav_set_row_mask: %lld bits for an index of %lld rows", (long long)n_rows, (long long)ix->size);
         return TAV_ERR_INVALID;
     }
-    // padded to whole 256-row tiles (the tensor-core epilogue reads one word per 32 rows of a tile)
-    const size_t words = static_cast<size_t>((n_rows + 255) / 256) * 8;
+    const size_t words = static_cast<size_t>(mask_words(n_rows));
     const size_t src_words = static_cast<size_t>((n_rows + 31) / 32);
     TAV_CUDA(ix->row_mask.ensure(words * sizeof(uint32_t)));
     TAV_CUDA(cudaMemsetAsync(ix->row_mask.p, 0, words * sizeof(uint32_t), s));
@@ -614,13 +614,10 @@ int tav_set_query_masks(tav_index* ix, const uint32_t* bits, int n_queries, int6
                         int on_device, void* stream) {
     if (!ix || n_queries < 0 || n_rows < 0 || (n_queries > 0 && !bits)) return TAV_ERR_INVALID;
     std::lock_guard<std::mutex> lock(ix->mu);
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;  // queued searches read the old masks
-    if (!ix->pending.empty()) {  // an outstanding search may still need the old masks for its exact redo
-        int redone = 0;
-        if (int rc = finish_pending(ix, s, &redone)) return rc;
-    }
+    if (int rc = enter_stream(ix, s)) return rc;  // queued searches read the old masks
+    // an outstanding search may still need the old masks for its exact redo
+    if (int rc = finish_pending(ix, s, nullptr)) return rc;
     if (n_queries == 0) {
         ix->qmask_n = 0;
         return TAV_OK;
@@ -636,8 +633,7 @@ int tav_set_query_masks(tav_index* ix, const uint32_t* bits, int n_queries, int6
                   (long long)src_words);
         return TAV_ERR_INVALID;
     }
-    // each mask padded to whole 256-row tiles, as the row mask (the tensor-core epilogue reads one word per 32 rows)
-    const int64_t words = (n_rows + 255) / 256 * 8;
+    const int64_t words = mask_words(n_rows);
     const size_t bytes = static_cast<size_t>(n_queries) * words * sizeof(uint32_t);
     ix->qmask_n = 0;
     cudaError_t e = ix->qmask.ensure(bytes);
@@ -674,6 +670,133 @@ static inline cudaError_t ev_record(cudaEvent_t& ev, cudaStream_t s) {
         if (e != cudaSuccess) return e;
     }
     return cudaEventRecord(ev, s);
+}
+
+// the timing record of a search that starts now: the next history entry when timing is on, else ix->untimed
+static TimedSearch* begin_search(tav_index* ix, int path) {
+    ix->last_first_slot = -1;
+    ix->last_n_slots = 0;
+    TimedSearch* ts = cur_timed(ix);
+    if (!ts) ts = &ix->untimed;
+    ts->used = 0;
+    ts->launches = 0;
+    ts->path = path;
+    ts->valid = false;
+    return ts;
+}
+
+// the search's work is queued: its closing event, and the record counts
+static int end_search(tav_index* ix, TimedSearch* ts, cudaStream_t s) {
+    if (ts != &ix->untimed) {
+        TAV_CUDA(ev_record(ts->total[1], s));
+        ++ix->search_seq;
+    }
+    ts->valid = true;
+    return TAV_OK;
+}
+
+// One kernel launch of a search, with an event pair of `kind` around it when the search is timed and a pair is
+// free; light timing (tav_set_timing(2)) times only the dominant kernels (kind 0).  ts may be nullptr.
+template <class Launch>
+static cudaError_t timed_launch(const tav_index* ix, TimedSearch* ts, bool timing, int kind, cudaStream_t s,
+                                Launch&& launch) {
+    const bool timed = timing && ts && ts->used < kMaxTimedKernels && (kind == 0 || !ix->timing_light);
+    cudaError_t e;
+    if (timed && (e = ev_record(ts->ev[ts->used][0], s)) != cudaSuccess) return e;
+    if ((e = launch()) != cudaSuccess || !timed) return e;
+    ts->kind[ts->used] = kind;
+    return ev_record(ts->ev[ts->used++][1], s);
+}
+
+// the tensor-core launchers record into existing events: every pair of a timed search is created first
+static int create_events(TimedSearch* ts) {
+    for (auto& pr : ts->ev)
+        for (auto& ev : pr)
+            if (!ev) TAV_CUDA(cudaEventCreate(&ev));
+    return TAV_OK;
+}
+
+// the corpus fields of a row-scan launch
+static ScanArgs scan_args(const tav_index* ix) {
+    ScanArgs a{};
+    a.corpus = ix->rows;
+    a.dtype = ix->dtype;
+    a.n_corpus = ix->size;
+    a.dim = ix->dim;
+    return a;
+}
+
+// the corpus fields of a tensor-core launch: the rows, or (split) the float32 index's two fp16 planes
+static MmaArgs mma_args(const tav_index* ix, bool split) {
+    MmaArgs m{};
+    m.device = ix->device;
+    m.corpus = split ? ix->split_hi.p : ix->rows;
+    m.corpus_lo = split ? ix->split_lo.p : nullptr;
+    m.split = split ? 1 : 0;
+    m.dtype = ix->dtype;
+    m.n_corpus = ix->size;
+    m.dim = ix->dim;
+    return m;
+}
+
+// the tensor-core search workspace, at least `bytes`: earlier searches may still use the old one, and the
+// sampler's unit counters (its first 64 KB) must read zero
+static int ensure_mma_ws(tav_index* ix, size_t bytes, cudaStream_t s) {
+    if (bytes <= ix->mma_ws.bytes) return TAV_OK;
+    TAV_CUDA(cudaStreamSynchronize(s));
+    TAV_CUDA(ix->mma_ws.ensure(bytes));
+    TAV_CUDA(cudaMemsetAsync(ix->mma_ws.p, 0, std::min<size_t>(ix->mma_ws.bytes, 65536), s));
+    return TAV_OK;
+}
+
+// Host outputs of a top-k search of n_queries x k, packed [items | scores | counts | done word] in one buffer
+// so that a single D2H copy (into pinned staging) brings them back.
+struct ResultPack {
+    size_t nk, n;  // hits, counts
+    size_t off_scores, off_counts, off_done;
+    ResultPack(int n_queries, int k)
+        : nk(static_cast<size_t>(n_queries) * k), n(static_cast<size_t>(n_queries)), off_scores(nk * sizeof(int64_t)),
+          off_counts(off_scores + ((nk * sizeof(float) + 7) & ~size_t(7))),
+          off_done(off_counts + ((n * sizeof(int32_t) + 7) & ~size_t(7))) {}
+    size_t bytes() const { return off_done + 8; }
+    size_t counts_end() const { return off_counts + n * sizeof(int32_t); }  // the pack without the done word
+    // the three arrays in a pack at `base`
+    void place(void* base, int64_t** items, float** scores, int32_t** counts) const {
+        char* b = static_cast<char*>(base);
+        *items = reinterpret_cast<int64_t*>(b);
+        *scores = reinterpret_cast<float*>(b + off_scores);
+        *counts = reinterpret_cast<int32_t*>(b + off_counts);
+    }
+    // a pack in host memory -> the caller's arrays
+    void unpack(const void* h, int64_t* items, float* scores, int32_t* counts) const {
+        const char* b = static_cast<const char*>(h);
+        memcpy(items, b, nk * sizeof(int64_t));
+        memcpy(scores, b + off_scores, nk * sizeof(float));
+        memcpy(counts, b + off_counts, n * sizeof(int32_t));
+    }
+};
+
+// a pack in device memory -> the caller's host arrays, each array copied on its own; synchronises s
+static int copy_pack_out(const ResultPack& p, const void* d, int64_t* items, float* scores, int32_t* counts,
+                         cudaStream_t s) {
+    const char* b = static_cast<const char*>(d);
+    TAV_CUDA(cudaMemcpyAsync(items, b, p.nk * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaMemcpyAsync(scores, b + p.off_scores, p.nk * sizeof(float), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaMemcpyAsync(counts, b + p.off_counts, p.n * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaStreamSynchronize(s));
+    return TAV_OK;
+}
+
+// CSR offsets of a threshold search -> the caller (host or device); the sort after the last synchronisation
+// may still run
+static int deliver_offsets(tav_index* ix, const std::vector<int64_t>& offsets, int64_t* out, bool o_dev, cudaStream_t s) {
+    const size_t bytes = offsets.size() * sizeof(int64_t);
+    if (o_dev) {  // from pageable memory: consumed when the call returns
+        TAV_CUDA(cudaMemcpyAsync(out, offsets.data(), bytes, cudaMemcpyHostToDevice, s));
+    } else {
+        memcpy(out, offsets.data(), bytes);
+    }
+    return mark_queued(ix, s);
 }
 
 // workspace of the row-scan kernels: [8] u64 bounds | [8] u32 counters | [1] u32 fused ticket, zeroed once
@@ -718,11 +841,7 @@ static int scan_search(tav_index* ix, TimedSearch* ts, bool timing, const float*
         const int nq = std::min(qb, nq_total - q0);
         for (int pass = 0; pass < n_pass; ++pass) {
             const int kk = std::min(pass_k, k - pass * pass_k);
-            ScanArgs a{};
-            a.corpus = ix->rows;
-            a.dtype = ix->dtype;
-            a.n_corpus = ix->size;
-            a.dim = ix->dim;
+            ScanArgs a = scan_args(ix);
             a.subset = d_subset;
             a.n_scan = n_scan;
             a.queries = d_queries + static_cast<size_t>(q0) * ix->dim;
@@ -747,13 +866,7 @@ static int scan_search(tav_index* ix, TimedSearch* ts, bool timing, const float*
                 a.out_scores = d_scores + static_cast<size_t>(q0) * k;
                 a.out_counts = d_counts + q0;
             }
-            const bool timed = timing && ts && ts->used < kMaxTimedKernels;
-            if (timed) TAV_CUDA(ev_record(ts->ev[ts->used][0], s));
-            TAV_CUDA(launch_scan(a, s));
-            if (timed) {
-                ts->kind[ts->used] = 0;
-                TAV_CUDA(ev_record(ts->ev[ts->used++][1], s));
-            }
+            TAV_CUDA(timed_launch(ix, ts, timing, 0, s, [&] { return launch_scan(a, s); }));
             if (fuse) {
                 if (ts) ts->launches += 1;
                 continue;
@@ -884,40 +997,71 @@ static int finish_pending(tav_index* ix, cudaStream_t s, int* redone) {
     // at the first synchronisation above (s joined the stream of the last call first), their redo scans at the
     // last.  So the regions can be reused and the outgrown buffers freed.
     ix->held_used = 0;
-    for (DevBuf& b : ix->held_retired) b.release();
     ix->held_retired.clear();
     if (redone) *redone = n_redone;
     return TAV_OK;
 }
 
-// TAV_USE_QUERY_MASKS of a search of n_queries: the index's masks in *qm, or the error.  One query takes the
-// row-mask form: its mask goes to *d_mask and *qm stays empty.
-static int use_query_masks(tav_index* ix, const char* fn, int n_queries, int flags, bool has_subset, QueryMasks* qm,
-                           const uint32_t** d_mask) {
-    if (flags & TAV_USE_ROW_MASK) {
-        set_error("%s: TAV_USE_QUERY_MASKS and TAV_USE_ROW_MASK cannot be combined", fn);
+// The subset arguments of tav_search / tav_range_search (`fn`), checked before the index is looked at; a
+// threshold search also refuses TAV_DEFER_RETRY.
+static int check_subset_args(const char* fn, int flags, const int64_t* subset, int64_t subset_len, bool threshold) {
+    if ((subset && subset_len < 0) || (!subset && subset_len != 0)) {
+        set_error("%s: subset / subset_len mismatch", fn);
         return TAV_ERR_INVALID;
     }
-    if (has_subset) {
-        set_error("%s: per-query masks and a subset cannot be combined", fn);
+    if (threshold && (flags & TAV_DEFER_RETRY)) {
+        set_error("%s: TAV_DEFER_RETRY is not available for threshold searches", fn);
         return TAV_ERR_INVALID;
     }
-    if (ix->qmask_n == 0 || ix->qmask_rows != ix->size || ix->size == 0) {
-        set_error("%s: TAV_USE_QUERY_MASKS without current per-query masks (tav_set_query_masks)", fn);
-        return TAV_ERR_STATE;
-    }
-    if (n_queries != ix->qmask_n) {
-        set_error("%s: %d queries for %d per-query masks", fn, n_queries, ix->qmask_n);
+    if ((flags & TAV_ITEMS_AS_POSITIONS) && !subset) {
+        set_error("%s: TAV_ITEMS_AS_POSITIONS needs a subset", fn);
         return TAV_ERR_INVALID;
     }
+    return TAV_OK;
+}
+
+// The filter of a search of n_queries (`fn` names the entry point in the messages), or the error:
+// TAV_USE_ROW_MASK -> the row mask in *d_mask; TAV_USE_QUERY_MASKS -> the index's per-query masks in *qm, except
+// that one query takes the row-mask form (its mask in *d_mask, *qm empty).
+static int resolve_masks(tav_index* ix, const char* fn, int n_queries, int flags, bool has_subset,
+                         const uint32_t** d_mask, QueryMasks* qm) {
+    *d_mask = nullptr;
     *qm = QueryMasks{};
-    if (n_queries == 1) {
-        *d_mask = static_cast<const uint32_t*>(ix->qmask.p);
-        return TAV_OK;
+    if (flags & TAV_USE_QUERY_MASKS) {
+        if (flags & TAV_USE_ROW_MASK) {
+            set_error("%s: TAV_USE_QUERY_MASKS and TAV_USE_ROW_MASK cannot be combined", fn);
+            return TAV_ERR_INVALID;
+        }
+        if (has_subset) {
+            set_error("%s: per-query masks and a subset cannot be combined", fn);
+            return TAV_ERR_INVALID;
+        }
+        if (ix->qmask_n == 0 || ix->qmask_rows != ix->size || ix->size == 0) {
+            set_error("%s: TAV_USE_QUERY_MASKS without current per-query masks (tav_set_query_masks)", fn);
+            return TAV_ERR_STATE;
+        }
+        if (n_queries != ix->qmask_n) {
+            set_error("%s: %d queries for %d per-query masks", fn, n_queries, ix->qmask_n);
+            return TAV_ERR_INVALID;
+        }
+        if (n_queries == 1) {
+            *d_mask = static_cast<const uint32_t*>(ix->qmask.p);
+            return TAV_OK;
+        }
+        qm->bits = static_cast<const uint32_t*>(ix->qmask.p);
+        qm->stride = ix->qmask_stride;
+        qm->pop = static_cast<const uint32_t*>(ix->qmask_pop.p);
+    } else if (flags & TAV_USE_ROW_MASK) {
+        if (ix->row_mask_rows != ix->size || ix->size == 0) {
+            set_error("%s: TAV_USE_ROW_MASK without a current row mask (tav_set_row_mask)", fn);
+            return TAV_ERR_STATE;
+        }
+        if (has_subset) {
+            set_error("%s: a row mask and a subset cannot be combined", fn);
+            return TAV_ERR_INVALID;
+        }
+        *d_mask = static_cast<const uint32_t*>(ix->row_mask.p);
     }
-    qm->bits = static_cast<const uint32_t*>(ix->qmask.p);
-    qm->stride = ix->qmask_stride;
-    qm->pop = static_cast<const uint32_t*>(ix->qmask_pop.p);
     return TAV_OK;
 }
 
@@ -1014,11 +1158,7 @@ static int collect_scans(tav_index* ix, TimedSearch* ts, bool timing, const floa
     }
     const int grid = scan_collect_grid(ix->device, ix->dim, qb, n_scan);
     for (int q0 = 0; q0 < nq; q0 += qb) {
-        ScanArgs a{};
-        a.corpus = ix->rows;
-        a.dtype = ix->dtype;
-        a.n_corpus = ix->size;
-        a.dim = ix->dim;
+        ScanArgs a = scan_args(ix);
         a.subset = d_subset;
         a.n_scan = n_scan;
         a.queries = d_queries + static_cast<size_t>(q0) * ix->dim;
@@ -1031,13 +1171,7 @@ static int collect_scans(tav_index* ix, TimedSearch* ts, bool timing, const floa
         a.row_mask = d_mask;
         if (qm.bits) a.qmask = qmask_from(qm, q0);
         a.ties_low = ties_low;
-        const bool timed = timing && ts->used < kMaxTimedKernels;
-        if (timed) TAV_CUDA(ev_record(ts->ev[ts->used][0], s));
-        TAV_CUDA(launch_scan_collect(a, s));
-        if (timed) {
-            ts->kind[ts->used] = 0;
-            TAV_CUDA(ev_record(ts->ev[ts->used++][1], s));
-        }
+        TAV_CUDA(timed_launch(ix, ts, timing, 0, s, [&] { return launch_scan_collect(a, s); }));
         ts->launches += 1;
     }
     return TAV_OK;
@@ -1112,13 +1246,7 @@ static int range_sort(tav_index* ix, TimedSearch* ts, bool timing, std::vector<S
     sa.ties_low = ties_low;
     sa.out_items = static_cast<int64_t*>(ix->range_items.p);
     sa.out_scores = static_cast<float*>(ix->range_scores.p);
-    const bool timed = timing && !ix->timing_light && ts->used < kMaxTimedKernels;
-    if (timed) TAV_CUDA(ev_record(ts->ev[ts->used][0], s));
-    TAV_CUDA(launch_segmented_sort(sa, s, &ts->launches));
-    if (timed) {
-        ts->kind[ts->used] = 2;
-        TAV_CUDA(ev_record(ts->ev[ts->used++][1], s));
-    }
+    TAV_CUDA(timed_launch(ix, ts, timing, 2, s, [&] { return launch_segmented_sort(sa, s, &ts->launches); }));
     return TAV_OK;
 }
 
@@ -1131,6 +1259,17 @@ static int gather_mask_map(tav_index* ix, const std::vector<int>& over, const Qu
     TAV_CUDA(cudaMemcpyAsync(ix->range_qmap.p, map.data(), map.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     out = qm;
     out.map = TAV_QUERY_MASK_MUTANT == 3 ? nullptr : static_cast<const int32_t*>(ix->range_qmap.p);
+    return TAV_OK;
+}
+
+// the queries `over` of d_queries, contiguous in ix->range_qgather for a re-pass (one copy per query)
+static int gather_repass_queries(tav_index* ix, const float* d_queries, const std::vector<int>& over, cudaStream_t s) {
+    const size_t qrow = static_cast<size_t>(ix->dim) * sizeof(float);
+    if (int rc = range_alloc(ix->range_qgather, over.size() * qrow, "the re-pass queries")) return rc;
+    char* qg = static_cast<char*>(ix->range_qgather.p);
+    for (size_t i = 0; i < over.size(); ++i)
+        TAV_CUDA(cudaMemcpyAsync(qg + i * qrow, reinterpret_cast<const char*>(d_queries) + over[i] * qrow, qrow,
+                                 cudaMemcpyDeviceToDevice, s));
     return TAV_OK;
 }
 
@@ -1168,22 +1307,17 @@ static int range_collect_scan(tav_index* ix, TimedSearch* ts, bool timing, const
     uint64_t* keys2 = nullptr;
     const int no = static_cast<int>(over.size());
     if (no > 0) {
-        const size_t qrow = static_cast<size_t>(ix->dim) * sizeof(float);
         if (int rc = range_alloc(ix->range_keys2, static_cast<size_t>(no) * over_max * sizeof(uint64_t), "the re-pass regions"))
             return rc;
-        if (int rc = range_alloc(ix->range_qgather, no * qrow, "the re-pass queries")) return rc;
+        if (int rc = gather_repass_queries(ix, d_queries, over, s)) return rc;
         keys2 = static_cast<uint64_t*>(ix->range_keys2.p);
-        char* qg = static_cast<char*>(ix->range_qgather.p);
-        for (int i = 0; i < no; ++i)
-            TAV_CUDA(cudaMemcpyAsync(qg + i * qrow, reinterpret_cast<const char*>(d_queries) + over[i] * qrow, qrow,
-                                     cudaMemcpyDeviceToDevice, s));
         TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(no) * sizeof(uint32_t), s));
         QueryMasks qm2{};
         if (qm.bits) {  // each gathered query keeps its own mask
             if (int rc = gather_mask_map(ix, over, qm, qm2, s)) return rc;
         }
-        if (int rc = collect_scans(ix, ts, timing, reinterpret_cast<const float*>(qg), no, floor, d_subset, n_scan,
-                                   d_mask, ties_low, keys2, over_max, d_counts, s, qm2))
+        if (int rc = collect_scans(ix, ts, timing, static_cast<const float*>(ix->range_qgather.p), no, floor, d_subset,
+                                   n_scan, d_mask, ties_low, keys2, over_max, d_counts, s, qm2))
             return rc;
     }
     std::vector<SortSeg> segs(static_cast<size_t>(nq));
@@ -1225,19 +1359,10 @@ static int range_collect_mma(tav_index* ix, TimedSearch* ts, bool timing, const 
     if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(nq) * 2 * sizeof(uint32_t), "the hit counters")) return rc;
     uint32_t* d_tot = static_cast<uint32_t*>(ix->range_counts.p);
     uint32_t* d_max = d_tot + nq;
-    if (timing)  // the launcher records into existing events
-        for (int i = 0; i < kMaxTimedKernels; ++i)
-            for (int j = 0; j < 2; ++j)
-                if (!ts->ev[i][j]) TAV_CUDA(cudaEventCreate(&ts->ev[i][j]));
-    MmaArgs m{};
-    m.device = ix->device;
-    m.corpus = split ? ix->split_hi.p : ix->rows;
-    m.corpus_lo = split ? ix->split_lo.p : nullptr;
-    m.split = split ? 1 : 0;
+    if (timing)
+        if (int rc = create_events(ts)) return rc;
+    MmaArgs m = mma_args(ix, split);
     m.split_overflow = split ? d_qflag : nullptr;
-    m.dtype = ix->dtype;
-    m.n_corpus = ix->size;
-    m.dim = ix->dim;
     m.queries = d_queries;
     m.nq = nq;
     m.floor_score = floor;
@@ -1292,14 +1417,9 @@ static int range_collect_mma(tav_index* ix, TimedSearch* ts, bool timing, const 
     if (no > 0) {
         // the overflowed queries, gathered, through the same units per chunk: every segment receives the
         // rows it received before, and the counts just read size it exactly
-        const size_t qrow = static_cast<size_t>(ix->dim) * sizeof(float);
-        if (int rc = range_alloc(ix->range_qgather, no * qrow, "the re-pass queries")) return rc;
-        char* qg = static_cast<char*>(ix->range_qgather.p);
-        for (int i = 0; i < no; ++i)
-            TAV_CUDA(cudaMemcpyAsync(qg + i * qrow, reinterpret_cast<const char*>(d_queries) + over[i] * qrow, qrow,
-                                     cudaMemcpyDeviceToDevice, s));
+        if (int rc = gather_repass_queries(ix, d_queries, over, s)) return rc;
         MmaArgs m2 = m;
-        m2.queries = reinterpret_cast<const float*>(qg);
+        m2.queries = static_cast<const float*>(ix->range_qgather.p);
         m2.nq = no;
         if (qm.bits) {  // each gathered query keeps its own mask
             if (int rc = gather_mask_map(ix, over, qm, m2.qmask, s)) return rc;
@@ -1353,14 +1473,6 @@ static int range_core(tav_index* ix, TimedSearch* ts, bool timing, const float* 
 
 // ---- removal and overwrite (tav_remove_rows, tav_write_rows) -----------------------------------------------
 constexpr size_t kCompactScratchBytes = size_t(256) << 20;  // window buffer of the in-place compaction
-
-// Entry of the calls that change rows in place, after join_stream: the outstanding deferred searches are
-// finished first, because their exact redo reads the rows.
-static int finish_before_row_change(tav_index* ix, cudaStream_t s) {
-    if (ix->pending.empty()) return TAV_OK;
-    int redone = 0;
-    return finish_pending(ix, s, &redone);
-}
 
 // Compacts the rows after the removal of `rem` (sorted, distinct, not empty) on s and synchronises s.  Rows
 // [0, rem[0]) are not written.  Out of place (tav_internal_compact_policy mode 1) — a fresh allocation of the
@@ -1434,7 +1546,6 @@ static int compact_rows(tav_index* ix, const std::vector<int64_t>& rem, cudaStre
                                     d1 - d0, row, s);
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    scratch.release();
     if (e != cudaSuccess) {
         set_error("tav_remove_rows: compaction failed: %s", cudaGetErrorString(e));
         return TAV_ERR_CUDA;
@@ -1457,22 +1568,16 @@ int tav_remove_rows(tav_index* ix, const int64_t* ordinals, int64_t n, void* str
         return TAV_ERR_STATE;
     }
     // np.delete semantics: negative ordinals count from the end, duplicates remove one row, order is free
-    std::vector<int64_t> rem(static_cast<size_t>(n));
-    for (int64_t i = 0; i < n; ++i) {
-        const int64_t v = ordinals[i];
-        if (v < -ix->size || v >= ix->size) {
-            set_error("index %lld is out of bounds for axis 0 with size %lld", (long long)v, (long long)ix->size);
-            return TAV_ERR_RANGE;
-        }
-        rem[i] = v < 0 ? v + ix->size : v;
-    }
+    if (int rc = check_subset_ordinals(ix, ordinals, n)) return rc;
     if (n == 0) return TAV_OK;
+    std::vector<int64_t> rem(static_cast<size_t>(n));
+    for (int64_t i = 0; i < n; ++i) rem[i] = ordinals[i] < 0 ? ordinals[i] + ix->size : ordinals[i];
     if (!std::is_sorted(rem.begin(), rem.end())) std::sort(rem.begin(), rem.end());
     rem.erase(std::unique(rem.begin(), rem.end()), rem.end());
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;  // queued searches read the old rows
-    if (int rc = finish_before_row_change(ix, s)) return rc;
+    if (int rc = enter_stream(ix, s)) return rc;  // queued searches read the old rows
+    // the outstanding deferred searches are finished first: their exact redo reads the rows
+    if (int rc = finish_pending(ix, s, nullptr)) return rc;
     void* old_rows = nullptr;
     if (int rc = compact_rows(ix, rem, s, &old_rows)) return rc;
     if (ix->compact_path != 0) mark_done(ix);  // s was synchronised after the compaction
@@ -1506,10 +1611,10 @@ int tav_write_rows(tav_index* ix, int64_t first, const void* rows, int64_t n, in
         return TAV_ERR_INVALID;
     }
     if (n == 0) return TAV_OK;
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;  // queued searches read the old rows
-    if (int rc = finish_before_row_change(ix, s)) return rc;
+    if (int rc = enter_stream(ix, s)) return rc;  // queued searches read the old rows
+    // the outstanding deferred searches are finished first: their exact redo reads the rows
+    if (int rc = finish_pending(ix, s, nullptr)) return rc;
     if (int rc = store_rows(ix, first, rows, n, src_dtype, src_on_device, s)) return rc;
     ix->split_rows = std::min(ix->split_rows, first);
     ix->split_recheck = true;
@@ -1555,62 +1660,29 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         set_error("tav_search: invalid argument (k must be >= 1)");
         return TAV_ERR_INVALID;
     }
-    if ((subset && subset_len < 0) || (!subset && subset_len != 0)) {
-        set_error("tav_search: subset / subset_len mismatch");
-        return TAV_ERR_INVALID;
-    }
-    if ((flags & TAV_ITEMS_AS_POSITIONS) && !subset) {
-        set_error("tav_search: TAV_ITEMS_AS_POSITIONS needs a subset");
-        return TAV_ERR_INVALID;
-    }
+    if (int rc = check_subset_args("tav_search", flags, subset, subset_len, false)) return rc;
     if (n_queries == 0) return TAV_OK;
     std::lock_guard<std::mutex> lock(ix->mu);
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;
+    if (int rc = enter_stream(ix, s)) return rc;
     const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
-    const size_t nk = static_cast<size_t>(n_queries) * k;
     const uint32_t* d_mask = nullptr;
-    QueryMasks qm{};
-    if (flags & TAV_USE_QUERY_MASKS) {
-        if (int rc = use_query_masks(ix, "tav_search", n_queries, flags, subset != nullptr, &qm, &d_mask)) return rc;
-    } else if (flags & TAV_USE_ROW_MASK) {
-        if (ix->row_mask_rows != ix->size || ix->size == 0) {
-            set_error("tav_search: TAV_USE_ROW_MASK without a current row mask (tav_set_row_mask)");
-            return TAV_ERR_STATE;
-        }
-        if (subset) {
-            set_error("tav_search: a row mask and a subset cannot be combined");
-            return TAV_ERR_INVALID;
-        }
-        d_mask = static_cast<const uint32_t*>(ix->row_mask.p);
-    }
+    QueryMasks qm;
+    if (int rc = resolve_masks(ix, "tav_search", n_queries, flags, subset != nullptr, &d_mask, &qm)) return rc;
     const int ties_low = (flags & TAV_TIES_LOW_FIRST) ? 1 : 0;
     const int positions = (flags & TAV_ITEMS_AS_POSITIONS) && TAV_SHARDED_FILTER_MUTANT != 3 ? 1 : 0;
 
     int64_t* d_items = out_items;
     float* d_scores = out_scores;
     int32_t* d_counts = out_counts;
-    // host outputs: results are packed [items | scores | counts | done word] in one buffer so that a
-    // single D2H copy (into pinned staging) brings them back
-    const size_t off_scores = nk * sizeof(int64_t);
-    const size_t off_counts = off_scores + ((nk * sizeof(float) + 7) & ~size_t(7));
-    const size_t off_done = off_counts + ((static_cast<size_t>(n_queries) * sizeof(int32_t) + 7) & ~size_t(7));
-    const size_t pack_bytes = off_done + 8;
+    const ResultPack pack(n_queries, k);
     // Small result sets are written by the kernels straight into the pinned host staging (zero
     // copy over PCIe: no D2H memcpy call on the single-lookup latency path).
-    const bool zero_copy_out = !o_dev && pack_bytes <= kZeroCopyOutLimit;
+    const bool zero_copy_out = !o_dev && pack.bytes() <= kZeroCopyOutLimit;
 
     const int64_t n_scan = subset ? subset_len : ix->size;
-    ix->last_first_slot = -1;
-    ix->last_n_slots = 0;
-    TimedSearch* ts = cur_timed(ix);
-    if (!ts) ts = &ix->untimed;
+    TimedSearch* ts = begin_search(ix, 0);
     const bool timing = ts != &ix->untimed;
-    ts->used = 0;
-    ts->launches = 0;
-    ts->path = 0;
-    ts->valid = false;
 
     // a NaN min_score admits nothing on every path (`scores >= nan` is all-false in the reference)
     if (n_scan == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score) {
@@ -1628,15 +1700,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     }
 
     // subset ordinals: validate on the host (numpy raises IndexError)
-    if (subset) {
-        for (int64_t i = 0; i < subset_len; ++i) {
-            if (subset[i] < -ix->size || subset[i] >= ix->size) {
-                set_error("index %lld is out of bounds for axis 0 with size %lld",
-                          (long long)subset[i], (long long)ix->size);
-                return TAV_ERR_RANGE;
-            }
-        }
-    }
+    if (int rc = check_subset_ordinals(ix, subset, subset_len)) return rc;
 
     // path choice: tensor cores for batches on 16-bit storage, row scan otherwise
     bool use_mma = false, use_split = false;
@@ -1665,11 +1729,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         if (int rc = range_core(ix, ts, timing, d_q, n_queries, min_score, d_sub, n_scan, item_offset, d_mask, ties_low,
                                 static_cast<int64_t>(n_queries) * n_scan, false, offsets, s, positions, qm))
             return rc;
-        if (timing) {
-            TAV_CUDA(ev_record(ts->total[1], s));
-            ++ix->search_seq;
-        }
-        ts->valid = true;
+        if (int rc = end_search(ix, ts, s)) return rc;
         ix->range_total = offsets[n_queries];
         // each query's hits straight into its row of the caller's arrays (copies from device memory into
         // pageable memory return when done), then the padding
@@ -1697,17 +1757,11 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
 
     // result staging for host outputs (after the routing above, which needs none)
     if (zero_copy_out) {
-        TAV_CUDA(ix->pin_out.ensure(pack_bytes));
-        char* base = static_cast<char*>(ix->pin_out.p);
-        d_items = reinterpret_cast<int64_t*>(base);
-        d_scores = reinterpret_cast<float*>(base + off_scores);
-        d_counts = reinterpret_cast<int32_t*>(base + off_counts);
+        TAV_CUDA(ix->pin_out.ensure(pack.bytes()));
+        pack.place(ix->pin_out.p, &d_items, &d_scores, &d_counts);
     } else if (!o_dev) {
-        TAV_CUDA(ix->out_pack.ensure(pack_bytes));
-        char* base = static_cast<char*>(ix->out_pack.p);
-        d_items = reinterpret_cast<int64_t*>(base);
-        d_scores = reinterpret_cast<float*>(base + off_scores);
-        d_counts = reinterpret_cast<int32_t*>(base + off_counts);
+        TAV_CUDA(ix->out_pack.ensure(pack.bytes()));
+        pack.place(ix->out_pack.p, &d_items, &d_scores, &d_counts);
     }
 
     // ---- single-lookup latency form: ONE launch, no copies -------------------------------------
@@ -1722,11 +1776,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         if (int rc = ensure_scan_counters(ix, s)) return rc;
         uint64_t* d_bound = static_cast<uint64_t*>(ix->cand_count.p);
         uint32_t* d_count = reinterpret_cast<uint32_t*>(d_bound + 8);
-        ScanArgs a{};
-        a.corpus = ix->rows;
-        a.dtype = ix->dtype;
-        a.n_corpus = ix->size;
-        a.dim = ix->dim;
+        ScanArgs a = scan_args(ix);
         a.n_scan = n_scan;
         a.nq = 1;
         a.floor_score = min_score;
@@ -1752,7 +1802,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         // all k items and scores; every slot is one aligned store, so it arrives whole.  Larger k: one
         // completion word behind a fence.
         const bool watch_slots = k <= kWatchSlotsMaxK;
-        volatile uint32_t* done = reinterpret_cast<volatile uint32_t*>(static_cast<char*>(ix->pin_out.p) + off_done);
+        volatile uint32_t* done = reinterpret_cast<volatile uint32_t*>(static_cast<char*>(ix->pin_out.p) + pack.off_done);
         volatile int64_t* w_items = reinterpret_cast<volatile int64_t*>(d_items);
         volatile uint32_t* w_scores = reinterpret_cast<volatile uint32_t*>(d_scores);
         volatile int32_t* w_count = reinterpret_cast<volatile int32_t*>(d_counts);
@@ -1780,20 +1830,10 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             clock_gettime(CLOCK_MONOTONIC, &tsn);
             t_host0 = static_cast<unsigned long long>(tsn.tv_sec) * 1000000000ull + tsn.tv_nsec;
         }
-        if (timing) {
-            TAV_CUDA(ev_record(ts->total[0], s));
-            TAV_CUDA(ev_record(ts->ev[0][0], s));
-        }
-        TAV_CUDA(launch_scan1(a, queries, subset, s));
-        if (timing) {
-            ts->kind[0] = 0;
-            TAV_CUDA(ev_record(ts->ev[0][1], s));
-            ts->used = 1;
-            TAV_CUDA(ev_record(ts->total[1], s));
-        }
+        if (timing) TAV_CUDA(ev_record(ts->total[0], s));
+        TAV_CUDA(timed_launch(ix, ts, timing, 0, s, [&] { return launch_scan1(a, queries, subset, s); }));
         ts->launches = 1;
-        ts->valid = true;
-        if (timing) ++ix->search_seq;
+        if (int rc = end_search(ix, ts, s)) return rc;
         // spin on the completion word (a stream synchronise costs several microseconds more); fall
         // back to the synchronise when the word does not show up quickly (error, or a busy GPU)
         bool seen = false;
@@ -1834,10 +1874,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
                         (trace_host[5] - trace_host[4]) / 1e3, (trace_host[6] - trace_host[5]) / 1e3,
                         (trace_host[6] - trace_host[0]) / 1e3, (t_host1 - t_host0) / 1e3);
         }
-        const char* h = static_cast<const char*>(ix->pin_out.p);
-        memcpy(out_items, h, nk * sizeof(int64_t));
-        memcpy(out_scores, h + off_scores, nk * sizeof(float));
-        memcpy(out_counts, h + off_counts, sizeof(int32_t));
+        pack.unpack(ix->pin_out.p, out_items, out_scores, out_counts);
         return TAV_OK;
     }
 
@@ -1854,8 +1891,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         if (need > ix->held_queries.bytes) {
             const size_t want = std::max(need, 2 * ix->held_queries.bytes);
             if (ix->held_used > 0) {  // pending searches read the current buffer
-                ix->held_retired.push_back(ix->held_queries);
-                ix->held_queries = DevBuf{};
+                ix->held_retired.push_back(std::move(ix->held_queries));
                 ix->held_used = 0;
             }
             TAV_CUDA(ix->held_queries.ensure(want));
@@ -1882,10 +1918,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     if (use_mma) {
         ts->path = use_split ? 3 : 2;
         if (n_queries > ix->retry_cap || !ix->retry.p) {
-            if (!ix->pending.empty()) {
-                int redone = 0;
-                if (int rc = finish_pending(ix, s, &redone)) return rc;
-            }
+            if (int rc = finish_pending(ix, s, nullptr)) return rc;
             const int cap = std::max(std::min(n_queries, kMmaMaxQueries), 1024);
             const size_t bytes = (static_cast<size_t>(2) * kMaxPending + static_cast<size_t>(kMaxPending) * cap) * sizeof(int32_t);
             TAV_CUDA(ix->retry.ensure(bytes));
@@ -1894,30 +1927,19 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             memset(ix->retry_host.p, 0, 2 * kMaxPending * sizeof(int32_t));
             ix->retry_cap = cap;
         }
-        if (timing)  // the events of this search exist before the launcher records them
-            for (int i = 0; i < kMaxTimedKernels; ++i)
-                for (int j = 0; j < 2; ++j)
-                    if (!ts->ev[i][j]) TAV_CUDA(cudaEventCreate(&ts->ev[i][j]));
+        if (timing)
+            if (int rc = create_events(ts)) return rc;
         // one launch sequence per slab of kMmaMaxQueries queries (in practice: one)
         for (int q0 = 0; q0 < n_queries; q0 += kMmaMaxQueries) {
             const int nq = std::min(kMmaMaxQueries, n_queries - q0);
             // bookkeeping slot of this (part of the) search
-            if (static_cast<int>(ix->pending.size()) >= kMaxPending) {
-                int redone = 0;
-                if (int rc = finish_pending(ix, s, &redone)) return rc;
-            }
+            if (static_cast<int>(ix->pending.size()) >= kMaxPending)
+                if (int rc = finish_pending(ix, s, nullptr)) return rc;
             const int slot = ix->next_slot++;
             if (q0 == 0) ix->last_first_slot = slot;
             ix->last_n_slots = slot - ix->last_first_slot + 1;
-            MmaArgs m{};
-            m.device = ix->device;
-            m.corpus = use_split ? ix->split_hi.p : ix->rows;
-            m.corpus_lo = use_split ? ix->split_lo.p : nullptr;
-            m.split = use_split ? 1 : 0;
+            MmaArgs m = mma_args(ix, use_split);
             m.split_overflow = use_split ? retry_totals(ix, slot) + 1 : nullptr;
-            m.dtype = ix->dtype;
-            m.n_corpus = ix->size;
-            m.dim = ix->dim;
             m.queries = d_queries + static_cast<size_t>(q0) * ix->dim;
             m.nq = nq;
             m.floor_score = min_score;
@@ -1939,13 +1961,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             m.ev_max = kMaxTimedKernels;
             m.ev_used = &ev_used;
             m.ev_main_only = ix->timing_light ? 1 : 0;
-            const size_t ws = mma_workspace_bytes(m);
-            if (ws > ix->mma_ws.bytes) {
-                TAV_CUDA(cudaStreamSynchronize(s));  // earlier searches may still use the old workspace
-                TAV_CUDA(ix->mma_ws.ensure(ws));
-                // the sampler's unit counters (start of the workspace) must read zero
-                TAV_CUDA(cudaMemsetAsync(ix->mma_ws.p, 0, std::min<size_t>(ix->mma_ws.bytes, 65536), s));
-            }
+            if (int rc = ensure_mma_ws(ix, mma_workspace_bytes(m), s)) return rc;
             int launches = 0;
             TAV_CUDA(launch_mma_search(m, ix->mma_ws.p, ix->mma_ws.bytes, s, &launches));
             if (slab_timed) ts->used = ev_used;
@@ -1958,45 +1974,27 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
         // Queries the sampled admission threshold could not settle (fewer than k admitted rows
         // although rows were cut, or candidate overflow) are redone exactly by the row scan —
         // now, or in tav_finish_search when the caller defers the (synchronising) check.
-        if (!defer) {
-            int redone = 0;
-            if (int rc = finish_pending(ix, s, &redone)) return rc;
-        }
+        if (!defer)
+            if (int rc = finish_pending(ix, s, nullptr)) return rc;
     } else {
         ts->path = 1;
         int rc = scan_search(ix, ts, timing, d_queries, n_queries, k, min_score, d_subset, n_scan, item_offset,
                              d_items, d_scores, d_counts, d_mask, ties_low, s, !(flags & TAV_NO_FUSED_SCAN), positions, qm);
         if (rc != TAV_OK) return rc;
     }
-    if (timing) {
-        TAV_CUDA(ev_record(ts->total[1], s));
-        ++ix->search_seq;
-    }
-    ts->valid = true;
+    if (int rc = end_search(ix, ts, s)) return rc;
 
     if (o_dev) return mark_queued(ix, s);
     if (zero_copy_out) {
         TAV_CUDA(cudaStreamSynchronize(s));
-        const char* h = static_cast<const char*>(ix->pin_out.p);
-        memcpy(out_items, h, nk * sizeof(int64_t));
-        memcpy(out_scores, h + off_scores, nk * sizeof(float));
-        memcpy(out_counts, h + off_counts, static_cast<size_t>(n_queries) * sizeof(int32_t));
+        pack.unpack(ix->pin_out.p, out_items, out_scores, out_counts);
+    } else if (pack.bytes() <= kPinnedStageLimit) {
+        TAV_CUDA(ix->pin_out.ensure(pack.bytes()));
+        TAV_CUDA(cudaMemcpyAsync(ix->pin_out.p, ix->out_pack.p, pack.off_done, cudaMemcpyDeviceToHost, s));
+        TAV_CUDA(cudaStreamSynchronize(s));
+        pack.unpack(ix->pin_out.p, out_items, out_scores, out_counts);
     } else {
-        if (pack_bytes <= kPinnedStageLimit) {
-            TAV_CUDA(ix->pin_out.ensure(pack_bytes));
-            TAV_CUDA(cudaMemcpyAsync(ix->pin_out.p, ix->out_pack.p, off_done, cudaMemcpyDeviceToHost, s));
-            TAV_CUDA(cudaStreamSynchronize(s));
-            const char* h = static_cast<const char*>(ix->pin_out.p);
-            memcpy(out_items, h, nk * sizeof(int64_t));
-            memcpy(out_scores, h + off_scores, nk * sizeof(float));
-            memcpy(out_counts, h + off_counts, static_cast<size_t>(n_queries) * sizeof(int32_t));
-        } else {
-            TAV_CUDA(cudaMemcpyAsync(out_items, d_items, nk * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-            TAV_CUDA(cudaMemcpyAsync(out_scores, d_scores, nk * sizeof(float), cudaMemcpyDeviceToHost, s));
-            TAV_CUDA(cudaMemcpyAsync(out_counts, d_counts, static_cast<size_t>(n_queries) * sizeof(int32_t),
-                                     cudaMemcpyDeviceToHost, s));
-            TAV_CUDA(cudaStreamSynchronize(s));
-        }
+        if (int rc = copy_pack_out(pack, ix->out_pack.p, out_items, out_scores, out_counts, s)) return rc;
     }
     mark_done(ix);  // host outputs: s was synchronised above
     return TAV_OK;
@@ -2009,65 +2007,25 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
         set_error("tav_range_search: invalid argument");
         return TAV_ERR_INVALID;
     }
-    if ((subset && subset_len < 0) || (!subset && subset_len != 0)) {
-        set_error("tav_range_search: subset / subset_len mismatch");
-        return TAV_ERR_INVALID;
-    }
-    if (flags & TAV_DEFER_RETRY) {
-        set_error("tav_range_search: TAV_DEFER_RETRY is not available for threshold searches");
-        return TAV_ERR_INVALID;
-    }
-    if ((flags & TAV_ITEMS_AS_POSITIONS) && !subset) {
-        set_error("tav_range_search: TAV_ITEMS_AS_POSITIONS needs a subset");
-        return TAV_ERR_INVALID;
-    }
+    if (int rc = check_subset_args("tav_range_search", flags, subset, subset_len, true)) return rc;
     std::lock_guard<std::mutex> lock(ix->mu);
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;  // (also: a queued tav_range_fetch reads the hits replaced here)
+    if (int rc = enter_stream(ix, s)) return rc;  // (also: a queued tav_range_fetch reads the hits replaced here)
     const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
     ix->range_total = 0;
     std::vector<int64_t> offsets(static_cast<size_t>(n_queries) + 1, 0);
-    auto write_offsets = [&]() -> int {
-        const size_t bytes = offsets.size() * sizeof(int64_t);
-        if (o_dev) {  // from pageable memory: consumed when the call returns
-            TAV_CUDA(cudaMemcpyAsync(out_offsets, offsets.data(), bytes, cudaMemcpyHostToDevice, s));
-        } else {
-            memcpy(out_offsets, offsets.data(), bytes);
-        }
-        return mark_queued(ix, s);  // the sort after the last synchronisation may still run
-    };
     const uint32_t* d_mask = nullptr;
-    QueryMasks qm{};
-    if (flags & TAV_USE_QUERY_MASKS) {
-        if (int rc = use_query_masks(ix, "tav_range_search", n_queries, flags, subset != nullptr, &qm, &d_mask)) return rc;
-    } else if (flags & TAV_USE_ROW_MASK) {
-        if (ix->row_mask_rows != ix->size || ix->size == 0) {
-            set_error("tav_range_search: TAV_USE_ROW_MASK without a current row mask (tav_set_row_mask)");
-            return TAV_ERR_STATE;
-        }
-        if (subset) {
-            set_error("tav_range_search: a row mask and a subset cannot be combined");
-            return TAV_ERR_INVALID;
-        }
-        d_mask = static_cast<const uint32_t*>(ix->row_mask.p);
-    }
+    QueryMasks qm;
+    if (int rc = resolve_masks(ix, "tav_range_search", n_queries, flags, subset != nullptr, &d_mask, &qm)) return rc;
     const int64_t n_scan = subset ? subset_len : ix->size;
     // NaN min_score, empty corpus or empty subset: no hits
-    if (n_queries == 0 || n_scan == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score) return write_offsets();
+    if (n_queries == 0 || n_scan == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score)
+        return deliver_offsets(ix, offsets, out_offsets, o_dev, s);
     if (n_scan > 0xFFFFFFFFll) {
         set_error("tav_range_search: more than 2^32 rows per index are not supported; shard the corpus");
         return TAV_ERR_INVALID;
     }
-    if (subset) {
-        for (int64_t i = 0; i < subset_len; ++i) {
-            if (subset[i] < -ix->size || subset[i] >= ix->size) {
-                set_error("index %lld is out of bounds for axis 0 with size %lld", (long long)subset[i],
-                          (long long)ix->size);
-                return TAV_ERR_RANGE;
-            }
-        }
-    }
+    if (int rc = check_subset_ordinals(ix, subset, subset_len)) return rc;
     // path choice as in tav_search: tensor cores for batches (no subset), the row scan otherwise
     const bool mma_able = (mma_supported(ix->dtype, ix->dim) || (ix->dtype == TAV_F32 && mma_split_supported(ix->dim))) &&
                           !subset && n_queries <= kMmaMaxQueries && ix->size < (1ll << 31);
@@ -2077,13 +2035,8 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
         set_error("tav_range_search: TAV_FORCE_MMA needs dim %% 8 == 0, no subset, at most %d queries", kMmaMaxQueries);
         return TAV_ERR_INVALID;
     }
-    TimedSearch* ts = cur_timed(ix);
-    if (!ts) ts = &ix->untimed;
+    TimedSearch* ts = begin_search(ix, use_mma ? (ix->dtype == TAV_F32 ? 3 : 2) : 1);
     const bool timing = ts != &ix->untimed;
-    ts->used = 0;
-    ts->launches = 0;
-    ts->path = use_mma ? (ix->dtype == TAV_F32 ? 3 : 2) : 1;
-    ts->valid = false;
     const float* d_queries = nullptr;
     const int64_t* d_subset = nullptr;
     if (int rc = stage_inputs(ix, ts, timing, queries, n_queries, q_dev, false, subset, subset_len, &d_queries, &d_subset, s))
@@ -2092,13 +2045,9 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
                             (flags & TAV_TIES_LOW_FIRST) ? 1 : 0, expected_hits, use_mma, offsets, s,
                             (flags & TAV_ITEMS_AS_POSITIONS) && TAV_SHARDED_FILTER_MUTANT != 3 ? 1 : 0, qm))
         return rc;
-    if (timing) {
-        TAV_CUDA(ev_record(ts->total[1], s));
-        ++ix->search_seq;
-    }
-    ts->valid = true;
+    if (int rc = end_search(ix, ts, s)) return rc;
     ix->range_total = offsets[n_queries];
-    return write_offsets();
+    return deliver_offsets(ix, offsets, out_offsets, o_dev, s);
 }
 
 int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items, float* out_scores, int flags,
@@ -2114,9 +2063,8 @@ int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items,
         return TAV_ERR_RANGE;
     }
     if (n == 0) return TAV_OK;
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;  // after the range search that wrote the hits
+    if (int rc = enter_stream(ix, s)) return rc;  // after the range search that wrote the hits
     const cudaMemcpyKind kind = (flags & TAV_OUTPUTS_ON_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     TAV_CUDA(cudaMemcpyAsync(out_items, static_cast<const int64_t*>(ix->range_items.p) + first,
                              static_cast<size_t>(n) * sizeof(int64_t), kind, s));
@@ -2159,21 +2107,14 @@ static int check_subsets(const char* fn, int n_queries, int flags, const int64_t
     return TAV_OK;
 }
 
-static int check_subset_ordinals(const tav_index* ix, const int64_t* ordinals, int64_t n) {
-    for (int64_t i = 0; i < n; ++i)
-        if (ordinals[i] < -ix->size || ordinals[i] >= ix->size) {
-            set_error("index %lld is out of bounds for axis 0 with size %lld", (long long)ordinals[i],
-                      (long long)ix->size);
-            return TAV_ERR_RANGE;
-        }
-    return TAV_OK;
-}
-
 // Every entry of every query's subset scored in one gather, each query's admitted keys sorted: the hits in CSR
 // order in ix->range_items / range_scores, csr[nq + 1] on the host.  Synchronises once, to learn the counts.
-static int subsets_core(tav_index* ix, TimedSearch* ts, bool timing, const float* queries, int nq, bool q_dev,
-                        float floor, int ties_low, int positions, const int64_t* offsets, const int64_t* ordinals,
-                        std::vector<int64_t>& csr, cudaStream_t s) {
+static int subsets_core(tav_index* ix, TimedSearch* ts, bool timing, const float* queries, int nq, int flags,
+                        float floor, const int64_t* offsets, const int64_t* ordinals, std::vector<int64_t>& csr,
+                        cudaStream_t s) {
+    const bool q_dev = flags & TAV_QUERIES_ON_DEVICE;
+    const int ties_low = (flags & TAV_TIES_LOW_FIRST) && TAV_SUBSETS_MUTANT != 3 ? 1 : 0;
+    const int positions = (flags & TAV_ITEMS_AS_POSITIONS) ? 1 : 0;
     if (scan_collect_max_queries(ix->dim) < 1) {  // one query row in shared memory, as the row scan stages it
         set_error("per-query subsets: embedding size %d too large for the row-scan kernel", ix->dim);
         return TAV_ERR_INVALID;
@@ -2221,13 +2162,7 @@ static int subsets_core(tav_index* ix, TimedSearch* ts, bool timing, const float
     a.ties_low = ties_low;
     a.keys = keys;
     a.counts = d_counts;
-    const bool timed = timing && ts->used < kMaxTimedKernels;
-    if (timed) TAV_CUDA(ev_record(ts->ev[ts->used][0], s));
-    TAV_CUDA(launch_subset_gather(a, s));
-    if (timed) {
-        ts->kind[ts->used] = 0;
-        TAV_CUDA(ev_record(ts->ev[ts->used++][1], s));
-    }
+    TAV_CUDA(timed_launch(ix, ts, timing, 0, s, [&] { return launch_subset_gather(a, s); }));
     ts->launches += 1;
 
     std::vector<uint32_t> cnt(static_cast<size_t>(nq));
@@ -2244,19 +2179,6 @@ static int subsets_core(tav_index* ix, TimedSearch* ts, bool timing, const float
     return range_sort(ix, ts, timing, segs, csr[nq], positions ? nullptr : d_ordinals, 0, ties_low, s);
 }
 
-// the timing record of a subsets call
-static TimedSearch* begin_subsets_timing(tav_index* ix) {
-    ix->last_first_slot = -1;
-    ix->last_n_slots = 0;
-    TimedSearch* ts = cur_timed(ix);
-    if (!ts) ts = &ix->untimed;
-    ts->used = 0;
-    ts->launches = 0;
-    ts->path = 1;
-    ts->valid = false;
-    return ts;
-}
-
 extern "C" {
 
 int tav_search_subsets(tav_index* ix, const float* queries, int n_queries, int k, float min_score, int flags,
@@ -2269,11 +2191,11 @@ int tav_search_subsets(tav_index* ix, const float* queries, int n_queries, int k
     if (int rc = check_subsets("tav_search_subsets", n_queries, flags, offsets, ordinals)) return rc;
     if (n_queries == 0) return TAV_OK;
     std::lock_guard<std::mutex> lock(ix->mu);
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;
-    const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
-    const size_t nk = static_cast<size_t>(n_queries) * k;
+    if (int rc = enter_stream(ix, s)) return rc;
+    const bool o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
+    const ResultPack pack(n_queries, k);
+    const size_t nk = pack.nk;
     const int64_t total = offsets[n_queries];
     // no entries, no rows or a NaN min_score: no hits (as tav_search, before the ordinals are looked at)
     if (total == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score) {
@@ -2289,13 +2211,11 @@ int tav_search_subsets(tav_index* ix, const float* queries, int n_queries, int k
         return TAV_OK;
     }
     if (int rc = check_subset_ordinals(ix, ordinals, total)) return rc;
-    TimedSearch* ts = begin_subsets_timing(ix);
+    TimedSearch* ts = begin_search(ix, 1);
     const bool timing = ts != &ix->untimed;
-    const int ties_low = (flags & TAV_TIES_LOW_FIRST) && TAV_SUBSETS_MUTANT != 3 ? 1 : 0;
     std::vector<int64_t> csr;
     ix->range_total = 0;  // the hits land in the threshold search's buffers
-    if (int rc = subsets_core(ix, ts, timing, queries, n_queries, q_dev, min_score, ties_low,
-                              (flags & TAV_ITEMS_AS_POSITIONS) ? 1 : 0, offsets, ordinals, csr, s))
+    if (int rc = subsets_core(ix, ts, timing, queries, n_queries, flags, min_score, offsets, ordinals, csr, s))
         return rc;
     ix->range_total = csr[n_queries];
     const size_t n1 = static_cast<size_t>(n_queries) + 1;
@@ -2305,29 +2225,16 @@ int tav_search_subsets(tav_index* ix, const float* queries, int n_queries, int k
     int64_t* d_items = out_items;
     float* d_scores = out_scores;
     int32_t* d_counts = out_counts;
-    const size_t off_scores = nk * sizeof(int64_t);
-    const size_t off_counts = off_scores + ((nk * sizeof(float) + 7) & ~size_t(7));
     if (!o_dev) {
-        TAV_CUDA(ix->out_pack.ensure(off_counts + static_cast<size_t>(n_queries) * sizeof(int32_t)));
-        char* base = static_cast<char*>(ix->out_pack.p);
-        d_items = reinterpret_cast<int64_t*>(base);
-        d_scores = reinterpret_cast<float*>(base + off_scores);
-        d_counts = reinterpret_cast<int32_t*>(base + off_counts);
+        TAV_CUDA(ix->out_pack.ensure(pack.counts_end()));
+        pack.place(ix->out_pack.p, &d_items, &d_scores, &d_counts);
     }
     TAV_CUDA(launch_subset_topk_layout(n_queries, k, d_csr, static_cast<const int64_t*>(ix->range_items.p),
                                        static_cast<const float*>(ix->range_scores.p), d_items, d_scores, d_counts, s));
     ts->launches += 1;
-    if (timing) {
-        TAV_CUDA(ev_record(ts->total[1], s));
-        ++ix->search_seq;
-    }
-    ts->valid = true;
+    if (int rc = end_search(ix, ts, s)) return rc;
     if (o_dev) return mark_queued(ix, s);
-    TAV_CUDA(cudaMemcpyAsync(out_items, d_items, nk * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-    TAV_CUDA(cudaMemcpyAsync(out_scores, d_scores, nk * sizeof(float), cudaMemcpyDeviceToHost, s));
-    TAV_CUDA(cudaMemcpyAsync(out_counts, d_counts, static_cast<size_t>(n_queries) * sizeof(int32_t),
-                             cudaMemcpyDeviceToHost, s));
-    TAV_CUDA(cudaStreamSynchronize(s));
+    if (int rc = copy_pack_out(pack, ix->out_pack.p, out_items, out_scores, out_counts, s)) return rc;
     mark_done(ix);
     return TAV_OK;
 }
@@ -2340,10 +2247,8 @@ int tav_range_search_subsets(tav_index* ix, const float* queries, int n_queries,
     }
     if (int rc = check_subsets("tav_range_search_subsets", n_queries, flags, offsets, ordinals)) return rc;
     std::lock_guard<std::mutex> lock(ix->mu);
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;  // (also: a queued tav_range_fetch reads the hits replaced here)
-    const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
+    if (int rc = enter_stream(ix, s)) return rc;  // (also: a queued tav_range_fetch reads the hits replaced here)
     const int64_t total = offsets[n_queries];
     const bool none = n_queries == 0 || total == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score;
     if (!none)
@@ -2351,26 +2256,14 @@ int tav_range_search_subsets(tav_index* ix, const float* queries, int n_queries,
     std::vector<int64_t> csr(static_cast<size_t>(n_queries) + 1, 0);
     ix->range_total = 0;
     if (!none) {
-        TimedSearch* ts = begin_subsets_timing(ix);
+        TimedSearch* ts = begin_search(ix, 1);
         const bool timing = ts != &ix->untimed;
-        if (int rc = subsets_core(ix, ts, timing, queries, n_queries, q_dev, min_score,
-                                  (flags & TAV_TIES_LOW_FIRST) && TAV_SUBSETS_MUTANT != 3 ? 1 : 0,
-                                  (flags & TAV_ITEMS_AS_POSITIONS) ? 1 : 0, offsets, ordinals, csr, s))
+        if (int rc = subsets_core(ix, ts, timing, queries, n_queries, flags, min_score, offsets, ordinals, csr, s))
             return rc;
-        if (timing) {
-            TAV_CUDA(ev_record(ts->total[1], s));
-            ++ix->search_seq;
-        }
-        ts->valid = true;
+        if (int rc = end_search(ix, ts, s)) return rc;
         ix->range_total = csr[n_queries];
     }
-    const size_t bytes = csr.size() * sizeof(int64_t);
-    if (o_dev) {  // from pageable memory: consumed when the call returns
-        TAV_CUDA(cudaMemcpyAsync(out_offsets, csr.data(), bytes, cudaMemcpyHostToDevice, s));
-    } else {
-        memcpy(out_offsets, csr.data(), bytes);
-    }
-    return mark_queued(ix, s);  // the sort after the synchronisation may still run
+    return deliver_offsets(ix, csr, out_offsets, flags & TAV_OUTPUTS_ON_DEVICE, s);
 }
 
 int tav_mma_scores(tav_index* ix, const float* queries, int n_queries, int flags, float* out_device,
@@ -2382,9 +2275,8 @@ int tav_mma_scores(tav_index* ix, const float* queries, int n_queries, int flags
         set_error("tav_mma_scores: needs a non-empty index with dim %% 8 == 0");
         return TAV_ERR_INVALID;
     }
-    if (int rc = set_device(ix)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = join_stream(ix, s)) return rc;
+    if (int rc = enter_stream(ix, s)) return rc;
     // staged as a search stages them: normalised on a TAV_NORMALIZE index, so these are the search's dots
     TimedSearch not_timed;
     const float* d_queries = nullptr;
@@ -2394,24 +2286,12 @@ int tav_mma_scores(tav_index* ix, const float* queries, int n_queries, int flags
         return rc;
     if (split)
         if (int rc = ensure_split_planes(ix, nullptr, s)) return rc;
-    MmaArgs m{};
-    m.device = ix->device;
-    m.corpus = split ? ix->split_hi.p : ix->rows;
-    m.corpus_lo = split ? ix->split_lo.p : nullptr;
-    m.split = split ? 1 : 0;
+    MmaArgs m = mma_args(ix, split);
     m.split_overflow = split ? static_cast<int*>(ix->split_flag.p) + 1 : nullptr;
-    m.dtype = ix->dtype;
-    m.n_corpus = ix->size;
-    m.dim = ix->dim;
     m.queries = d_queries;
     m.nq = n_queries;
     m.k = 1;
-    const size_t ws = mma_workspace_bytes(m);
-    if (ws > ix->mma_ws.bytes) {
-        TAV_CUDA(cudaStreamSynchronize(s));
-        TAV_CUDA(ix->mma_ws.ensure(ws));
-        TAV_CUDA(cudaMemsetAsync(ix->mma_ws.p, 0, std::min<size_t>(ix->mma_ws.bytes, 65536), s));
-    }
+    if (int rc = ensure_mma_ws(ix, mma_workspace_bytes(m), s)) return rc;
     TAV_CUDA(launch_mma_dump(m, ix->mma_ws.p, ix->mma_ws.bytes, out_device, s));
     TAV_CUDA(cudaStreamSynchronize(s));
     mark_done(ix);
@@ -2497,8 +2377,6 @@ int tav_set_timing(tav_index* ix, int enabled) {
     if (ix->timing_on && !ix->hist) {
         ix->hist = new (std::nothrow) TimedSearch[kHistory];
         if (!ix->hist) return TAV_ERR_OOM;
-        for (int h = 0; h < kHistory; ++h)
-            for (auto& pr : ix->hist[h].ev) pr[0] = pr[1] = nullptr;
     }
     ix->search_seq = 0;
     ix->untimed.valid = false;
