@@ -13,6 +13,9 @@ real batch of 1024, config 5):
   * structure: full counts, scores descending, ordinals in range and unique;
   * decomposition: top-k over the whole corpus == merge of top-k over two halves (the sharded
     path's merge kernel), bit for bit.
+
+These checks run on random data, with tolerances, for a handful of queries.  Every query of every batch
+at these sizes is compared bit for bit in tests/test_gpu_scale_exact.py, on exact-arithmetic corpora.
 """
 
 from __future__ import annotations
@@ -37,7 +40,7 @@ class _Null:
 @pytest.mark.parametrize("rows,dim,storage,batch,k", [
     (1_000_000, 768, "bfloat16", 64, 32),      # BASELINE configs[1]
     (10_000_000, 768, "bfloat16", 256, 100),   # BASELINE configs[2] (the bench workload)
-    (1_250_000, 1536, "float16", 1024, 100),   # one shard of configs[3], with its real batch (4 query chunks)
+    (1_250_000, 1536, "float16", 1024, 100),   # one shard of configs[3], with its real batch (8 query chunks of 128)
     (50_000, 384, "bfloat16", 1000, 5),        # BASELINE configs[4]
 ])
 def test_full_size_properties(rows, dim, storage, batch, k):

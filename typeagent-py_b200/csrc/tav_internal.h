@@ -129,6 +129,14 @@ cudaError_t launch_subset_topk_layout(int nq, int k, const int64_t* csr_offsets,
 #define TAV_SUBSETS_MUTANT 0
 #endif
 
+// TAV_SCALE_MUTANT (tests only, never set by build.py): 1..3 compile one deliberate defect each that only shows on
+// corpora or subsets past 2^24 entries, so that tests/test_gpu_scale_exact.py can show its exact checks catch what
+// the small exact tests cannot: 1 the tensor-core MAIN epilogue keeps 24 bits of the row in its keys, 2 the subset
+// gather keeps 24 bits of the flat index j, 3 the segmented radix sort skips the byte of bits 24..31 of the position.
+#ifndef TAV_SCALE_MUTANT
+#define TAV_SCALE_MUTANT 0
+#endif
+
 // ---- segmented sort of the threshold search's keys (tav_sort.cu) -----------------------
 // One segment per query: n keys (unsorted, unique) at `keys`; sorted descending and decoded into
 // out_items / out_scores [out, out + n).  Segments above kSmallSortMax keys also need `tmp` (n keys of

@@ -148,7 +148,11 @@ __device__ __forceinline__ void admit_group(const float (&d)[NACC], int g, int h
                 const int i = 8 * jj + 2 * t4 + e;
                 if (x >= tau && ((amask >> i) & 1u)) {
                     if (n_admitted < cap_seg)
+#if TAV_SCALE_MUTANT == 1
+                        my_cand[n_admitted] = (static_cast<uint64_t>(__float_as_uint(x)) << 32) | ((rbase + i) & 0xFFFFFFu);
+#else
                         my_cand[n_admitted] = (static_cast<uint64_t>(__float_as_uint(x)) << 32) | (rbase + i);
+#endif
                     ++n_admitted;
                 }
             }

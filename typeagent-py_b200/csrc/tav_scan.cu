@@ -709,7 +709,11 @@ __global__ void __launch_bounds__(kScanThreads) subset_gather_kernel(const Subse
             if (lane == leader) base = atomicAdd(&a.counts[q], static_cast<uint32_t>(__popc(m)));
             base = __shfl_sync(0xFFFFFFFFu, base, leader);
             if (want) {
-                const uint32_t j = static_cast<uint32_t>(pos);  // flat index into the ordinals (< 2^32)
+                const uint32_t j = static_cast<uint32_t>(pos)  // flat index into the ordinals (< 2^32)
+#if TAV_SCALE_MUTANT == 2
+                                   & 0xFFFFFFu
+#endif
+                    ;
                 qkeys[base + __popc(m & ((1u << lane) - 1u))] = make_key(s, a.ties_low ? ~j : j);
             }
         }

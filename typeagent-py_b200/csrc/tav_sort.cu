@@ -34,6 +34,9 @@ __device__ __forceinline__ int radix_passes(const uint64_t* minmax, int l) {
 }
 
 __device__ __forceinline__ uint32_t bucket_of(uint64_t key, int pass) {
+#if TAV_SCALE_MUTANT == 3
+    if (pass == 3) return 0u;
+#endif
     return 255u - static_cast<uint32_t>((key >> (8 * pass)) & 0xFFu);
 }
 
