@@ -168,6 +168,7 @@ struct tav_index {
     size_t held_used = 0;        // bytes of held_queries used by pending searches
     std::vector<DevBuf> held_retired;  // outgrown held_queries buffers that pending searches still read
     int last_first_slot = -1, last_n_slots = 0;   // bookkeeping slots of the most recent search (-1: row scan)
+    bool last_split = false;     // the most recent search ran the split form (finish redoes it all on split_flag[0])
     // float32 indexes: the rows as two fp16 planes for the tensor-core path (built lazily,
     // extended on append); split_flag[0] = a corpus value left the fp16 range
     DevBuf split_hi, split_lo, split_flag;
@@ -676,6 +677,7 @@ static inline cudaError_t ev_record(cudaEvent_t& ev, cudaStream_t s) {
 static TimedSearch* begin_search(tav_index* ix, int path) {
     ix->last_first_slot = -1;
     ix->last_n_slots = 0;
+    ix->last_split = false;
     TimedSearch* ts = cur_timed(ix);
     if (!ts) ts = &ix->untimed;
     ts->used = 0;
@@ -1644,6 +1646,11 @@ const int32_t* tav_internal_retry_totals(tav_index* ix, int* count) {
     return retry_totals(ix, ix->last_first_slot);
 }
 
+const int* tav_internal_split_flag(tav_index* ix) {
+    if (!ix || ix->last_first_slot < 0 || !ix->last_split) return nullptr;
+    return static_cast<const int*>(ix->split_flag.p);
+}
+
 int tav_finish_search(tav_index* ix, void* stream, int* redone) {
     if (!ix) return TAV_ERR_INVALID;
     std::lock_guard<std::mutex> lock(ix->mu);
@@ -1938,6 +1945,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             const int slot = ix->next_slot++;
             if (q0 == 0) ix->last_first_slot = slot;
             ix->last_n_slots = slot - ix->last_first_slot + 1;
+            ix->last_split = use_split;
             MmaArgs m = mma_args(ix, use_split);
             m.split_overflow = use_split ? retry_totals(ix, slot) + 1 : nullptr;
             m.queries = d_queries + static_cast<size_t>(q0) * ix->dim;

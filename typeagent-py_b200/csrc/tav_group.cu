@@ -48,10 +48,12 @@ struct PeerTable {
 // every peer's region, then arrive[me] = seq everywhere.  Waits first until every peer acknowledged
 // the search that used this slot `depth` searches ago.
 // The last 16 bytes of a slot are its tail: word 0 = number of this rank's queries that its exact redo
-// will still correct at finish (read here from the local search's device counters).
+// will still correct at finish (read here from the local search's device counters and, for a split search,
+// the index's corpus flag), exactly the number tav_finish_search will redo.
 __global__ void __launch_bounds__(256)
 publish_kernel(PeerTable peers, int me, int world, size_t off_ack, size_t off_slot, size_t bytes, uint32_t seq,
-               uint32_t need_ack, uint32_t* ticket, const int32_t* retry_totals, int n_retry) {
+               uint32_t need_ack, uint32_t* ticket, const int32_t* retry_totals, int n_retry, const int* corpus_flag,
+               int nq) {
     __shared__ int s_last;
     const char* src = peers.region[me] + off_slot;
     if (blockIdx.x == 0 && threadIdx.x < world && threadIdx.x != me) {
@@ -72,12 +74,19 @@ publish_kernel(PeerTable peers, int me, int world, size_t off_ack, size_t off_sl
     }
     __syncthreads();
     if (blockIdx.x == 0 && threadIdx.x < world) {
+        // per bookkeeping slot (a slab of up to kMmaMaxQueries queries): its flagged queries, or all of them when
+        // the split form left the fp16 range in the corpus or in one of its queries (finish then redoes the slab)
+        const bool corpus_out = corpus_flag && __ldcg(corpus_flag);
         uint32_t flagged = 0;
-        for (int i = 0; i < n_retry; ++i)  // flagged queries + "a query value left the fp16 range" (split form)
-            flagged += static_cast<uint32_t>(__ldcg(&retry_totals[2 * i])) + static_cast<uint32_t>(__ldcg(&retry_totals[2 * i + 1]));
-        *reinterpret_cast<uint32_t*>(peers.region[threadIdx.x] + off_slot + bytes - 16) = flagged;
+        for (int i = 0; i < n_retry; ++i) {
+            const int slab = min(kMmaMaxQueries, nq - i * kMmaMaxQueries);
+            flagged += static_cast<uint32_t>(corpus_out || __ldcg(&retry_totals[2 * i + 1]) ? slab
+                                                                                          : __ldcg(&retry_totals[2 * i]));
+        }
+        *reinterpret_cast<uint32_t*>(peers.region[threadIdx.x] + off_slot + bytes - 16) = TAV_GROUP_MUTANT == 1 ? 0u : flagged;
     }
-    const size_t n16 = (bytes - 16) / 16;  // sections are padded to 16 bytes by the host side; the tail goes separately
+    // sections are padded to 16 bytes by the host side; the tail goes separately
+    const size_t n16 = (bytes - 16) / 16 - (TAV_GROUP_MUTANT == 2 ? 1 : 0);
     for (int w = 0; w < world; ++w) {
         if (w == me) continue;
         uint4* dst = reinterpret_cast<uint4*>(peers.region[w] + off_slot);
@@ -256,7 +265,8 @@ int tav_group_capacity(const tav_group* g, int* max_queries, int* max_k, int* de
 
 // exchange + merge of the list this rank holds in its own slot for sequence number `seq`
 static int publish_and_merge(tav_group* g, int nq, int k, uint32_t seq, const int32_t* retry_totals, int n_retry,
-                             int64_t* out_items, float* out_scores, int32_t* out_counts, cudaStream_t s) {
+                             const int* corpus_flag, int64_t* out_items, float* out_scores, int32_t* out_counts,
+                             cudaStream_t s) {
     const int slot = static_cast<int>(seq % static_cast<uint32_t>(g->depth));
     size_t off_scores, off_counts, bytes;
     packed_offsets(nq, k, &off_scores, &off_counts, &bytes);
@@ -268,7 +278,7 @@ static int publish_and_merge(tav_group* g, int nq, int k, uint32_t seq, const in
         const uint32_t need_ack = seq - static_cast<uint32_t>(g->depth);
         const uint32_t need = seq > static_cast<uint32_t>(g->depth) ? need_ack : 0u;
         publish_kernel<<<grid, 256, 0, s>>>(g->peers, g->rank, g->world, g->off_ack, off_mine, bytes, seq, need,
-                                            g->ticket, retry_totals, retry_totals ? n_retry : 0);
+                                            g->ticket, retry_totals, retry_totals ? n_retry : 0, corpus_flag, nq);
         TAVG_CUDA(cudaGetLastError());
     }
     // lists of all ranks for this slot lie side by side in MY region: strides between ranks = slot_bytes.
@@ -348,6 +358,7 @@ int tav_sharded_search(tav_index* ix, tav_group* g, const float* queries_device,
     }
     int n_retry = 0;
     const int32_t* retry_totals = tav_size(ix) == 0 ? nullptr : tav_internal_retry_totals(ix, &n_retry);
+    const int* corpus_flag = tav_size(ix) == 0 ? nullptr : tav_internal_split_flag(ix);
     // deferred (pipelined) searches: exchange on the group's stream, ordered after the local search by an event
     cudaStream_t xs = s;
     if (defer && g->world > 1) {
@@ -359,7 +370,8 @@ int tav_sharded_search(tav_index* ix, tav_group* g, const float* queries_device,
         TAVG_CUDA(cudaStreamWaitEvent(s, g->ev_merged[slot], 0));
         g->x_pending = false;
     }
-    int rc = publish_and_merge(g, n_queries, k, seq, retry_totals, n_retry, out_items, out_scores, out_counts, xs);
+    int rc = publish_and_merge(g, n_queries, k, seq, retry_totals, n_retry, corpus_flag, out_items, out_scores,
+                               out_counts, xs);
     if (rc != TAV_OK) return rc;
     if (xs != s) g->x_pending = true;
     g->open.push_back({seq, n_queries, k, out_items, out_scores, out_counts});
@@ -416,14 +428,14 @@ int tav_sharded_finish(tav_index* ix, tav_group* g, void* stream, int* redone_to
             const uint32_t seq = ++g->seq;
             const int old_slot = static_cast<int>(o.seq % static_cast<uint32_t>(g->depth));
             const int new_slot = static_cast<int>(seq % static_cast<uint32_t>(g->depth));
-            if (new_slot != old_slot) {
+            if (new_slot != old_slot && TAV_GROUP_MUTANT != 3) {
                 size_t os, oc, bytes;
                 packed_offsets(o.nq, o.k, &os, &oc, &bytes);
                 const char* from = g->region + g->off_slots + (static_cast<size_t>(old_slot) * g->world + g->rank) * g->slot_bytes;
                 char* to = g->region + g->off_slots + (static_cast<size_t>(new_slot) * g->world + g->rank) * g->slot_bytes;
                 TAVG_CUDA(cudaMemcpyAsync(to, from, bytes, cudaMemcpyDeviceToDevice, s));
             }
-            rc = publish_and_merge(g, o.nq, o.k, seq, nullptr, 0, o.items, o.scores, o.counts, s);
+            rc = publish_and_merge(g, o.nq, o.k, seq, nullptr, 0, nullptr, o.items, o.scores, o.counts, s);
             if (rc != TAV_OK) return rc;
         }
         TAVG_CUDA(cudaStreamSynchronize(s));

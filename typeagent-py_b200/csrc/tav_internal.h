@@ -215,6 +215,15 @@ cudaError_t launch_map_items(int64_t n, const int64_t* table, int64_t table_len,
 #define TAV_SHARDED_FILTER_MUTANT 0
 #endif
 
+// TAV_GROUP_MUTANT (tests only, never set by build.py): 1..3 compile one deliberate defect each into the peer
+// exchange (tav_group.cu), so that tests/test_gpu_peer_exchange.py can show its exact checks catch it: 1 the
+// published tail is always 0 (no search is ever repaired), 2 one 16-byte vector fewer of each list is stored
+// into the peers (its last counts reach them stale), 3 a repair publishes from its new slot without copying the
+// list there.  Every wait of the protocol stays satisfiable: the results are wrong, nothing spins out.
+#ifndef TAV_GROUP_MUTANT
+#define TAV_GROUP_MUTANT 0
+#endif
+
 // ---- compaction after a removal (tav_compact.cu) -----------------------------------------
 // keys: device [m], keys[i] = rem[i] - i over the sorted distinct removed ordinals.  Destinations
 // [d_begin, d_end) of the compacted rows: dst row (d - d_base) = src row (d + #{keys <= d}).  src and dst
@@ -303,6 +312,10 @@ void set_error(const char* fmt, ...);
 // published candidate list so that every rank learns, without a second exchange, whether some rank will
 // correct its candidates at finish.
 extern "C" const int32_t* tav_internal_retry_totals(tav_index* ix, int* count);
+// library-internal: device address of the index's "a corpus value left the fp16 range" flag when its most recent
+// search ran the split form (float32 rows as two fp16 planes), else nullptr.  While the flag is set, finish redoes
+// every query of such a search, so the sharded search counts all of them in the published tail.
+extern "C" const int* tav_internal_split_flag(tav_index* ix);
 
 // library-internal: how tav_remove_rows compacts on this index.  `mode` 0 the default (in place), 1 out of
 // place (TAV_ERR_OOM when its allocation fails), 2 in place; `scratch_bytes` bounds the in-place window buffer (0: the

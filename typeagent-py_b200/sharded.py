@@ -142,6 +142,26 @@ class CudaShardEngine:
             self._group_keep.clear()
         return redone.value
 
+    def close(self, dist, process_group) -> None:
+        """Collective: free this rank's exchange region and its rows, in the order that keeps every peer safe —
+        synchronise the device, wait for every rank, destroy the region and the index, wait again — so that no
+        rank frees a region a peer may still publish into.  Every rank passes both barriers even when its device
+        failed; that error is raised afterwards."""
+        error = None
+        try:
+            self.torch.cuda.synchronize(self.device)
+        except Exception as e:  # noqa: BLE001
+            error = e
+        dist.barrier(group=process_group)
+        group, self._group = self._group, None
+        self._group_keep.clear()
+        if group is not None:
+            _capi.load().tav_group_destroy(group)
+        self.base.clear()
+        dist.barrier(group=process_group)
+        if error is not None:
+            raise error
+
     def __del__(self):
         try:
             if self._group is not None:
@@ -720,6 +740,15 @@ class ShardedVectorBase:
         if not defer_check:
             self.finish()
         return out
+
+    def close(self) -> None:
+        """Release this rank's device state (its rows and, with ``exchange="peer"``, its exchange region).
+        Collective: every rank calls it.  Deferred lookups that were not finished are dropped; call ``finish()``
+        first to keep them.  An engine without device state has nothing to release."""
+        self._pending = []
+        close = getattr(self._engine, "close", None)
+        if close is not None:
+            close(self._dist, self._group)
 
     def finish(self) -> int:
         """Resolve a deferred lookup on every rank; returns the number of queries (summed over
