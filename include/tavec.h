@@ -355,6 +355,42 @@ int tav_sharded_search(tav_index* ix, tav_group* g, const float* queries_device,
 int tav_sharded_finish(tav_index* ix, tav_group* g, void* stream, int* redone_total);
 
 /*
+ * Rebalance of row-sharded indexes (ShardedVectorBase.rebalance): every rank's new block is copied from the
+ * ranks' current row allocations over CUDA IPC, in the storage dtype, byte for byte, by the copy engines.
+ *
+ *   tav_rows_export  writes this index's record (tav_rows_handle_bytes() bytes: the IPC handle of its row
+ *                    allocation and its row count) to handle_out and the row count to *rows_out, after the
+ *                    work queued by earlier calls on the index has run.  An index without rows gives a record
+ *                    that no piece may read.  Adopted memory: TAV_ERR_STATE.
+ *   tav_rows_stage   allocates this rank's new block (library-owned, capacity = its row count) and copies
+ *                    `n_parts` pieces into it in order: piece i is rows [part_first[i], part_first[i] +
+ *                    part_rows[i]) of rank part_src_rank[i]'s block, this index's own rows for
+ *                    part_src_rank[i] == rank, the peers' through the records in `handles` (world records,
+ *                    rank order).  A piece outside its source's rows: TAV_ERR_RANGE; a bad rank, or a source
+ *                    whose rows have another width or dtype: TAV_ERR_INVALID; all checked on the host before
+ *                    anything is allocated.  With `mirror_out` (host float32
+ *                    [rows, dim]; a float32 index without TAV_NORMALIZE only, else TAV_ERR_INVALID) the staged
+ *                    rows are also read back into it.  Joins the index's call order, finishes outstanding
+ *                    TAV_DEFER_RETRY searches, synchronises `stream` and closes the peers' mappings before it
+ *                    returns.  An allocation failure gives TAV_ERR_OOM; on any failure nothing stays staged and
+ *                    the index is unchanged.  One staged block at a time: a second stage gives TAV_ERR_STATE.
+ *   tav_rows_commit  commit = 1: the staged block becomes the index's rows, the old allocation is freed, the
+ *                    row mask and per-query masks are dropped and the fp16 planes of a float32 index are
+ *                    rebuilt from row 0 at the next tensor-core search (with their "left the fp16 range" flag).
+ *                    Nothing staged: TAV_ERR_STATE.  commit = 0: the staged block is freed, nothing changes.
+ *
+ * Protocol: every rank exports, the records are exchanged (any host-side means), every rank stages, the ranks
+ * agree that all stages succeeded (a rank has finished reading its peers' rows when its stage returns), then
+ * every rank commits (or every rank drops).  No rank may change or free its rows between its export and the
+ * agreement.
+ */
+int tav_rows_handle_bytes(void);
+int tav_rows_export(tav_index* ix, void* handle_out, int64_t* rows_out);
+int tav_rows_stage(tav_index* ix, int world, int rank, const void* handles, int n_parts, const int32_t* part_src_rank,
+                   const int64_t* part_first, const int64_t* part_rows, float* mirror_out, void* stream);
+int tav_rows_commit(tav_index* ix, int commit);
+
+/*
  * Chunk -> message fold of hit lists, on the device, in place (storage/memory/messageindex.py:
  * 185-207 `to_scored_message_ordinals`; the reference folds AFTER the top-k over chunks): walking
  * each query's hits in score order, the first hit of a group keeps its score, later hits of the

@@ -71,6 +71,11 @@ SIGNATURES = {
     "tav_sharded_search": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int,
                                      C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tav_sharded_finish": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
+    "tav_rows_handle_bytes": (C.c_int, []),
+    "tav_rows_export": (C.c_int, [C.c_void_p, C.c_void_p, _i64p]),
+    "tav_rows_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tav_rows_commit": (C.c_int, [C.c_void_p, C.c_int]),
     "tav_timing_history": (C.c_int, [C.c_void_p, C.c_int, _f32p, _f32p, _f32p, _f32p, C.POINTER(C.c_int)]),
     "tav_merge_topk": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_int64, C.c_int64, C.c_int64,

@@ -184,6 +184,12 @@ struct tav_index {
     int64_t compact_scratch = 0;     // bytes of the in-place window buffer (0: kCompactScratchBytes)
     int compact_path = 0;            // 0 nothing moved, 1 out of place, 2 in place
     int64_t compact_windows = 0;
+    // rebalance (tav_rows_stage / tav_rows_commit): the staged new block and the cap on its allocation
+    void* staged = nullptr;
+    int64_t staged_rows = 0;
+    size_t rows_bytes = 0;           // bytes of the library-owned allocation behind `rows` (0 when adopted)
+    size_t staged_bytes = 0;
+    int64_t stage_cap = -1;          // bytes, -1 = no cap (tav_internal_stage_cap)
     // predicate pushdown: one bit per row (tav_set_row_mask)
     DevBuf row_mask;
     int64_t row_mask_rows = 0;   // 0 = no mask set
@@ -213,6 +219,20 @@ struct tav_index {
     bool timing_on = false;
     bool timing_light = false;  // events only around the dominant kernel and the whole search
 };
+
+// Bytes held in row blocks (the library-owned rows of every index of the process, and their staged blocks): every
+// such allocation and free goes through these two, so tav_internal_row_bytes can show that a replaced block was freed.
+static std::atomic<int64_t> g_row_bytes{0};
+static cudaError_t rows_malloc(void** p, size_t bytes) {
+    cudaError_t e = cudaMalloc(p, bytes);
+    if (e == cudaSuccess) g_row_bytes += static_cast<int64_t>(bytes);
+    return e;
+}
+static void rows_free(void* p, size_t bytes) {
+    if (!p) return;
+    cudaFree(p);
+    g_row_bytes -= static_cast<int64_t>(bytes);
+}
 
 static TimedSearch* cur_timed(tav_index* ix) {
     return ix->timing_on && ix->hist ? &ix->hist[(ix->search_seq) % kHistory] : nullptr;
@@ -416,7 +436,8 @@ int tav_destroy(tav_index* ix) {
     if (!ix) return TAV_OK;
     cudaSetDevice(ix->device);
     cudaDeviceSynchronize();  // searches may still be in flight on the caller's streams
-    if (ix->rows && !ix->adopted) cudaFree(ix->rows);
+    if (!ix->adopted) rows_free(ix->rows, ix->rows_bytes);
+    rows_free(ix->staged, ix->staged_bytes);
     if (ix->ev_last) cudaEventDestroy(ix->ev_last);
     if (ix->ev_pin_in) cudaEventDestroy(ix->ev_pin_in);
     for (auto& ev : ix->ev_append)
@@ -459,22 +480,24 @@ static int reserve_locked(tav_index* ix, int64_t rows, cudaStream_t s) {
     if (int rc = set_device(ix)) return rc;
     const size_t row_bytes = static_cast<size_t>(ix->dim) * dtype_size(ix->dtype);
     void* fresh = nullptr;
-    TAV_CUDA(cudaMalloc(&fresh, std::max<size_t>(static_cast<size_t>(rows) * row_bytes, 256)));
+    const size_t fresh_bytes = std::max<size_t>(static_cast<size_t>(rows) * row_bytes, 256);
+    TAV_CUDA(rows_malloc(&fresh, fresh_bytes));
     if (ix->size > 0) {
         cudaError_t e = cudaMemcpyAsync(fresh, ix->rows, static_cast<size_t>(ix->size) * row_bytes,
                                         cudaMemcpyDeviceToDevice, s);
         if (e == cudaSuccess) e = cudaStreamSynchronize(s);
         if (e != cudaSuccess) {
-            cudaFree(fresh);
+            rows_free(fresh, fresh_bytes);
             set_error("tav_reserve: copy failed: %s", cudaGetErrorString(e));
             return TAV_ERR_CUDA;
         }
     }
     if (ix->rows) {
         cudaDeviceSynchronize();
-        cudaFree(ix->rows);
+        rows_free(ix->rows, ix->rows_bytes);
     }
     ix->rows = fresh;
+    ix->rows_bytes = fresh_bytes;
     ix->capacity = rows;
     return TAV_OK;
 }
@@ -539,8 +562,9 @@ int tav_adopt_device(tav_index* ix, void* device_rows, int64_t n, int dim) {
     if (int rc = wait_queued(ix)) return rc;  // queued searches read the rows replaced here
     if (ix->rows && !ix->adopted) {
         cudaDeviceSynchronize();
-        cudaFree(ix->rows);
+        rows_free(ix->rows, ix->rows_bytes);
     }
+    ix->rows_bytes = 0;
     ix->dim = dim;
     ix->rows = device_rows;
     ix->split_rows = 0;  // (the planes' overflow flag is reset where they are rebuilt from row 0)
@@ -1481,8 +1505,10 @@ constexpr size_t kCompactScratchBytes = size_t(256) << 20;  // window buffer of 
 // capacity, the rows before rem[0] copied over unchanged, each moving row read and written once; the old
 // allocation is handed back in *old_rows for the caller to free.  In place by default: ascending windows of destinations, each gathered into a scratch buffer and copied back (the
 // sources of a window lie at or above its first row, and rows above it are written only by later windows).
-static int compact_rows(tav_index* ix, const std::vector<int64_t>& rem, cudaStream_t s, void** old_rows) {
+static int compact_rows(tav_index* ix, const std::vector<int64_t>& rem, cudaStream_t s, void** old_rows,
+                        size_t* old_bytes) {
     *old_rows = nullptr;
+    *old_bytes = 0;
     ix->compact_path = 0;
     ix->compact_windows = 0;
     const int64_t m = static_cast<int64_t>(rem.size());
@@ -1502,7 +1528,8 @@ static int compact_rows(tav_index* ix, const std::vector<int64_t>& rem, cudaStre
     // of the rows cost about what the scratch round trip costs (DESIGN.md §3.5), and it needs no second copy.
     if (ix->compact_mode == 1) {
         void* fresh = nullptr;
-        cudaError_t e = cudaMalloc(&fresh, std::max<size_t>(static_cast<size_t>(ix->capacity) * row, 256));
+        const size_t fresh_bytes = std::max<size_t>(static_cast<size_t>(ix->capacity) * row, 256);
+        cudaError_t e = rows_malloc(&fresh, fresh_bytes);
         if (e != cudaSuccess) {
             cudaGetLastError();
             set_error("tav_remove_rows: no device memory for an out-of-place compaction");
@@ -1513,12 +1540,14 @@ static int compact_rows(tav_index* ix, const std::vector<int64_t>& rem, cudaStre
         if (e == cudaSuccess) e = launch_compact_gather(ix->rows, fresh, d_keys, m, first, new_size, 0, row, s);
         if (e == cudaSuccess) e = cudaStreamSynchronize(s);
         if (e != cudaSuccess) {
-            cudaFree(fresh);
+            rows_free(fresh, fresh_bytes);
             set_error("tav_remove_rows: compaction failed: %s", cudaGetErrorString(e));
             return TAV_ERR_CUDA;
         }
         *old_rows = ix->rows;
+        *old_bytes = ix->rows_bytes;
         ix->rows = fresh;
+        ix->rows_bytes = fresh_bytes;
         ix->compact_path = 1;
         ix->compact_windows = 1;
         return TAV_OK;
@@ -1581,9 +1610,10 @@ int tav_remove_rows(tav_index* ix, const int64_t* ordinals, int64_t n, void* str
     // the outstanding deferred searches are finished first: their exact redo reads the rows
     if (int rc = finish_pending(ix, s, nullptr)) return rc;
     void* old_rows = nullptr;
-    if (int rc = compact_rows(ix, rem, s, &old_rows)) return rc;
+    size_t old_bytes = 0;
+    if (int rc = compact_rows(ix, rem, s, &old_rows, &old_bytes)) return rc;
     if (ix->compact_path != 0) mark_done(ix);  // s was synchronised after the compaction
-    if (old_rows) cudaFree(old_rows);
+    rows_free(old_rows, old_bytes);
     ix->size -= static_cast<int64_t>(rem.size());
     ix->split_rows = std::min(ix->split_rows, rem[0]);
     ix->split_recheck = true;
@@ -1636,6 +1666,210 @@ int tav_internal_compact_stats(tav_index* ix, int* path, int64_t* windows) {
     std::lock_guard<std::mutex> lock(ix->mu);
     if (path) *path = ix->compact_path;
     if (windows) *windows = ix->compact_windows;
+    return TAV_OK;
+}
+
+int tav_internal_row_bytes(tav_index* ix, int64_t* index_bytes, int64_t* process_bytes) {
+    if (!ix) return TAV_ERR_INVALID;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (index_bytes) *index_bytes = static_cast<int64_t>((ix->adopted ? 0 : ix->rows_bytes) + ix->staged_bytes);
+    if (process_bytes) *process_bytes = g_row_bytes.load();
+    return TAV_OK;
+}
+
+int tav_internal_stage_cap(tav_index* ix, int64_t max_bytes) {
+    if (!ix || max_bytes < -1) return TAV_ERR_INVALID;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    ix->stage_cap = max_bytes;
+    return TAV_OK;
+}
+
+}  // extern "C"
+
+// ---- rebalance: a rank's new block copied from the ranks' row allocations over CUDA IPC -------------------
+// one rank's record, as tav_rows_export writes it and tav_rows_stage reads it
+struct RowsRecord {
+    cudaIpcMemHandle_t handle;
+    int64_t rows;       // rows of the rank's block
+    int64_t has_handle; // 0: the rank has no row allocation (no piece can come from it)
+    int32_t dim;        // the row layout: a piece is read with the stager's row size, so the ranks' must match
+    int32_t dtype;
+};
+
+// the peers' row allocations mapped into this process for one stage; closed when it goes out of scope
+struct PeerMappings {
+    std::vector<void*> base;
+    explicit PeerMappings(int world) : base(static_cast<size_t>(world), nullptr) {}
+    ~PeerMappings() {
+        for (void* p : base)
+            if (p) cudaIpcCloseMemHandle(p);
+    }
+};
+
+extern "C" {
+
+int tav_rows_handle_bytes(void) { return static_cast<int>(sizeof(RowsRecord)); }
+
+int tav_rows_export(tav_index* ix, void* handle_out, int64_t* rows_out) {
+    if (!ix || !handle_out) return TAV_ERR_INVALID;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (ix->adopted) {
+        set_error("tav_rows_export: index uses adopted device memory");
+        return TAV_ERR_STATE;
+    }
+    if (int rc = set_device(ix)) return rc;
+    if (int rc = wait_queued(ix)) return rc;  // the peers read the rows as the calls so far leave them
+    RowsRecord rec;
+    memset(&rec, 0, sizeof(rec));
+    rec.rows = ix->size;
+    rec.dim = ix->dim;
+    rec.dtype = ix->dtype;
+    if (ix->rows && ix->size > 0) {
+        TAV_CUDA(cudaIpcGetMemHandle(&rec.handle, ix->rows));
+        rec.has_handle = 1;
+    }
+    memcpy(handle_out, &rec, sizeof(rec));
+    if (rows_out) *rows_out = ix->size;
+    return TAV_OK;
+}
+
+int tav_rows_stage(tav_index* ix, int world, int rank, const void* handles, int n_parts, const int32_t* part_src_rank,
+                   const int64_t* part_first, const int64_t* part_rows, float* mirror_out, void* stream) {
+    if (!ix || world < 1 || rank < 0 || rank >= world || n_parts < 0 || (world > 1 && !handles) ||
+        (n_parts > 0 && (!part_src_rank || !part_first || !part_rows))) {
+        set_error("tav_rows_stage: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (ix->adopted) {
+        set_error("tav_rows_stage: index uses adopted device memory");
+        return TAV_ERR_STATE;
+    }
+    if (ix->staged) {
+        set_error("tav_rows_stage: rows are already staged (tav_rows_commit first)");
+        return TAV_ERR_STATE;
+    }
+    if (mirror_out && (ix->dtype != TAV_F32 || (ix->flags & TAV_NORMALIZE))) {
+        set_error("tav_rows_stage: the rows read back equal the appended ones only on a float32 index without "
+                  "TAV_NORMALIZE");
+        return TAV_ERR_INVALID;
+    }
+    std::vector<RowsRecord> recs(static_cast<size_t>(world));
+    if (world > 1) memcpy(recs.data(), handles, recs.size() * sizeof(RowsRecord));
+    int64_t total = 0;
+    for (int i = 0; i < n_parts; ++i) {
+        const int src = part_src_rank[i];
+        if (src < 0 || src >= world) {
+            set_error("tav_rows_stage: piece %d names rank %d of %d", i, src, world);
+            return TAV_ERR_INVALID;
+        }
+        const int64_t have = src == rank ? ix->size : recs[src].rows;
+        const bool mapped = src == rank || recs[src].has_handle;
+        if (src != rank && part_rows[i] > 0 && (recs[src].dim != ix->dim || recs[src].dtype != ix->dtype)) {
+            set_error("tav_rows_stage: rank %d holds rows of %d elements of dtype %d, this index %d of dtype %d", src,
+                      recs[src].dim, recs[src].dtype, ix->dim, ix->dtype);
+            return TAV_ERR_INVALID;
+        }
+        if (part_first[i] < 0 || part_rows[i] < 0 || part_rows[i] > have - part_first[i] ||
+            (part_rows[i] > 0 && !mapped)) {
+            set_error("tav_rows_stage: piece %d, rows [%lld, %lld) of rank %d, is outside its %lld rows", i,
+                      (long long)part_first[i], (long long)(part_first[i] + part_rows[i]), src, (long long)have);
+            return TAV_ERR_RANGE;
+        }
+        total += part_rows[i];
+    }
+    const size_t row = static_cast<size_t>(ix->dim) * dtype_size(ix->dtype);
+    const size_t bytes = std::max<size_t>(static_cast<size_t>(total) * row, 256);
+    if (ix->stage_cap >= 0 && bytes > static_cast<size_t>(ix->stage_cap)) {
+        set_error("tav_rows_stage: %zu bytes for the new block exceed the stage cap of %lld", bytes,
+                  (long long)ix->stage_cap);
+        return TAV_ERR_OOM;
+    }
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = enter_stream(ix, s)) return rc;
+    // the rows are about to be replaced: the outstanding deferred searches' exact redo reads them
+    if (int rc = finish_pending(ix, s, nullptr)) return rc;
+    void* fresh = nullptr;
+    cudaError_t e = rows_malloc(&fresh, bytes);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        set_error("tav_rows_stage: cannot allocate %zu bytes for the new block: %s", bytes, cudaGetErrorString(e));
+        return e == cudaErrorMemoryAllocation ? TAV_ERR_OOM : TAV_ERR_CUDA;
+    }
+    // destination order; TAV_REBALANCE_MUTANT 1 lays the first two pieces out swapped (the same bytes in all)
+    std::vector<int> order(static_cast<size_t>(n_parts));
+    for (int i = 0; i < n_parts; ++i) order[i] = i;
+    if (TAV_REBALANCE_MUTANT == 1 && n_parts >= 2) std::swap(order[0], order[1]);
+    {
+        PeerMappings peers(world);
+        int64_t dst = 0;
+        for (int j = 0; j < n_parts && e == cudaSuccess; ++j) {
+            const int i = order[j];
+            const int src = part_src_rank[i];
+            if (part_rows[i] == 0) continue;
+            const char* base = static_cast<const char*>(ix->rows);
+            if (src != rank) {
+                if (!peers.base[src]) {
+                    e = cudaIpcOpenMemHandle(&peers.base[src], recs[src].handle, cudaIpcMemLazyEnablePeerAccess);
+                    if (e != cudaSuccess) {
+                        peers.base[src] = nullptr;
+                        break;
+                    }
+                }
+                base = static_cast<const char*>(peers.base[src]);
+            }
+            // across GPUs the copy engines move the piece over NVLink; on one GPU it is a device-to-device copy
+            e = cudaMemcpyAsync(static_cast<char*>(fresh) + static_cast<size_t>(dst) * row,
+                                base + static_cast<size_t>(part_first[i]) * row, static_cast<size_t>(part_rows[i]) * row,
+                                cudaMemcpyDefault, s);
+            dst += part_rows[i];
+        }
+        if (e == cudaSuccess && mirror_out && total > 0)
+            e = cudaMemcpyAsync(mirror_out, fresh, static_cast<size_t>(total) * row, cudaMemcpyDeviceToHost, s);
+        // before the mappings close, also after a failure: no queued copy may still read a peer's rows
+        const cudaError_t se = cudaStreamSynchronize(s);
+        if (e == cudaSuccess) e = se;
+    }
+    if (e != cudaSuccess) {
+        rows_free(fresh, bytes);
+        set_error("tav_rows_stage: copying the new block failed: %s", cudaGetErrorString(e));
+        return TAV_ERR_CUDA;
+    }
+    mark_done(ix);
+    ix->staged = fresh;
+    ix->staged_rows = total;
+    ix->staged_bytes = bytes;
+    return TAV_OK;
+}
+
+int tav_rows_commit(tav_index* ix, int commit) {
+    if (!ix || (commit != 0 && commit != 1)) return TAV_ERR_INVALID;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (int rc = set_device(ix)) return rc;
+    if (!commit) {
+        rows_free(ix->staged, ix->staged_bytes);
+        ix->staged = nullptr;
+        ix->staged_rows = 0;
+        ix->staged_bytes = 0;
+        return TAV_OK;
+    }
+    if (!ix->staged) {
+        set_error("tav_rows_commit: no rows are staged");
+        return TAV_ERR_STATE;
+    }
+    if (int rc = wait_queued(ix)) return rc;  // queued searches read the old rows
+    if (TAV_REBALANCE_MUTANT != 4) rows_free(ix->rows, ix->rows_bytes);  // mutant 4 leaks the old rows
+    ix->rows = ix->staged;
+    ix->rows_bytes = ix->staged_bytes;
+    ix->size = ix->capacity = ix->staged_rows;
+    ix->staged = nullptr;
+    ix->staged_rows = 0;
+    ix->staged_bytes = 0;
+    // every row may have changed: the planes are rebuilt from row 0, which also resets their overflow flag
+    ix->split_rows = TAV_REBALANCE_MUTANT == 2 ? std::min(ix->split_rows, ix->size) : 0;
+    ix->split_recheck = false;
+    if (TAV_REBALANCE_MUTANT != 3) ix->row_mask_rows = 0;  // ordinals changed meaning
+    ix->qmask_n = 0;
     return TAV_OK;
 }
 

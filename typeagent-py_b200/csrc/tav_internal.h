@@ -323,6 +323,21 @@ extern "C" const int* tav_internal_split_flag(tav_index* ix);
 // 2 in place, and the number of windows.  Tests use them to reach both paths on small indexes.
 extern "C" int tav_internal_compact_policy(tav_index* ix, int mode, int64_t scratch_bytes);
 extern "C" int tav_internal_compact_stats(tav_index* ix, int* path, int64_t* windows);
+// library-internal: the largest allocation tav_rows_stage may make on this index, in bytes (-1: no cap).  A
+// stage above it gives TAV_ERR_OOM as a failed cudaMalloc would; tests use it to reach that path.
+extern "C" int tav_internal_stage_cap(tav_index* ix, int64_t max_bytes);
+// library-internal: bytes of this index's library-owned row allocation and staged block, and bytes held in such row
+// blocks by every index of the process.  Tests use it to see that a rebalance frees the block it replaced.
+extern "C" int tav_internal_row_bytes(tav_index* ix, int64_t* index_bytes, int64_t* process_bytes);
+
+// TAV_REBALANCE_MUTANT (tests only, never set by build.py): 1..3 compile one deliberate defect each into the
+// rebalance (tav_rows_stage / tav_rows_commit), so that tests/test_gpu_rebalance.py can show its exact checks catch
+// it: 1 the first two pieces of a stage are laid out in swapped order, 2 the fp16 planes of a float32 index are kept
+// at commit, 3 the row mask is kept at commit, 4 the old rows are not freed at commit.  No variant reads or writes
+// outside an allocation.
+#ifndef TAV_REBALANCE_MUTANT
+#define TAV_REBALANCE_MUTANT 0
+#endif
 
 namespace tav {
 

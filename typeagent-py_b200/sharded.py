@@ -38,6 +38,7 @@ offsets) is testable on CPU with the ``gloo`` backend.
 from __future__ import annotations
 
 import ctypes as C
+import operator
 from array import array as _array
 
 import numpy as np
@@ -56,6 +57,48 @@ def shard_bounds(n_rows: int, world: int) -> list[tuple[int, int]]:
     """Rank g owns rows [g*ceil(N/G), (g+1)*ceil(N/G)) clipped to N."""
     per = -(-n_rows // world) if world > 0 else 0
     return [(min(g * per, n_rows), min((g + 1) * per, n_rows)) for g in range(world)]
+
+
+def rebalance_starts(n_rows: int, world: int, sizes=None) -> list[int]:
+    """Block starts [world + 1] of a rebalance to ``shard_bounds(n_rows, world)``, or to blocks of ``sizes`` rows
+    (``world`` non-negative integers summing to ``n_rows``; ValueError otherwise)."""
+    if sizes is None:
+        bounds = shard_bounds(n_rows, world)
+        return [lo for lo, _ in bounds] + [n_rows]
+    try:
+        counts = [operator.index(s) for s in sizes]
+    except TypeError:
+        raise ValueError("sizes must be integers") from None
+    if len(counts) != world:
+        raise ValueError(f"sizes has {len(counts)} entries for {world} ranks")
+    if any(c < 0 for c in counts):
+        raise ValueError(f"sizes must not be negative: {counts}")
+    if sum(counts) != n_rows:
+        raise ValueError(f"sizes sum to {sum(counts)}, not to the {n_rows} rows")
+    return [0] + np.cumsum(counts, dtype=np.int64).tolist()
+
+
+def rebalance_plan(old_starts, new_starts) -> list[tuple[int, int, int, int]]:
+    """Which rows a rebalance moves: pieces (destination rank, source rank, first row within the source's block,
+    rows), destination by destination and, within one, in global row order, so that each rank's pieces laid out
+    one after another are its new block.  Blocks are contiguous and ordered, so a (source, destination) pair
+    has at most one piece."""
+    world = len(old_starts) - 1
+    if len(new_starts) != world + 1 or old_starts[-1] != new_starts[-1]:
+        raise ValueError("old and new blocks must cover the same rows with the same number of ranks")
+    plan = []
+    for dst in range(world):
+        lo, hi = new_starts[dst], new_starts[dst + 1]
+        for src in range(world):
+            a, b = max(lo, old_starts[src]), min(hi, old_starts[src + 1])
+            if b > a:
+                plan.append((dst, src, a - old_starts[src], b - a))
+    return plan
+
+
+# rows of one (source, destination) pair per round of the float32 mirror exchange of a rebalance: bounds the
+# exchange's buffers on the communication device
+MIRROR_ROUND_BYTES = 256 << 20
 
 
 def packed_layout(n_queries: int, k: int) -> tuple[int, int, int]:
@@ -189,6 +232,53 @@ class CudaShardEngine:
 
     def remove_rows(self, local_ordinals: np.ndarray) -> None:
         self.base.remove_embeddings(local_ordinals)
+
+    # ---- rebalance (per-rank steps; ShardedVectorBase.rebalance runs the protocol) ------------------------
+    def rows_adopted(self) -> bool:
+        """The rows are caller-owned device memory (``adopt_tensor``): they cannot be handed out or replaced."""
+        return self.base._adopted_tensor is not None
+
+    def rows_export(self) -> bytes:
+        """This rank's record for the peers (``tav_rows_export``), after the device rows caught up with the mirror."""
+        lib, ix = self.base._ensure_device()
+        rec = C.create_string_buffer(lib.tav_rows_handle_bytes())
+        _capi.check(lib.tav_rows_export(ix, rec, None))
+        return bytes(rec.raw)
+
+    def mirror_from_rows(self) -> bool:
+        """The device rows equal the float32 mirror bit for bit (float32 storage, not normalised): the new
+        mirror is read back from the staged rows instead of being exchanged."""
+        return self.base._storage_dtype == "float32" and not self.base._normalize
+
+    def local_rows(self) -> np.ndarray:
+        return self.base.serialize()
+
+    def rows_stage(self, records: list[bytes], pieces: list[tuple[int, int, int]], rank: int, dim: int):
+        """``tav_rows_stage`` of this rank's new block from ``pieces`` [(source rank, first row of its block, rows)]
+        in order; returns the staged rows read back as the new mirror (``mirror_from_rows``) or None."""
+        lib, ix = self.base._ensure_device()
+        if lib.tav_dim(ix) == 0:  # a rank that never held a row learns the width (an empty append)
+            _capi.check(lib.tav_append(ix, None, 0, dim, _capi.TAV_F32, 0, None))
+        src = np.array([p[0] for p in pieces], np.int32)
+        first = np.array([p[1] for p in pieces], np.int64)
+        rows = np.array([p[2] for p in pieces], np.int64)
+        mirror = np.empty((int(rows.sum()), dim), np.float32) if self.mirror_from_rows() else None
+        stream = self.torch.cuda.current_stream(self.device).cuda_stream
+        _capi.check(lib.tav_rows_stage(ix, len(records), rank, b"".join(records), len(pieces),
+                                       src.ctypes.data_as(C.c_void_p), first.ctypes.data_as(C.c_void_p),
+                                       rows.ctypes.data_as(C.c_void_p),
+                                       None if mirror is None else mirror.ctypes.data_as(C.c_void_p),
+                                       C.c_void_p(stream)))
+        return mirror
+
+    def rows_commit(self, commit: bool, mirror: np.ndarray | None = None) -> None:
+        """Swap in the staged rows and ``mirror`` as the host mirror (``commit``), or drop them."""
+        lib, ix = _capi.load(), self.base._ix
+        if ix is None:
+            return
+        _capi.check(lib.tav_rows_commit(ix, int(commit)))
+        if commit:
+            self.base._replace_rebalanced(mirror)
 
     def finish(self) -> int:
         return self.base.finish_search()
@@ -595,12 +685,19 @@ class ShardedVectorBase:
 
     def __init__(self, settings: TextEmbeddingIndexSettings, *, process_group=None,
                  device: int | None = None, storage_dtype: str = "float32", engine=None,
-                 exchange: str = "peer"):
+                 exchange: str = "peer", rebalance_at: float | None = None):
+        """``rebalance_at``: when set (at least 1), ``add_embeddings`` and ``remove_embeddings`` call ``rebalance()``
+        whenever the largest block holds more than ``rebalance_at`` times the even share (rows / ranks).  A rebalance
+        holds each rank's new block beside its old one until it commits, so the bound must fire while the fullest
+        GPU still has room for an even share more."""
         import torch.distributed as dist
 
         if exchange not in ("peer", "nccl"):
             raise ValueError("exchange must be 'peer' or 'nccl'")
+        if rebalance_at is not None and not rebalance_at >= 1.0:
+            raise ValueError(f"rebalance_at must be at least 1, not {rebalance_at}")
         self.exchange = exchange
+        self.rebalance_at = rebalance_at
         self.settings = settings
         self._dist = dist
         self._group = process_group
@@ -629,6 +726,11 @@ class ShardedVectorBase:
     @property
     def local_range(self) -> tuple[int, int]:
         return self._starts[self.rank], self._starts[self.rank + 1]
+
+    @property
+    def blocks(self) -> list[tuple[int, int]]:
+        """Every rank's block of global rows, [(lo, hi)] in rank order (the same on every rank)."""
+        return [(self._starts[r], self._starts[r + 1]) for r in range(self.world)]
 
     def _set_bounds(self, bounds) -> None:
         self._starts = [lo for lo, _ in bounds] + [bounds[-1][1]]
@@ -663,8 +765,13 @@ class ShardedVectorBase:
             self._engine.adopt_tensor(rows)
 
     def add_embeddings(self, keys, embeddings: np.ndarray) -> None:
-        """Append rows (global ordinals continue at len(self)); they join the LAST rank's
-        block so that blocks stay contiguous and ordered.  ``rebalance`` evens blocks out."""
+        """Append rows (global ordinals continue at len(self)); they join the LAST rank's block so that blocks stay
+        contiguous and ordered.  ``rebalance()`` moves rows between ranks so that every block is its even share
+        again; with ``rebalance_at`` set, this call does so when the last block grew past that bound.  If that
+        rebalance fails (MemoryError when a rank cannot hold its new block beside its old one, for one), this call
+        raises on every rank AFTER the rows were appended: they are in the index, with their ordinals, and the
+        blocks stay as they were; do not append them again.  The next append or removal tries the rebalance
+        again."""
         if embeddings.ndim != 2:
             raise ValueError(f"Expected 2D embeddings array, got {embeddings.ndim}D")
         if self._embedding_size == 0:
@@ -678,6 +785,7 @@ class ShardedVectorBase:
         if keys is not None:
             for key, row in zip(keys, embeddings):
                 self.settings.embedding_model.add_embedding(key, row)
+        self._rebalance_if_skewed()
 
     def remove_embeddings(self, ordinals) -> None:
         """Remove rows by global ordinal, as ``VectorBase.remove_embeddings`` does on one GPU (``np.delete``
@@ -686,7 +794,9 @@ class ShardedVectorBase:
         (``finish()``, collective): the local removal redoes their flagged queries on the old rows, and only
         ``finish()`` exchanges and merges the corrected candidates again.  Each rank then removes its own block's
         share and recomputes the block starts from the replicated list, without a collective; blocks may become
-        uneven (a block may empty)."""
+        uneven (a block may empty) until ``rebalance()``, which this call runs when ``rebalance_at`` says so.  If
+        that rebalance fails, this call raises on every rank AFTER the rows were removed; the blocks stay as they
+        were, and the next append or removal tries again."""
         removed = removal_ordinals(ordinals, len(self))
         if removed.size == 0:
             return
@@ -698,6 +808,133 @@ class ShardedVectorBase:
         starts = np.asarray(self._starts, np.int64)
         self._starts = (starts - np.searchsorted(removed, starts, side="left")).tolist()
         self._generation += 1
+        self._rebalance_if_skewed()
+
+    # ---- rebalance -----------------------------------------------------------------------
+    def _rebalance_if_skewed(self) -> None:
+        if self.rebalance_at is None or len(self) == 0:
+            return
+        largest = max(hi - lo for lo, hi in self.blocks)
+        if largest * self.world > self.rebalance_at * len(self):
+            self.rebalance()
+
+    def rebalance(self, sizes=None) -> int:
+        """Move rows between ranks so that rank r holds ``shard_bounds(len(self), world)[r]``, or, with ``sizes``
+        (one non-negative integer per rank, summing to ``len(self)``), that many rows, blocks contiguous and in
+        rank order.  Returns the number of rows that changed rank, the same on every rank.  Collective and SPMD.
+
+        Global ordinals do not change, so every lookup returns what it returned before.  Nothing happens, and no
+        collective runs, when the blocks already are the target.  Invalid ``sizes`` raise ValueError on every rank
+        before any collective.  Deferred lookups are finished first (``finish()``).  Each rank then copies its new
+        block, in the storage dtype and byte for byte, from its own rows and its peers' (CUDA IPC, the copy
+        engines); the float32 host mirrors follow, read back from the new rows or exchanged over the process
+        group.  If any rank fails (an allocation, a copy, rows that are adopted device memory), every rank raises
+        (MemoryError for a failed allocation) and nothing changes anywhere.  Until it commits, each rank holds its
+        new block (device memory for its new row count) beside its old one."""
+        target = rebalance_starts(len(self), self.world, sizes)
+        if target == list(self._starts):
+            return 0
+        plan = rebalance_plan(self._starts, target)
+        moved = sum(n for dst, src, _, n in plan if dst != src)
+        self.finish()
+        engine = self._engine
+        # every rank's record of its rows, with a status: 0 fine, 1 adopted rows, 2 failed
+        status, record, error = 0, b"", None
+        try:
+            if engine.rows_adopted():
+                status = 1
+            else:
+                record = engine.rows_export()
+        except Exception as e:  # noqa: BLE001
+            status, error = 2, e
+        got = [(status, record)]
+        if self.world > 1:
+            got = [None] * self.world
+            self._dist.all_gather_object(got, (status, record), group=self._group)
+        adopted = [r for r, (st, _) in enumerate(got) if st == 1]
+        if adopted:
+            raise RuntimeError(f"rebalance: the rows of rank(s) {adopted} are adopted device memory "
+                               "(from_device_tensor / load_local_shard with a tensor) and cannot move")
+        if any(st for st, _ in got):
+            raise error if error is not None else RuntimeError("rebalance: another rank failed to export its rows")
+        error, mirror = None, None
+        try:
+            mirror = engine.rows_stage([rec for _, rec in got], [(src, first, n) for dst, src, first, n in plan
+                                                                 if dst == self.rank],
+                                       self.rank, self._embedding_size)
+        except Exception as e:  # noqa: BLE001
+            error = e
+        code = 0
+        if not engine.mirror_from_rows():
+            # the mirror exchange is a collective: the ranks agree first that every one of them can enter it
+            code = self._worst_status(error)
+            if code == 0:
+                try:
+                    mirror = self._exchange_mirror(plan)
+                except Exception as e:  # noqa: BLE001
+                    error = e
+        if code == 0:
+            code = self._worst_status(error)
+        if code:
+            engine.rows_commit(False)
+            if error is not None:
+                raise error
+            raise (MemoryError if code == 2 else RuntimeError)("rebalance: another rank failed; nothing was moved")
+        engine.rows_commit(True, mirror)
+        self._starts = list(target)
+        self._generation += 1
+        return moved
+
+    def _worst_status(self, error) -> int:
+        """Every rank's status, agreed by one all-reduce (max): 0 fine, 1 failed, 2 out of memory."""
+        code = 0 if error is None else 2 if isinstance(error, MemoryError) else 1
+        if self.world == 1:
+            return code
+        import torch
+        from torch.distributed import ReduceOp
+
+        dev = self._engine.comm_device() if hasattr(self._engine, "comm_device") else torch.device("cpu")
+        word = torch.tensor([code], dtype=torch.int64, device=dev)
+        self._dist.all_reduce(word, op=ReduceOp.MAX, group=self._group)
+        return int(word.item())
+
+    def _exchange_mirror(self, plan) -> np.ndarray:
+        """This rank's new float32 host mirror: its kept rows, and the moving pieces from their ranks' mirrors
+        through ``all_to_all_single`` on the communication device, in rounds of at most ``MIRROR_ROUND_BYTES``
+        per pair of ranks."""
+        import torch
+
+        d = self._embedding_size
+        mine = self._engine.local_rows()
+        dev = torch.device("cpu")  # gloo moves device tensors through host memory anyway
+        if hasattr(self._engine, "comm_device") and self._dist.get_backend(self._group) != "gloo":
+            dev = self._engine.comm_device()
+        send = {dst: (first, n) for dst, src, first, n in plan if src == self.rank and dst != self.rank}
+        recv = {src: n for dst, src, _, n in plan if dst == self.rank and src != self.rank}
+        parts = {src: [] for src in recv}
+        per_round = max(1, MIRROR_ROUND_BYTES // (4 * max(d, 1)))
+        rounds = -(-max([n for dst, src, _, n in plan if dst != src], default=0) // per_round)
+        for r in range(rounds):
+            a = r * per_round
+            out_sizes = [max(0, min(recv.get(src, 0) - a, per_round)) for src in range(self.world)]
+            in_sizes = [max(0, min(send.get(dst, (0, 0))[1] - a, per_round)) for dst in range(self.world)]
+            chunks = [mine[send[dst][0] + a: send[dst][0] + a + in_sizes[dst]] for dst in range(self.world)
+                      if in_sizes[dst]]
+            data = np.concatenate(chunks) if chunks else np.zeros((0, d), np.float32)
+            inp = torch.from_numpy(np.ascontiguousarray(data, np.float32)).to(dev)
+            out = torch.empty((sum(out_sizes), d), dtype=torch.float32, device=dev)
+            self._dist.all_to_all_single(out, inp, out_sizes, in_sizes, group=self._group)
+            host = out.cpu().numpy()
+            at = 0
+            for src in range(self.world):
+                if out_sizes[src]:
+                    parts[src].append(host[at: at + out_sizes[src]])
+                    at += out_sizes[src]
+        rows = []
+        for dst, src, first, n in plan:
+            if dst == self.rank:
+                rows.append(mine[first: first + n] if src == self.rank else np.concatenate(parts[src]))
+        return np.concatenate(rows) if rows else np.zeros((0, d), np.float32)
 
     # ---- lookups -----------------------------------------------------------------------
     def _gather_and_merge(self, local, b: int, k: int):

@@ -356,6 +356,23 @@ class VectorBase:
         self._qmask_ref = None
         self._predicate_masks.clear()
 
+    def _replace_rebalanced(self, rows: np.ndarray) -> None:
+        """The host mirror becomes ``rows`` (float32 [n, D]) after the device rows were replaced by the same rows
+        (``tav_rows_commit``).  The generation is kept: the device already holds them, and a new generation would
+        upload them all again.  Row masks and cached predicate masks are dropped: ordinals changed meaning."""
+        rows = np.ascontiguousarray(rows, dtype=np.float32)
+        if self._embedding_size == 0 and rows.ndim == 2 and rows.shape[1] > 0:
+            self._embedding_size = rows.shape[1]
+        self._buf = rows
+        self._buf_is_callers = False
+        self._count = len(rows)
+        self._ix_rows = len(rows)
+        self._mask_key = None
+        self._mask_ref = None
+        self._qmask_key = None
+        self._qmask_ref = None
+        self._predicate_masks.clear()
+
     def remove_embedding_at(self, pos: int) -> None:
         if not 0 <= pos < len(self):
             raise IndexError(f"Index {pos} out of bounds for embedding index of size {len(self)}")
