@@ -55,7 +55,8 @@ enum tav_status {
     TAV_ERR_CUDA = -2,    /* CUDA runtime / driver failure, or no device  (RuntimeError) */
     TAV_ERR_OOM = -3,     /* device or pinned-host allocation failed      (MemoryError) */
     TAV_ERR_RANGE = -4,   /* ordinal out of range                         (IndexError) */
-    TAV_ERR_STATE = -5    /* operation not valid in this state (e.g. append to adopted memory) */
+    TAV_ERR_STATE = -5,   /* operation not valid in this state (e.g. append to adopted memory) */
+    TAV_ERR_PEER = -6     /* a sharded search failed on another rank (tav_sharded_*)     (RuntimeError) */
 };
 
 /* tav_create flags */
@@ -340,7 +341,30 @@ int tav_merge_range(int device, int n_lists, int n_queries, const int64_t* offse
  * replicated on every rank.  With TAV_DEFER_RETRY in `flags` up to `depth` searches may be
  * outstanding before tav_sharded_finish, which also agrees, across ranks, which of them had a query
  * redone exactly by some rank, and repeats the exchange for exactly those (their output buffers must
- * stay valid until then).
+ * stay valid until then), each merged again in the order it was first merged in.  A deferred search
+ * beyond `depth`: TAV_ERR_STATE; a synchronous one finishes the open ones first.
+ *
+ * tav_sharded_search also takes TAV_USE_ROW_MASK, TAV_USE_QUERY_MASKS (each rank's masks cover its own
+ * rows, set with tav_set_row_mask / tav_set_query_masks) and TAV_TIES_LOW_FIRST, which merges with
+ * order 1 of tav_merge_topk_ordered (the lists come in rank order, each rank's block in ascending rows).
+ *
+ * tav_sharded_search_subset: the subset forms.  `subset` holds this rank's BLOCK-LOCAL host ordinals
+ * (subset_len of them).  offsets == NULL: one subset shared by every query, searched as tav_search
+ * with a subset; otherwise host int64 [n_queries + 1] CSR offsets of per-query subsets (offsets[0] == 0,
+ * offsets[n_queries] == subset_len), searched as tav_search_subsets, which synchronises `stream` once.
+ * The local search runs with TAV_ITEMS_AS_POSITIONS into this rank's slot, and tav_map_items through
+ * `positions_device` (device int64 [subset_len]: where each entry stands in the caller's whole list, or
+ * in the concatenation of the per-query lists) makes them global positions before the publish.  The
+ * merge is by position, order 2 (3 with TAV_TIES_LOW_FIRST): the outputs are global positions, decoded
+ * by the caller (tav_map_items through its list).  A rank without a share passes subset_len 0.  Other
+ * accepted flags: TAV_DEFER_RETRY, TAV_FORCE_SCAN (shared subset only).
+ *
+ * Failures.  A sharded search that fails on a rank's host side (a local error other than TAV_ERR_CUDA:
+ * an invalid argument, a missing mask, an allocation) still publishes an empty list with a status word
+ * set, and returns that rank's own error; every rank's merge adds up the status words, and every other
+ * rank gets TAV_ERR_PEER: on return for a synchronous call, from tav_sharded_finish for a deferred one
+ * (which still completes every open search and its repairs).  A local TAV_ERR_CUDA is not published
+ * (the device may be unusable): the peers' merges then wait about 4 s and trap.
  */
 typedef struct tav_group tav_group;
 int tav_group_handle_bytes(void);
@@ -352,6 +376,10 @@ int tav_group_destroy(tav_group* g);
 int tav_sharded_search(tav_index* ix, tav_group* g, const float* queries_device, int n_queries, int k,
                        float min_score, int flags, int64_t item_offset, int64_t* out_items, float* out_scores,
                        int32_t* out_counts, void* stream);
+int tav_sharded_search_subset(tav_index* ix, tav_group* g, const float* queries_device, int n_queries, int k,
+                              float min_score, int flags, const int64_t* subset, int64_t subset_len,
+                              const int64_t* offsets, const int64_t* positions_device, int64_t* out_items,
+                              float* out_scores, int32_t* out_counts, void* stream);
 int tav_sharded_finish(tav_index* ix, tav_group* g, void* stream, int* redone_total);
 
 /*

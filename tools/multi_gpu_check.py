@@ -12,7 +12,11 @@ float32 split form and the bf16 / fp16 tensor-core paths, and agrees with the CP
 threshold search (``search_range``: offsets and hits all-gathered, ``tav_merge_range``) must equal the
 single-GPU ``search_range`` bit for bit on every rank: float32 row scan, bf16 tensor cores, float32 split form.
 Filtered and subset lookups (row masks, predicates, subsets; top-k and threshold) must equal the single-GPU
-``VectorBase`` bit for bit on every rank.
+``VectorBase`` bit for bit on every rank.  The same filtered, per-query-mask and per-query-subset top-k lookups go
+through the peer exchange (``tav_sharded_search`` / ``tav_sharded_search_subset``) with ``exchange="peer"``, also
+deferred on the device (``search_tensors(..., defer_check=True)`` and one ``finish()``), and through the NCCL
+exchange with ``exchange="nccl"``: both must equal the single-GPU lookup.  These peer-exchange cases have not been
+run on two or more GPUs.
 """
 import os
 import sys
@@ -119,7 +123,8 @@ def main():
             print(f"multi-gpu ok: world={world} search_range {storage} n={n} d={d} b={b} min_score={ms} path={path} "
                   f"hits={int(want[0][-1])}", flush=True)
     # filtered and subset lookups (row masks, predicates, subsets with duplicates and negative ordinals): equal to
-    # the single-GPU VectorBase bit for bit on every rank, over the process group whatever `exchange` says
+    # the single-GPU VectorBase bit for bit on every rank (top-k through the peer exchange, the default; threshold
+    # searches over the process group)
     for storage, n, d, b in (("float32", 50001, 96, 6), ("bfloat16", 120001, 128, 24)):
         v, q = O.make_corpus(n, d, seed=n + 2, n_queries=b)
         v[n // 2: n // 2 + 500] = v[:500]  # equal scores on different ranks
@@ -159,10 +164,32 @@ def main():
                 for g, w in zip(got, want):
                     np.testing.assert_array_equal(g.view(np.uint32) if g.dtype == np.float32 else g,
                                                   w.view(np.uint32) if w.dtype == np.float32 else w)
+        # the same top-k lookups through either exchange, synchronous and deferred on the device
+        subsets = [rng.permutation(n)[: 200 + 50 * i].astype(np.int64) - (n if i % 3 == 1 else 0) for i in range(b)]
+        lookups = [dict(allowed=allowed), dict(allowed=allowed, ties_low_first=True), dict(allowed=qmasks),
+                   dict(subset=sub), dict(subset=sub, ties_low_first=True), dict(subsets=subsets),
+                   dict(subsets=subsets, ties_low_first=True)]
+        wants = [whole.search_arrays(q, 40, 0.4, **kw) for kw in lookups]
+        for exchange in ("peer", "nccl"):
+            shx = sh if exchange == "peer" else ShardedVectorBase(settings, device=local, storage_dtype=storage,
+                                                                  exchange="nccl")
+            if exchange == "nccl":
+                shx.deserialize(v)
+            outs = [shx.search_tensors(q, 40, 0.4, defer_check=True, **kw) for kw in lookups]
+            shx.finish()
+            torch.cuda.synchronize()
+            for kw, out, want in zip(lookups, outs, wants):
+                got = [t.cpu().numpy() for t in out]
+                for g, w in zip(got, want):
+                    np.testing.assert_array_equal(g.view(np.uint32) if g.dtype == np.float32 else g,
+                                                  w.view(np.uint32) if w.dtype == np.float32 else w)
+                for g, w in zip(shx.search_arrays(q, 40, 0.4, **kw), want):
+                    np.testing.assert_array_equal(g.view(np.uint32) if g.dtype == np.float32 else g,
+                                                  w.view(np.uint32) if w.dtype == np.float32 else w)
         dist.barrier()
         if rank == 0:
             print(f"multi-gpu ok: world={world} filtered, subset and per-query-mask lookups {storage} n={n} d={d} "
-                  f"b={b}", flush=True)
+                  f"b={b}, synchronous and deferred, peer and nccl exchanges", flush=True)
     dist.destroy_process_group()
 
 

@@ -23,7 +23,7 @@ TAV_USE_ROW_MASK, TAV_TIES_LOW_FIRST, TAV_NO_FUSED_SCAN, TAV_ITEMS_AS_POSITIONS 
 TAV_USE_QUERY_MASKS = 512
 ABI_VERSION = 2
 
-TAV_ERR_INVALID, TAV_ERR_CUDA, TAV_ERR_OOM, TAV_ERR_RANGE, TAV_ERR_STATE = -1, -2, -3, -4, -5
+TAV_ERR_INVALID, TAV_ERR_CUDA, TAV_ERR_OOM, TAV_ERR_RANGE, TAV_ERR_STATE, TAV_ERR_PEER = -1, -2, -3, -4, -5, -6
 
 # every symbol include/tavec.h declares: (name, restype, argtypes)
 _i64p = C.POINTER(C.c_int64)
@@ -70,6 +70,9 @@ SIGNATURES = {
     "tav_group_destroy": (C.c_int, [C.c_void_p]),
     "tav_sharded_search": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int,
                                      C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tav_sharded_search_subset": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int,
+                                            C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]),
     "tav_sharded_finish": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
     "tav_rows_handle_bytes": (C.c_int, []),
     "tav_rows_export": (C.c_int, [C.c_void_p, C.c_void_p, _i64p]),

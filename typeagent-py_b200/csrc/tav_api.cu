@@ -190,6 +190,8 @@ struct tav_index {
     size_t rows_bytes = 0;           // bytes of the library-owned allocation behind `rows` (0 when adopted)
     size_t staged_bytes = 0;
     int64_t stage_cap = -1;          // bytes, -1 = no cap (tav_internal_stage_cap)
+    int64_t qmask_cap = -1;          // bytes of per-query masks, -1 = no cap (tav_internal_qmask_cap)
+    bool alloc_fail = false;         // tensor-core searches ask cudaMalloc for too much (tav_internal_search_alloc_fail)
     // predicate pushdown: one bit per row (tav_set_row_mask)
     DevBuf row_mask;
     int64_t row_mask_rows = 0;   // 0 = no mask set
@@ -661,7 +663,8 @@ int tav_set_query_masks(tav_index* ix, const uint32_t* bits, int n_queries, int6
     const int64_t words = mask_words(n_rows);
     const size_t bytes = static_cast<size_t>(n_queries) * words * sizeof(uint32_t);
     ix->qmask_n = 0;
-    cudaError_t e = ix->qmask.ensure(bytes);
+    cudaError_t e = ix->qmask_cap >= 0 && bytes > static_cast<size_t>(ix->qmask_cap) ? cudaErrorMemoryAllocation
+                                                                                      : ix->qmask.ensure(bytes);
     if (e == cudaSuccess) e = ix->qmask_pop.ensure(static_cast<size_t>(n_queries) * sizeof(uint32_t));
     if (e != cudaSuccess) {
         cudaGetLastError();  // no sticky error: the index stays usable
@@ -1684,6 +1687,20 @@ int tav_internal_stage_cap(tav_index* ix, int64_t max_bytes) {
     return TAV_OK;
 }
 
+int tav_internal_qmask_cap(tav_index* ix, int64_t max_bytes) {
+    if (!ix || max_bytes < -1) return TAV_ERR_INVALID;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    ix->qmask_cap = max_bytes;
+    return TAV_OK;
+}
+
+int tav_internal_search_alloc_fail(tav_index* ix, int on) {
+    if (!ix) return TAV_ERR_INVALID;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    ix->alloc_fail = on != 0;
+    return TAV_OK;
+}
+
 }  // extern "C"
 
 // ---- rebalance: a rank's new block copied from the ranks' row allocations over CUDA IPC -------------------
@@ -2158,11 +2175,11 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
 
     if (use_mma) {
         ts->path = use_split ? 3 : 2;
-        if (n_queries > ix->retry_cap || !ix->retry.p) {
+        if (n_queries > ix->retry_cap || !ix->retry.p || ix->alloc_fail) {
             if (int rc = finish_pending(ix, s, nullptr)) return rc;
             const int cap = std::max(std::min(n_queries, kMmaMaxQueries), 1024);
             const size_t bytes = (static_cast<size_t>(2) * kMaxPending + static_cast<size_t>(kMaxPending) * cap) * sizeof(int32_t);
-            TAV_CUDA(ix->retry.ensure(bytes));
+            TAV_CUDA(ix->retry.ensure(ix->alloc_fail ? ~size_t(0) >> 4 : bytes));
             TAV_CUDA(cudaMemsetAsync(ix->retry.p, 0, 2 * kMaxPending * sizeof(int32_t), s));
             TAV_CUDA(ix->retry_host.ensure(2 * kMaxPending * sizeof(int32_t)));
             memset(ix->retry_host.p, 0, 2 * kMaxPending * sizeof(int32_t));

@@ -333,9 +333,11 @@ struct MergeSync {
     uint32_t* ack[16];         // ack[w]: this rank's acknowledgement word in rank w's region
     int me;
     uint32_t* ticket;          // device counter (zero on entry, self-resetting): last-CTA-done
-    const char* tails;         // slot tails of the world's lists: tails + r * slot_bytes, word 0 = "still to be corrected"
+    const char* tails;         // slot tails of the world's lists: tails + r * slot_bytes, word 0 = "still to be
+                               // corrected", word 1 = status (1: the rank's local search failed, its list is empty)
     size_t slot_bytes;
-    uint32_t* flagged_host;    // mapped pinned word receiving the world-wide sum of the tails
+    uint32_t* flagged_host;    // mapped pinned word receiving the world-wide sum of the tails' word 0
+    uint32_t* status_host;     // mapped pinned word receiving the world-wide sum of the tails' word 1
 };
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) costs a driver call; remember, per device, the

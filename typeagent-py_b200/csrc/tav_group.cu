@@ -21,14 +21,23 @@
 //                                    reads what this rank published for it)
 //   slots[depth][world][slot_bytes]   packed lists [items i64 | scores f32 | counts i32 | tail] (8-byte
 //                                    aligned sections, the layout ShardedVectorBase always used; tail word
-//                                    0 = queries the rank's exact redo will still correct at finish)
+//                                    0 = queries the rank's exact redo will still correct at finish, word 1 =
+//                                    status: 1 when the rank's local search failed and it published no hits)
 // `depth` searches may be in flight (deferred) before a rank has to wait for its peers' acks.
+//
+// Failure protocol.  A rank whose local search fails on the host side (an invalid argument, a missing mask, an
+// allocation: any status but TAV_ERR_CUDA) still publishes, an empty list with status 1, and merges, so that no
+// peer waits for it; its call returns its own error.  Every merge adds the world's status words up into a mapped
+// host word per slot, and every rank reports TAV_ERR_PEER for a search whose sum is not zero: a synchronous call
+// on return, a deferred one at tav_sharded_finish.  A CUDA error cannot be published (the device may be unusable):
+// the call returns without publishing and its peers' waits end in the ~4 s trap of spin_until.
 
 #include <stdio.h>
 #include <string.h>
 
 #include <algorithm>
 #include <new>
+#include <string>
 #include <vector>
 
 #include "tav_common.cuh"
@@ -49,11 +58,11 @@ struct PeerTable {
 // the search that used this slot `depth` searches ago.
 // The last 16 bytes of a slot are its tail: word 0 = number of this rank's queries that its exact redo
 // will still correct at finish (read here from the local search's device counters and, for a split search,
-// the index's corpus flag), exactly the number tav_finish_search will redo.
+// the index's corpus flag), exactly the number tav_finish_search will redo; word 1 = `status`.
 __global__ void __launch_bounds__(256)
 publish_kernel(PeerTable peers, int me, int world, size_t off_ack, size_t off_slot, size_t bytes, uint32_t seq,
                uint32_t need_ack, uint32_t* ticket, const int32_t* retry_totals, int n_retry, const int* corpus_flag,
-               int nq) {
+               int nq, uint32_t status) {
     __shared__ int s_last;
     const char* src = peers.region[me] + off_slot;
     if (blockIdx.x == 0 && threadIdx.x < world && threadIdx.x != me) {
@@ -83,7 +92,9 @@ publish_kernel(PeerTable peers, int me, int world, size_t off_ack, size_t off_sl
             flagged += static_cast<uint32_t>(corpus_out || __ldcg(&retry_totals[2 * i + 1]) ? slab
                                                                                           : __ldcg(&retry_totals[2 * i]));
         }
-        *reinterpret_cast<uint32_t*>(peers.region[threadIdx.x] + off_slot + bytes - 16) = TAV_GROUP_MUTANT == 1 ? 0u : flagged;
+        uint32_t* tail = reinterpret_cast<uint32_t*>(peers.region[threadIdx.x] + off_slot + bytes - 16);
+        tail[0] = TAV_GROUP_MUTANT == 1 ? 0u : flagged;
+        tail[1] = status;
     }
     // sections are padded to 16 bytes by the host side; the tail goes separately
     const size_t n16 = (bytes - 16) / 16 - (TAV_GROUP_MUTANT == 2 ? 1 : 0);
@@ -129,6 +140,7 @@ struct tav_group {
     uint32_t seq = 0;                 // searches published so far
     uint32_t* ticket = nullptr;       // device counter of the publish kernel
     uint32_t* flagged_host = nullptr; // pinned, mapped: [depth] world-wide "still to be corrected" counts per slot
+    uint32_t* status_host = nullptr;  // pinned, mapped: [depth] world-wide sums of the status words per slot
     // Deferred searches run their exchange (publish + merge) on the group's own stream, behind an event that
     // follows the local search: the next search's kernels start at once on the caller's stream and the wait
     // for the slowest rank no longer sits between two searches.  tav_sharded_finish joins the streams.
@@ -139,6 +151,8 @@ struct tav_group {
     struct OpenSearch {               // a deferred search since the last finish: what a re-merge needs
         uint32_t seq;
         int nq, k;
+        int order;                    // the merge's order (tav_merge_topk_ordered): a repair merges in it again
+        uint32_t status;              // this rank's status word (1: its local search failed)
         int64_t* items;
         float* scores;
         int32_t* counts;
@@ -199,8 +213,11 @@ int tav_group_create(int device, int rank, int world, int max_queries, int max_k
         e = cudaEventCreateWithFlags(&g->ev_local[i], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_merged[i], cudaEventDisableTiming);
     }
-    if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&g->flagged_host), 64 * sizeof(uint32_t));
-    if (e == cudaSuccess) memset(g->flagged_host, 0, 64 * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&g->flagged_host), 2 * 64 * sizeof(uint32_t));
+    if (e == cudaSuccess) {
+        memset(g->flagged_host, 0, 2 * 64 * sizeof(uint32_t));
+        g->status_host = g->flagged_host + 64;
+    }
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
     if (e != cudaSuccess) {
         set_error("tav_group_create: %s", cudaGetErrorString(e));
@@ -264,9 +281,9 @@ int tav_group_capacity(const tav_group* g, int* max_queries, int* max_k, int* de
 }
 
 // exchange + merge of the list this rank holds in its own slot for sequence number `seq`
-static int publish_and_merge(tav_group* g, int nq, int k, uint32_t seq, const int32_t* retry_totals, int n_retry,
-                             const int* corpus_flag, int64_t* out_items, float* out_scores, int32_t* out_counts,
-                             cudaStream_t s) {
+static int publish_and_merge(tav_group* g, int nq, int k, uint32_t seq, int order, uint32_t status,
+                             const int32_t* retry_totals, int n_retry, const int* corpus_flag, int64_t* out_items,
+                             float* out_scores, int32_t* out_counts, cudaStream_t s) {
     const int slot = static_cast<int>(seq % static_cast<uint32_t>(g->depth));
     size_t off_scores, off_counts, bytes;
     packed_offsets(nq, k, &off_scores, &off_counts, &bytes);
@@ -278,7 +295,8 @@ static int publish_and_merge(tav_group* g, int nq, int k, uint32_t seq, const in
         const uint32_t need_ack = seq - static_cast<uint32_t>(g->depth);
         const uint32_t need = seq > static_cast<uint32_t>(g->depth) ? need_ack : 0u;
         publish_kernel<<<grid, 256, 0, s>>>(g->peers, g->rank, g->world, g->off_ack, off_mine, bytes, seq, need,
-                                            g->ticket, retry_totals, retry_totals ? n_retry : 0, corpus_flag, nq);
+                                            g->ticket, retry_totals, retry_totals ? n_retry : 0, corpus_flag, nq,
+                                            status);
         TAVG_CUDA(cudaGetLastError());
     }
     // lists of all ranks for this slot lie side by side in MY region: strides between ranks = slot_bytes.
@@ -297,29 +315,31 @@ static int publish_and_merge(tav_group* g, int nq, int k, uint32_t seq, const in
         sync.tails = base + bytes - 16;
         sync.slot_bytes = g->slot_bytes;
         sync.flagged_host = g->flagged_host + slot;
+        sync.status_host = g->status_host + slot;
     }
-    TAVG_CUDA(launch_merge(g->world, nq, k, reinterpret_cast<const int64_t*>(base),
-                           reinterpret_cast<const float*>(base + off_scores),
-                           reinterpret_cast<const int32_t*>(base + off_counts),
-                           static_cast<int64_t>(g->slot_bytes / 8), static_cast<int64_t>(g->slot_bytes / 4),
-                           static_cast<int64_t>(g->slot_bytes / 4), out_items, out_scores, out_counts, s,
-                           g->world > 1 ? &sync : nullptr));
+    TAVG_CUDA(launch_merge_ordered(g->world, nq, k, reinterpret_cast<const int64_t*>(base),
+                                   reinterpret_cast<const float*>(base + off_scores),
+                                   reinterpret_cast<const int32_t*>(base + off_counts),
+                                   static_cast<int64_t>(g->slot_bytes / 8), static_cast<int64_t>(g->slot_bytes / 4),
+                                   static_cast<int64_t>(g->slot_bytes / 4), order, out_items, out_scores, out_counts,
+                                   s, g->world > 1 ? &sync : nullptr));
     return TAV_OK;
 }
 
-int tav_sharded_search(tav_index* ix, tav_group* g, const float* queries_device, int n_queries, int k,
-                       float min_score, int flags, int64_t item_offset, int64_t* out_items, float* out_scores,
-                       int32_t* out_counts, void* stream) {
-    if (!ix || !g || n_queries < 1 || k < 1 || !queries_device || !out_items || !out_scores || !out_counts) {
-        set_error("tav_sharded_search: invalid argument");
-        return TAV_ERR_INVALID;
-    }
+}  // extern "C"
+
+// One sharded search: `local(mine, off_scores, off_counts, &searched)` writes this rank's packed list into its
+// slot (searched = false when it wrote only zero counts and ran no search), then the list is published and merged
+// in `order`.  Argument errors come from replicated arguments and return before anything is published.
+template <typename Local>
+static int sharded_run(const char* fn, tav_index* ix, tav_group* g, int n_queries, int k, int flags, int order,
+                       Local local, int64_t* out_items, float* out_scores, int32_t* out_counts, void* stream) {
     if (!g->connected) {
-        set_error("tav_sharded_search: tav_group_connect has not run");
+        set_error("%s: tav_group_connect has not run", fn);
         return TAV_ERR_STATE;
     }
     if (n_queries > g->max_queries || k > g->max_k) {
-        set_error("tav_sharded_search: %d queries x top-%d exceed the group's capacity (%d x %d)", n_queries, k,
+        set_error("%s: %d queries x top-%d exceed the group's capacity (%d x %d)", fn, n_queries, k,
                   g->max_queries, g->max_k);
         return TAV_ERR_INVALID;
     }
@@ -329,7 +349,7 @@ int tav_sharded_search(tav_index* ix, tav_group* g, const float* queries_device,
     if (g->outstanding >= g->depth) {
         // the next sequence number's slot still belongs to the oldest open search
         if (defer) {
-            set_error("tav_sharded_search: %d deferred searches outstanding (the group's depth); call tav_sharded_finish",
+            set_error("%s: %d deferred searches outstanding (the group's depth); call tav_sharded_finish", fn,
                       g->outstanding);
             return TAV_ERR_STATE;
         }
@@ -342,23 +362,26 @@ int tav_sharded_search(tav_index* ix, tav_group* g, const float* queries_device,
     size_t off_scores, off_counts, bytes;
     packed_offsets(n_queries, k, &off_scores, &off_counts, &bytes);
     char* mine = g->region + g->off_slots + (static_cast<size_t>(slot) * g->world + g->rank) * g->slot_bytes;
-    // local search straight into this rank's slot (global ordinals through item_offset)
-    const int sflags = (flags & (TAV_FORCE_SCAN | TAV_FORCE_MMA | TAV_USE_ROW_MASK)) | TAV_QUERIES_ON_DEVICE |
-                       TAV_OUTPUTS_ON_DEVICE | TAV_DEFER_RETRY;
-    if (tav_size(ix) == 0) {
+    bool searched = false;
+    const int lrc = local(mine, off_scores, off_counts, &searched);
+    if (lrc == TAV_ERR_CUDA) {
+        --g->seq;  // nothing was published under this number (see the failure protocol above)
+        return lrc;
+    }
+    // any other failure: publish an empty list with status 1 so that no peer waits for this rank
+    std::string error;
+    if (lrc != TAV_OK) {
+        error = tav_last_error();
+        searched = false;
+        // A failed allocation (TAV_ERR_OOM from a cudaMalloc inside the local search) leaves the runtime's last
+        // error set; the publish's launch check would read it and return before the merge, which would then never
+        // acknowledge this sequence number to the peers.  Such errors are not sticky: clear it.
+        cudaGetLastError();
         TAVG_CUDA(cudaMemsetAsync(mine + off_counts, 0, static_cast<size_t>(n_queries) * 4, s));
-    } else {
-        int rc = tav_search(ix, queries_device, n_queries, k, min_score, sflags, nullptr, 0, item_offset,
-                            reinterpret_cast<int64_t*>(mine), reinterpret_cast<float*>(mine + off_scores),
-                            reinterpret_cast<int32_t*>(mine + off_counts), stream);
-        if (rc != TAV_OK) {
-            --g->seq;  // nothing was published under this number
-            return rc;
-        }
     }
     int n_retry = 0;
-    const int32_t* retry_totals = tav_size(ix) == 0 ? nullptr : tav_internal_retry_totals(ix, &n_retry);
-    const int* corpus_flag = tav_size(ix) == 0 ? nullptr : tav_internal_split_flag(ix);
+    const int32_t* retry_totals = searched ? tav_internal_retry_totals(ix, &n_retry) : nullptr;
+    const int* corpus_flag = searched ? tav_internal_split_flag(ix) : nullptr;
     // deferred (pipelined) searches: exchange on the group's stream, ordered after the local search by an event
     cudaStream_t xs = s;
     if (defer && g->world > 1) {
@@ -370,17 +393,89 @@ int tav_sharded_search(tav_index* ix, tav_group* g, const float* queries_device,
         TAVG_CUDA(cudaStreamWaitEvent(s, g->ev_merged[slot], 0));
         g->x_pending = false;
     }
-    int rc = publish_and_merge(g, n_queries, k, seq, retry_totals, n_retry, corpus_flag, out_items, out_scores,
-                               out_counts, xs);
+    const uint32_t status = lrc != TAV_OK ? 1u : 0u;
+    int rc = publish_and_merge(g, n_queries, k, seq, order, status, retry_totals, n_retry, corpus_flag, out_items,
+                               out_scores, out_counts, xs);
     if (rc != TAV_OK) return rc;
     if (xs != s) g->x_pending = true;
-    g->open.push_back({seq, n_queries, k, out_items, out_scores, out_counts});
+    g->open.push_back({seq, n_queries, k, order, status, out_items, out_scores, out_counts});
     g->outstanding += 1;
     if (!defer) {
         int redone = 0;
-        return tav_sharded_finish(ix, g, stream, &redone);
+        rc = tav_sharded_finish(ix, g, stream, &redone);
     }
-    return TAV_OK;
+    if (lrc != TAV_OK) {  // this rank's own error comes first
+        set_error("%s", error.c_str());
+        return lrc;
+    }
+    return rc;
+}
+
+extern "C" {
+
+int tav_sharded_search(tav_index* ix, tav_group* g, const float* queries_device, int n_queries, int k,
+                       float min_score, int flags, int64_t item_offset, int64_t* out_items, float* out_scores,
+                       int32_t* out_counts, void* stream) {
+    if (!ix || !g || n_queries < 1 || k < 1 || !queries_device || !out_items || !out_scores || !out_counts) {
+        set_error("tav_sharded_search: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    // local search straight into this rank's slot (global ordinals through item_offset)
+    const int sflags = (flags & (TAV_FORCE_SCAN | TAV_FORCE_MMA | TAV_USE_ROW_MASK | TAV_USE_QUERY_MASKS |
+                                 TAV_TIES_LOW_FIRST)) |
+                       TAV_QUERIES_ON_DEVICE | TAV_OUTPUTS_ON_DEVICE | TAV_DEFER_RETRY;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    auto local = [&](char* mine, size_t off_scores, size_t off_counts, bool* searched) -> int {
+        if (tav_size(ix) == 0) {
+            TAVG_CUDA(cudaMemsetAsync(mine + off_counts, 0, static_cast<size_t>(n_queries) * 4, s));
+            return TAV_OK;
+        }
+        *searched = true;
+        return tav_search(ix, queries_device, n_queries, k, min_score, sflags, nullptr, 0, item_offset,
+                          reinterpret_cast<int64_t*>(mine), reinterpret_cast<float*>(mine + off_scores),
+                          reinterpret_cast<int32_t*>(mine + off_counts), stream);
+    };
+    // lists in rank order, each rank's block in ascending rows: order 1 is the lower row first
+    return sharded_run("tav_sharded_search", ix, g, n_queries, k, flags, (flags & TAV_TIES_LOW_FIRST) ? 1 : 0, local,
+                       out_items, out_scores, out_counts, stream);
+}
+
+int tav_sharded_search_subset(tav_index* ix, tav_group* g, const float* queries_device, int n_queries, int k,
+                              float min_score, int flags, const int64_t* subset, int64_t subset_len,
+                              const int64_t* offsets, const int64_t* positions_device, int64_t* out_items,
+                              float* out_scores, int32_t* out_counts, void* stream) {
+    if (!ix || !g || n_queries < 1 || k < 1 || !queries_device || !out_items || !out_scores || !out_counts ||
+        subset_len < 0 || (subset_len > 0 && (!subset || !positions_device)) ||
+        (offsets && (offsets[0] != 0 || offsets[n_queries] != subset_len))) {
+        set_error("tav_sharded_search_subset: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    const bool ties_low = (flags & TAV_TIES_LOW_FIRST) != 0;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    auto local = [&](char* mine, size_t off_scores, size_t off_counts, bool* searched) -> int {
+        int64_t* items = reinterpret_cast<int64_t*>(mine);
+        if (tav_size(ix) == 0 || subset_len == 0) {  // no share of the subset(s) on this rank
+            TAVG_CUDA(cudaMemsetAsync(mine + off_counts, 0, static_cast<size_t>(n_queries) * 4, s));
+            return TAV_OK;
+        }
+        *searched = true;
+        const int pos = TAV_ITEMS_AS_POSITIONS | TAV_QUERIES_ON_DEVICE | TAV_OUTPUTS_ON_DEVICE |
+                        (ties_low ? TAV_TIES_LOW_FIRST : 0);
+        int rc = offsets ? tav_search_subsets(ix, queries_device, n_queries, k, min_score, pos, offsets, subset,
+                                              items, reinterpret_cast<float*>(mine + off_scores),
+                                              reinterpret_cast<int32_t*>(mine + off_counts), stream)
+                         : tav_search(ix, queries_device, n_queries, k, min_score,
+                                      pos | (flags & TAV_FORCE_SCAN) | TAV_DEFER_RETRY, subset, subset_len, 0, items,
+                                      reinterpret_cast<float*>(mine + off_scores),
+                                      reinterpret_cast<int32_t*>(mine + off_counts), stream);
+        if (rc != TAV_OK || TAV_PEER_FILTER_MUTANT == 1) return rc;
+        // positions in this rank's share -> positions in the caller's list(s), in the slot, before the publish
+        TAVG_CUDA(launch_map_items(static_cast<int64_t>(n_queries) * k, positions_device, subset_len, items, s));
+        return TAV_OK;
+    };
+    // positions are distinct across the ranks' shares: merged by position, later entry first (order 2)
+    return sharded_run("tav_sharded_search_subset", ix, g, n_queries, k, flags, ties_low ? 3 : 2, local, out_items,
+                       out_scores, out_counts, stream);
 }
 
 int tav_sharded_finish(tav_index* ix, tav_group* g, void* stream, int* redone_total) {
@@ -408,8 +503,9 @@ int tav_sharded_finish(tav_index* ix, tav_group* g, void* stream, int* redone_to
     open.swap(g->open);
     g->outstanding = 0;
     std::vector<uint32_t> flagged(open.size(), 0);
-    uint32_t total = 0;
+    uint32_t total = 0, failed = 0;
     for (size_t i = 0; i < open.size(); ++i) {
+        if (g->world > 1) failed += g->status_host[open[i].seq % static_cast<uint32_t>(g->depth)];
         // one rank: no tails were exchanged; the local redo count says "something changed", re-merge them all
         flagged[i] = g->world > 1 ? g->flagged_host[open[i].seq % static_cast<uint32_t>(g->depth)]
                                   : static_cast<uint32_t>(redone);
@@ -422,6 +518,10 @@ int tav_sharded_finish(tav_index* ix, tav_group* g, void* stream, int* redone_to
         // slot is that of an open search no younger than the one being repaired (the open searches are the last
         // `outstanding` <= depth consecutive ones) — i.e. one that is unflagged or already repaired; its peers'
         // acknowledgements are what the publish kernel waits for anyway.
+        // The repair merges in the search's own order, but only order-0 searches can be flagged today: a flag
+        // comes from the tensor-core path, which takes neither a subset nor TAV_TIES_LOW_FIRST.  A flagged subset
+        // search would also need more than a re-merge: the redo writes block-local positions into the slot, and
+        // nothing here maps them through the search's positions (tav_map_items) again.
         for (size_t i = 0; i < open.size(); ++i) {
             if (flagged[i] == 0) continue;
             const tav_group::OpenSearch& o = open[i];
@@ -435,12 +535,18 @@ int tav_sharded_finish(tav_index* ix, tav_group* g, void* stream, int* redone_to
                 char* to = g->region + g->off_slots + (static_cast<size_t>(new_slot) * g->world + g->rank) * g->slot_bytes;
                 TAVG_CUDA(cudaMemcpyAsync(to, from, bytes, cudaMemcpyDeviceToDevice, s));
             }
-            rc = publish_and_merge(g, o.nq, o.k, seq, nullptr, 0, nullptr, o.items, o.scores, o.counts, s);
+            rc = publish_and_merge(g, o.nq, o.k, seq, o.order, o.status, nullptr, 0,
+                                   nullptr, o.items, o.scores, o.counts, s);
             if (rc != TAV_OK) return rc;
         }
         TAVG_CUDA(cudaStreamSynchronize(s));
     }
     if (redone_total) *redone_total = static_cast<int>(total);
+    if (failed) {
+        set_error("tav_sharded_finish: a rank's local search failed (%u failures among the %zu searches finished); "
+                  "their results are not valid", failed, open.size());
+        return TAV_ERR_PEER;
+    }
     return TAV_OK;
 }
 

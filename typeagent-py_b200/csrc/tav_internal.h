@@ -198,12 +198,13 @@ cudaError_t launch_fold_groups(int n_queries, int k, const int32_t* row_to_group
 cudaError_t launch_merge(int n_lists, int n_queries, int k, const int64_t* items,
                          const float* scores, const int32_t* counts, int64_t items_stride,
                          int64_t scores_stride, int64_t counts_stride, int64_t* out_items,
-                         float* out_scores, int32_t* out_counts, cudaStream_t s, const MergeSync* sync = nullptr);
-// the same merge with tav_merge_topk_ordered's `order` (0..3) among equal scores
+                         float* out_scores, int32_t* out_counts, cudaStream_t s);
+// the same merge with tav_merge_topk_ordered's `order` (0..3) among equal scores; with `sync` the fused wait /
+// merge / acknowledge of the peer exchange (tav_group.cu)
 cudaError_t launch_merge_ordered(int n_lists, int n_queries, int k, const int64_t* items, const float* scores,
                                  const int32_t* counts, int64_t items_stride, int64_t scores_stride,
                                  int64_t counts_stride, int order, int64_t* out_items, float* out_scores,
-                                 int32_t* out_counts, cudaStream_t s);
+                                 int32_t* out_counts, cudaStream_t s, const MergeSync* sync = nullptr);
 // in place: items[i] = table[items[i]] where 0 <= items[i] < table_len
 cudaError_t launch_map_items(int64_t n, const int64_t* table, int64_t table_len, int64_t* items, cudaStream_t s);
 
@@ -222,6 +223,15 @@ cudaError_t launch_map_items(int64_t n, const int64_t* table, int64_t table_len,
 // list there.  Every wait of the protocol stays satisfiable: the results are wrong, nothing spins out.
 #ifndef TAV_GROUP_MUTANT
 #define TAV_GROUP_MUTANT 0
+#endif
+
+// TAV_PEER_FILTER_MUTANT (tests only, never set by build.py): 1..2 compile one deliberate defect each into the
+// filtered and subset searches of the peer exchange, so that tests/test_gpu_peer_filtered.py can show its checks
+// catch it: 1 a subset search publishes its share's positions without mapping them to the caller's list
+// (tav_map_items), 2 the merge ignores the slot tails' status words (a peer's failure is not reported).  Every wait
+// of the protocol stays satisfiable.
+#ifndef TAV_PEER_FILTER_MUTANT
+#define TAV_PEER_FILTER_MUTANT 0
 #endif
 
 // ---- compaction after a removal (tav_compact.cu) -----------------------------------------
@@ -326,6 +336,13 @@ extern "C" int tav_internal_compact_stats(tav_index* ix, int* path, int64_t* win
 // library-internal: the largest allocation tav_rows_stage may make on this index, in bytes (-1: no cap).  A
 // stage above it gives TAV_ERR_OOM as a failed cudaMalloc would; tests use it to reach that path.
 extern "C" int tav_internal_stage_cap(tav_index* ix, int64_t max_bytes);
+// Tests only: tav_set_query_masks fails with TAV_ERR_OOM, as a failed allocation does, for masks of more than
+// max_bytes bytes (-1: no cap), so that one rank's mask upload can fail without a device fault.
+extern "C" int tav_internal_qmask_cap(tav_index* ix, int64_t max_bytes);
+// Tests only: while `on`, every tensor-core search of the index asks cudaMalloc for 2^60 bytes for its bookkeeping
+// (a real allocation failure: cudaErrorMemoryAllocation, not sticky) and returns TAV_ERR_OOM, as a search does when
+// its buffers do not fit.
+extern "C" int tav_internal_search_alloc_fail(tav_index* ix, int on);
 // library-internal: bytes of this index's library-owned row allocation and staged block, and bytes held in such row
 // blocks by every index of the process.  Tests use it to see that a rebalance frees the block it replaced.
 extern "C" int tav_internal_row_bytes(tav_index* ix, int64_t* index_bytes, int64_t* process_bytes);

@@ -992,10 +992,15 @@ merge_kernel(int n_lists, int n_queries, int k, const int64_t* items, const floa
             __threadfence();
             if (tid < sync.world && tid != sync.me) st_release_sys(sync.ack[tid], sync.seq);
             if (tid == 0) {
-                uint32_t sum = 0;
-                for (int r = 0; r < sync.world; ++r)
-                    sum += *reinterpret_cast<const volatile uint32_t*>(sync.tails + static_cast<size_t>(r) * sync.slot_bytes);
+                uint32_t sum = 0, status = 0;
+                for (int r = 0; r < sync.world; ++r) {
+                    const volatile uint32_t* tail =
+                        reinterpret_cast<const volatile uint32_t*>(sync.tails + static_cast<size_t>(r) * sync.slot_bytes);
+                    sum += tail[0];
+                    status += tail[1];
+                }
                 *sync.flagged_host = sum;
+                *sync.status_host = TAV_PEER_FILTER_MUTANT == 2 ? 0u : status;
             }
         }
     }
@@ -1004,7 +1009,7 @@ merge_kernel(int n_lists, int n_queries, int k, const int64_t* items, const floa
 cudaError_t launch_merge(int n_lists, int n_queries, int k, const int64_t* items,
                          const float* scores, const int32_t* counts, int64_t items_stride,
                          int64_t scores_stride, int64_t counts_stride, int64_t* out_items,
-                         float* out_scores, int32_t* out_counts, cudaStream_t s, const MergeSync* sync) {
+                         float* out_scores, int32_t* out_counts, cudaStream_t s) {
     if (items_stride == 0) items_stride = static_cast<int64_t>(n_queries) * k;
     if (scores_stride == 0) scores_stride = static_cast<int64_t>(n_queries) * k;
     if (counts_stride == 0) counts_stride = n_queries;
@@ -1012,11 +1017,10 @@ cudaError_t launch_merge(int n_lists, int n_queries, int k, const int64_t* items
     static int granted[16] = {};
     cudaError_t e = ensure_dynamic_smem(merge_kernel<0>, smem, granted);
     if (e != cudaSuccess) return e;
-    MergeSync none{};
     merge_kernel<0><<<n_queries, kSelectThreads, smem, s>>>(n_lists, n_queries, k, items, scores,
                                                             counts, items_stride, scores_stride,
                                                             counts_stride, out_items, out_scores,
-                                                            out_counts, sync ? *sync : none);
+                                                            out_counts, MergeSync{});
     return cudaGetLastError();
 }
 
@@ -1024,36 +1028,37 @@ template <int ORDER>
 static cudaError_t launch_merge_t(int n_lists, int n_queries, int k, const int64_t* items, const float* scores,
                                   const int32_t* counts, int64_t items_stride, int64_t scores_stride,
                                   int64_t counts_stride, int64_t* out_items, float* out_scores, int32_t* out_counts,
-                                  cudaStream_t s) {
+                                  cudaStream_t s, const MergeSync& sync) {
     const size_t smem = static_cast<size_t>(select_cap(k)) * sizeof(uint64_t);
     static int granted[16] = {};
     cudaError_t e = ensure_dynamic_smem(merge_kernel<ORDER>, smem, granted);
     if (e != cudaSuccess) return e;
     merge_kernel<ORDER><<<n_queries, kSelectThreads, smem, s>>>(n_lists, n_queries, k, items, scores, counts,
                                                                 items_stride, scores_stride, counts_stride, out_items,
-                                                                out_scores, out_counts, MergeSync{});
+                                                                out_scores, out_counts, sync);
     return cudaGetLastError();
 }
 
 cudaError_t launch_merge_ordered(int n_lists, int n_queries, int k, const int64_t* items, const float* scores,
                                  const int32_t* counts, int64_t items_stride, int64_t scores_stride,
                                  int64_t counts_stride, int order, int64_t* out_items, float* out_scores,
-                                 int32_t* out_counts, cudaStream_t s) {
+                                 int32_t* out_counts, cudaStream_t s, const MergeSync* sync) {
     if (items_stride == 0) items_stride = static_cast<int64_t>(n_queries) * k;
     if (scores_stride == 0) scores_stride = static_cast<int64_t>(n_queries) * k;
     if (counts_stride == 0) counts_stride = n_queries;
 #if TAV_SHARDED_FILTER_MUTANT == 1
     order = 0;
 #endif
+    const MergeSync none{};
     switch (order) {
         case 0: return launch_merge_t<0>(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride,
-                                         counts_stride, out_items, out_scores, out_counts, s);
+                                         counts_stride, out_items, out_scores, out_counts, s, sync ? *sync : none);
         case 1: return launch_merge_t<1>(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride,
-                                         counts_stride, out_items, out_scores, out_counts, s);
+                                         counts_stride, out_items, out_scores, out_counts, s, sync ? *sync : none);
         case 2: return launch_merge_t<2>(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride,
-                                         counts_stride, out_items, out_scores, out_counts, s);
+                                         counts_stride, out_items, out_scores, out_counts, s, sync ? *sync : none);
         case 3: return launch_merge_t<3>(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride,
-                                         counts_stride, out_items, out_scores, out_counts, s);
+                                         counts_stride, out_items, out_scores, out_counts, s, sync ? *sync : none);
     }
     return cudaErrorInvalidValue;
 }

@@ -22,8 +22,10 @@ results whose size is known only after the local searches: they exchange over th
 the hits padded to the largest rank's total) and merge with ``tav_merge_range``.
 
 Filtered and subset lookups (``predicate=``, ``fuzzy_lookup_embedding_in_subset``, ``subset=`` / ``allowed=`` /
-``ties_low_first=``) return what ``VectorBase`` returns for the whole corpus, tie order included.  They exchange
-the packed layout over the process group and merge with ``tav_merge_topk_ordered``: a row mask (a predicate is
+``ties_low_first=``) return what ``VectorBase`` returns for the whole corpus, tie order included.  With
+``exchange="peer"`` they take the peer exchange as well (``tav_sharded_search`` with the mask and tie flags,
+``tav_sharded_search_subset``), can stay on the device and be deferred (``search_tensors``); otherwise they exchange
+the packed layout over the process group and merge with ``tav_merge_topk_ordered``.  Either way: a row mask (a predicate is
 evaluated by each rank over its own rows only) merges low row first where the reference's predicate path does;
 a subset is searched per rank with ``TAV_ITEMS_AS_POSITIONS``, its hits mapped to positions in the caller's
 subset (``tav_map_items``), merged by position and decoded through the caller's list at the end.  Per-query
@@ -155,7 +157,13 @@ class CudaShardEngine:
         self._group = handle
         return handle
 
-    def group_search(self, dist, process_group, rank, world, queries, k, min_score, item_offset, defer_check):
+    def group_search(self, dist, process_group, rank, world, queries, k, min_score, item_offset, defer_check,
+                     ties_low_first=False, mask=None, subset=None):
+        """One search through the peer exchange.  ``mask``: this block's packed words, key and owner (as
+        ``search_rows_packed`` takes them), uploaded unless already on the device; ``subset``: this rank's share
+        (block-local ordinals, their CSR offsets per query or None for one shared subset, their positions in the
+        caller's list), searched by ``tav_sharded_search_subset``, whose merged items are those positions.  A local
+        failure (the mask upload here, or the local search) is still published, so that every peer raises too."""
         torch = self.torch
         if isinstance(queries, np.ndarray):
             queries = torch.from_numpy(np.ascontiguousarray(queries, dtype=np.float32)).to(self.device, non_blocking=True)
@@ -167,12 +175,53 @@ class CudaShardEngine:
         counts = torch.empty((b,), dtype=torch.int32, device=self.device)
         stream = torch.cuda.current_stream(self.device).cuda_stream
         flags = self.base._flags() | (_capi.TAV_DEFER_RETRY if defer_check else 0)
-        _capi.check(lib.tav_sharded_search(ix, group, C.c_void_p(queries.data_ptr()), b, k, C.c_float(min_score), flags,
-                                           item_offset, C.c_void_p(items.data_ptr()), C.c_void_p(scores.data_ptr()),
-                                           C.c_void_p(counts.data_ptr()), C.c_void_p(stream)))
-        if defer_check:
-            self._group_keep.append((queries, items, scores, counts, stream))
+        flags |= _capi.TAV_TIES_LOW_FIRST if ties_low_first else 0
+        error = None
+        if mask is not None:
+            flags |= _capi.TAV_USE_QUERY_MASKS if np.ndim(mask[0]) == 2 else _capi.TAV_USE_ROW_MASK
+            try:
+                self.upload_mask(mask, b)
+            except Exception as e:  # noqa: BLE001
+                error = e
+                self._drop_masks(lib, ix)  # the local search then fails and publishes this rank's failure
+        keep = (queries, items, scores, counts, stream)
+        if subset is None:
+            rc = lib.tav_sharded_search(ix, group, C.c_void_p(queries.data_ptr()), b, k, C.c_float(min_score), flags,
+                                        item_offset, C.c_void_p(items.data_ptr()), C.c_void_p(scores.data_ptr()),
+                                        C.c_void_p(counts.data_ptr()), C.c_void_p(stream))
+        else:
+            local, offsets, positions = subset
+            sub = np.ascontiguousarray(local, np.int64)
+            offs = None if offsets is None else np.ascontiguousarray(offsets, np.int64)
+            pos = torch.from_numpy(np.ascontiguousarray(positions, np.int64)).to(self.device)
+            keep += (pos,)
+            rc = lib.tav_sharded_search_subset(
+                ix, group, C.c_void_p(queries.data_ptr()), b, k, C.c_float(min_score), flags,
+                sub.ctypes.data_as(C.c_void_p), len(sub), None if offs is None else offs.ctypes.data_as(C.c_void_p),
+                C.c_void_p(pos.data_ptr()), C.c_void_p(items.data_ptr()), C.c_void_p(scores.data_ptr()),
+                C.c_void_p(counts.data_ptr()), C.c_void_p(stream))
+        if defer_check:  # a search that failed after its publish is open too: its buffers live until finish
+            self._group_keep.append(keep)
+        if error is not None:
+            raise error
+        _capi.check(rc)
         return items, scores, counts
+
+    def upload_mask(self, mask, n_queries: int) -> None:
+        """Put this block's mask (words, key, owner) on the device unless it is there already."""
+        if self.n_local() == 0:
+            return
+        words, key, owner = mask
+        lib, ix = self.base._ensure_device()
+        if np.ndim(words) == 2:
+            self.base._use_query_masks(lib, ix, words, n_queries)
+        else:
+            self.base._use_row_mask(lib, ix, words, key, owner)
+
+    def _drop_masks(self, lib, ix) -> None:
+        lib.tav_set_row_mask(ix, None, 0, 0, None)
+        lib.tav_set_query_masks(ix, None, 0, 0, 0, 0, None)
+        self.base._mask_key = self.base._qmask_key = None
 
     def group_finish(self) -> int:
         if self._group is None or not self._group_keep:
@@ -715,6 +764,8 @@ class ShardedVectorBase:
         self._pending: list = []  # deferred searches since the last finish(): ["group"] or (local, b, k, out) tuples
         self._generation = 0      # bumped whenever rows are replaced or removed (part of the mask cache keys)
         self._masks: dict = {}    # (kind, id(mask or predicate), generation, rows) -> (this block's words, owner)
+        self._peer_masks: dict = {}  # "row" / "query" -> key of the mask every rank uploaded for the peer exchange
+        self._decode: list = []   # (items, list) of deferred subset lookups: positions decoded at finish()
 
     # ---- corpus ------------------------------------------------------------------------
     def __len__(self) -> int:
@@ -947,23 +998,35 @@ class ShardedVectorBase:
             self._dist.all_gather_into_tensor(gathered.view(-1), local, group=self._group)
         return self._engine.merge(gathered, self.world, b, k)
 
-    def search_tensors(self, queries, k: int, min_score: float = 0.0, defer_check: bool = False):
+    def search_tensors(self, queries, k: int, min_score: float = 0.0, defer_check: bool = False, *, allowed=None,
+                       subset=None, subsets=None, ties_low_first: bool = False):
         """SPMD lookup; returns engine tensors (items, scores, counts), replicated on every
         rank.  ``queries``: float32 [B, D] numpy array or engine-device tensor.
 
         The local search, the candidate all-gather and the merge are enqueued back to back
         without a host synchronisation; the (rare) "redo this query exactly" check runs at the
         end — immediately, or in ``finish()`` when ``defer_check`` is set — and repeats the
-        exchange only if some rank actually had to redo a query."""
+        exchange only if some rank actually had to redo a query.
+
+        ``allowed``, ``subset``, ``subsets`` and ``ties_low_first`` as ``search_arrays`` takes them, with its
+        results and errors (the queries are read on the host for their checks).  With ``exchange="peer"`` these
+        lookups go through the peer exchange too, and with ``defer_check`` they are resolved by ``finish()``
+        together with the plain deferred ones; a subset lookup's items are the caller's ordinals only after
+        ``finish()`` then.  Otherwise they exchange over the process group and are complete on return."""
+        if allowed is not None or subset is not None or subsets is not None or ties_low_first:
+            if hasattr(queries, "cpu"):
+                queries = queries.cpu().numpy()
+            if subsets is not None:
+                return self._search_arrays_subsets(queries, k, min_score, subsets, subset, allowed, ties_low_first,
+                                                   tensors=True, defer_check=defer_check)
+            return self._search_arrays_filtered(queries, k, min_score, subset, allowed, ties_low_first, tensors=True,
+                                                defer_check=defer_check)
         n = len(self)
         b = int(queries.shape[0])
         k = max(1, min(int(k), max(n, 1)))
         lo, _ = self.local_range
-        if self.exchange == "peer" and self.world > 1 and hasattr(self._engine, "group_search"):
-            out = self._engine.group_search(self._dist, self._group, self.rank, self.world, queries, k,
-                                            float(np.float32(min_score)), lo, defer_check)
-            self._pending = ["group"] if defer_check else []
-            return out
+        if self._peer():
+            return self._group_search(queries, k, float(np.float32(min_score)), defer_check)
         deferrable = hasattr(self._engine, "finish")
         local = (self._engine.search_packed(queries, k, float(np.float32(min_score)), lo, defer_check=True)
                  if deferrable else self._engine.search_packed(queries, k, float(np.float32(min_score)), lo))
@@ -983,6 +1046,8 @@ class ShardedVectorBase:
         Collective: every rank calls it.  Deferred lookups that were not finished are dropped; call ``finish()``
         first to keep them.  An engine without device state has nothing to release."""
         self._pending = []
+        self._decode = []
+        self._peer_masks = {}
         close = getattr(self._engine, "close", None)
         if close is not None:
             close(self._dist, self._group)
@@ -997,7 +1062,11 @@ class ShardedVectorBase:
             return 0
         self._pending = []
         if pending == ["group"]:       # libtavec agrees across ranks inside tav_sharded_finish
-            return self._engine.group_finish()
+            decode, self._decode = self._decode, []
+            redone = self._engine.group_finish()
+            for items, table in decode:  # merged subset positions -> the caller's ordinals, as given
+                self._engine.map_items(items, table)
+            return redone
         # a local failure must not leave the other ranks waiting in the collective: reduce an error
         # flag together with the count and raise on every rank
         error = None
@@ -1024,7 +1093,9 @@ class ShardedVectorBase:
         [B].  ``subset``, ``subsets``, ``allowed`` and ``ties_low_first`` as ``VectorBase.search_arrays`` takes
         them over the whole corpus (global ordinals; ``allowed`` a bool [N] mask or its packed words, or one mask
         per query: bool [B, N] or packed words [B, ceil(N / 32)]), with its results and
-        errors; such lookups exchange over the process group whatever ``exchange`` says."""
+        errors.  With ``exchange="peer"`` such lookups go through the peer exchange (``tav_sharded_search`` /
+        ``tav_sharded_search_subset``), otherwise over the process group; threshold routes (k >= rows > 8192, per-query
+        subsets with k > 2048) always exchange over the process group."""
         if subsets is not None:
             return self._search_arrays_subsets(queries, k, min_score, subsets, subset, allowed, ties_low_first)
         if subset is not None or allowed is not None or ties_low_first:
@@ -1045,6 +1116,56 @@ class ShardedVectorBase:
         return items.cpu().numpy(), scores.cpu().numpy(), counts.cpu().numpy()
 
     # ---- filtered and subset lookups ------------------------------------------------------
+    def _peer(self) -> bool:
+        """Lookups go through the engine's peer exchange (``tav_sharded_search*``)."""
+        return self.exchange == "peer" and self.world > 1 and hasattr(self._engine, "group_search")
+
+    def _group_search(self, q, k: int, floor: float, defer_check: bool, ties_low_first: bool = False, mask=None,
+                      subset=None, decode=None):
+        """One lookup through the peer exchange; ``decode``: the merged items are positions in this list, replaced
+        by its entries now, or at ``finish()`` for a deferred lookup.  A mask that is not the one every rank
+        uploaded last is uploaded first, and the ranks agree on that upload (one all-reduce) before the publish."""
+        if mask is not None:
+            self._agree_mask(mask, len(q))
+        lo, _ = self.local_range
+        try:
+            out = self._engine.group_search(self._dist, self._group, self.rank, self.world, q, k, floor, lo,
+                                            defer_check, ties_low_first=ties_low_first, mask=mask, subset=subset)
+        except Exception:
+            if defer_check:  # a deferred search that failed after its publish is open on every rank
+                self._pending = ["group"]
+            raise
+        self._pending = ["group"] if defer_check else []
+        if defer_check:
+            if decode is not None:
+                self._decode.append((out[0], decode))
+        else:
+            # a synchronous search finished every open one inside the library: decode theirs, then its own
+            for items, table in self._decode:
+                self._engine.map_items(items, table)
+            self._decode = []
+            if decode is not None:
+                self._engine.map_items(out[0], decode)
+        return out
+
+    def _agree_mask(self, mask, n_queries: int) -> None:
+        """Upload this block's mask for the peer exchange unless every rank uploaded it last: the upload finishes
+        the deferred lookups first, and its failure on any rank raises on every rank, before anything is
+        published.  A mask already agreed on adds no collective."""
+        kind = "query" if np.ndim(mask[0]) == 2 else "row"
+        if self._peer_masks.get(kind) == mask[1]:
+            return
+        self.finish()
+        self._peer_masks.pop(kind, None)
+        error = None
+        try:
+            self._engine.upload_mask(mask, n_queries)
+        except Exception as e:  # noqa: BLE001
+            error = e
+        if self._any_failed(error is not None):
+            raise error if error is not None else RuntimeError("a mask upload failed on another rank")
+        self._peer_masks[kind] = mask[1]
+
     def _check_queries(self, queries) -> np.ndarray:
         q = np.ascontiguousarray(queries, dtype=np.float32)
         if q.ndim == 1:
@@ -1129,9 +1250,21 @@ class ShardedVectorBase:
             raise error if error is not None else RuntimeError("a lookup failed on another rank")
         return self._engine.merge_ordered(gathered, self.world, b, k, order)
 
-    def _search_arrays_filtered(self, queries, k, min_score, subset, allowed, ties_low_first, mask=None):
+    def _as_output(self, arrays, tensors: bool):
+        """(items, scores, counts): numpy arrays, or with ``tensors`` tensors on the engine's device."""
+        if not tensors:
+            return tuple(a.cpu().numpy() if hasattr(a, "cpu") else a for a in arrays)
+        import torch
+
+        dev = self._engine.comm_device() if hasattr(self._engine, "comm_device") else torch.device("cpu")
+        return tuple(torch.from_numpy(np.ascontiguousarray(a)).to(dev) if isinstance(a, np.ndarray) else a
+                     for a in arrays)
+
+    def _search_arrays_filtered(self, queries, k, min_score, subset, allowed, ties_low_first, mask=None,
+                                tensors=False, defer_check=False):
         """``VectorBase.search_arrays`` with a subset, a row mask (``allowed``, or ``mask`` = this block's words,
-        key, owner as ``_block_mask`` returns them) or ties low-first, checks in its order."""
+        key, owner as ``_block_mask`` returns them) or ties low-first, checks in its order.  ``tensors``: the
+        result as engine tensors; ``defer_check`` as ``search_tensors`` takes it (the peer exchange only)."""
         q = self._check_queries(queries)
         b = len(q)
         if k < 1:
@@ -1148,7 +1281,7 @@ class ShardedVectorBase:
         floor = _as_f32_scalar(min_score)
         # early returns and errors on replicated state only: every rank takes them together
         if b == 0 or n_rows == 0 or len(self) == 0 or np.isnan(floor):
-            return items, scores, counts
+            return self._as_output((items, scores, counts), tensors)
         if allowed is not None and sub is not None:
             raise ValueError("allowed= and subset= cannot be combined")
         if allowed is not None:
@@ -1158,8 +1291,16 @@ class ShardedVectorBase:
         if k_eff >= n_rows > RANGE_ROUTE_MIN_ROWS:
             # every passing row, as tav_search routes it on one GPU: one threshold search, laid out [B, n_rows]
             csr = self._search_range_filtered(q, floor, ties_low_first, sub, mask)
-            return as_topk_arrays(*csr, b, k_eff)
+            return self._as_output(as_topk_arrays(*csr, b, k_eff), tensors)
         lo, hi = self.local_range
+        if self._peer():
+            if sub is not None:
+                positions, local_sub = subset_share(sub, len(self), lo, hi)
+                out = self._group_search(q, k_eff, float(floor), defer_check, ties_low_first,
+                                         subset=(local_sub, None, positions), decode=sub)
+            else:
+                out = self._group_search(q, k_eff, float(floor), defer_check, ties_low_first, mask=mask)
+            return self._as_output(out, tensors)
         if sub is not None:
             positions, local_sub = subset_share(sub, len(self), lo, hi)
             items_t, scores_t, counts_t = self._exchange_topk(
@@ -1173,7 +1314,7 @@ class ShardedVectorBase:
             items_t, scores_t, counts_t = self._exchange_topk(
                 lambda: self._engine.search_rows_packed(q, k_eff, float(floor), lo, ties_low_first, words, key, owner),
                 b, k_eff, 1 if ties_low_first else 0)
-        return items_t.cpu().numpy(), scores_t.cpu().numpy(), counts_t.cpu().numpy()
+        return self._as_output((items_t, scores_t, counts_t), tensors)
 
     def _subsets_checked(self, queries, subsets, subset, allowed):
         """(queries, offsets, ordinals) of a per-query subsets lookup; every error is raised from replicated
@@ -1184,10 +1325,12 @@ class ShardedVectorBase:
         offsets, ordinals = VectorBase._subsets_csr(subsets, len(q))
         return q, offsets, ordinals
 
-    def _search_arrays_subsets(self, queries, k, min_score, subsets, subset, allowed, ties_low_first):
+    def _search_arrays_subsets(self, queries, k, min_score, subsets, subset, allowed, ties_low_first, tensors=False,
+                               defer_check=False):
         """``VectorBase.search_arrays(subsets=)`` over the whole corpus.  Each rank searches its share of every
         query's subset with flat positions as items, maps them to positions in the caller's ordinals, the ranks'
-        lists are merged by position and decoded through the caller's ordinals."""
+        lists are merged by position and decoded through the caller's ordinals.  ``tensors`` / ``defer_check`` as
+        ``_search_arrays_filtered`` takes them."""
         if k < 1:
             raise ValueError("k must be >= 1")
         q, offsets, ordinals = self._subsets_checked(queries, subsets, subset, allowed)
@@ -1196,19 +1339,25 @@ class ShardedVectorBase:
         k_eff = max(1, min(k, longest))
         floor = _as_f32_scalar(min_score)
         if b == 0 or longest == 0 or len(self) == 0 or np.isnan(floor):
-            return np.full((b, k_eff), -1, np.int64), np.zeros((b, k_eff), np.float32), np.zeros(b, np.int32)
+            return self._as_output((np.full((b, k_eff), -1, np.int64), np.zeros((b, k_eff), np.float32),
+                                    np.zeros(b, np.int32)), tensors)
         check_subset(ordinals, len(self))
         check_subsets_total(len(ordinals))
         if k_eff > SUBSETS_MERGE_MAX_K:
-            return as_topk_arrays(*self._search_range_subsets(q, floor, ties_low_first, offsets, ordinals), b, k_eff)
+            csr = self._search_range_subsets(q, floor, ties_low_first, offsets, ordinals)
+            return self._as_output(as_topk_arrays(*csr, b, k_eff), tensors)
         lo, hi = self.local_range
         positions, local_offsets, local_ordinals = subsets_share(offsets, ordinals, len(self), lo, hi)
+        if self._peer():
+            out = self._group_search(q, k_eff, float(floor), defer_check, ties_low_first,
+                                     subset=(local_ordinals, local_offsets, positions), decode=ordinals)
+            return self._as_output(out, tensors)
         items_t, scores_t, counts_t = self._exchange_topk(
             lambda: self._engine.search_subsets_packed(q, k_eff, float(floor), local_offsets, local_ordinals, positions,
                                                        ties_low_first),
             b, k_eff, 3 if ties_low_first else 2)
         self._engine.map_items(items_t, ordinals)  # flat positions -> the caller's ordinals, as given
-        return items_t.cpu().numpy(), scores_t.cpu().numpy(), counts_t.cpu().numpy()
+        return self._as_output((items_t, scores_t, counts_t), tensors)
 
     def _search_range_subsets(self, q, floor, ties_low_first, offsets, ordinals):
         """The threshold search of validated per-query subsets: flat positions merged, then decoded."""
