@@ -383,6 +383,74 @@ int tav_sharded_search_subset(tav_index* ix, tav_group* g, const float* queries_
 int tav_sharded_finish(tav_index* ix, tav_group* g, void* stream, int* redone_total);
 
 /*
+ * Row-sharded threshold search through peer memory: every hit at or above min_score over every rank's rows, merged
+ * on every rank (the result of tav_range_search over the whole corpus), with no NCCL call.  Its results have sizes
+ * known only after the local search, so it uses a second allocation of the group, the RANGE INBOX:
+ *
+ *   range_arrive[world] u32 | range_ack[world] u32 | hdr[world][max_queries + 2] int64 |
+ *   items[world][capacity] int64 | scores[world][capacity] float32
+ *
+ * Section r (rank r's CSR offsets [B + 1] and a word status | hits-included << 1, then its hits) is written only
+ * by rank r, and tav_merge_range merges the world's sections in place.  The host side runs these steps on every
+ * rank in lockstep, taking every decision from replicated data:
+ *
+ *   tav_group_range_reserve   frees this rank's inbox (closing its mappings of the peers' inboxes) and allocates
+ *                             one for max_queries queries and `capacity` hits per rank (0, 0: only frees it).
+ *                             Collective with _handle and _connect, as tav_group_create / _local_handle / _connect
+ *                             are: the ranks quiesce and agree first, reserve, exchange the handles, connect.  The
+ *                             new inbox counts its rounds from 0.  An allocation failure gives TAV_ERR_OOM and no
+ *                             inbox; the host side then frees the inbox on every rank.
+ *   tav_group_range_capacity  max_queries and capacity of the connected inbox (0, 0: none).
+ *   tav_sharded_range_search  the local search (tav_range_search over this rank's rows, items + item_offset; with
+ *                             TAV_ITEMS_AS_POSITIONS one subset of block-local ordinals, or per-query subsets with
+ *                             CSR `offsets` as tav_range_search_subsets takes them, whose hits are mapped through
+ *                             `positions` (host int64 [subset_len], copied to the device by the library) as
+ *                             tav_sharded_search_subset maps them); it synchronises once, as tav_range_search
+ *                             does.  Then round 1: this rank's header, and its hits when they fit in `capacity`,
+ *                             stored into every peer's inbox over NVLink with a system-scope release flag; a wait
+ *                             for every rank's round, and every rank's header to `world_headers` (host int64
+ *                             [world][n_queries + 2]).  A second synchronisation, which sizes the result.
+ *                             Flags: TAV_FORCE_SCAN, TAV_FORCE_MMA, TAV_USE_ROW_MASK, TAV_USE_QUERY_MASKS,
+ *                             TAV_TIES_LOW_FIRST, TAV_ITEMS_AS_POSITIONS.  queries are host float32.
+ *   tav_sharded_range_republish  round 2, when some rank's hits-included bit was 0: after every rank reserved an
+ *                             inbox that holds the largest total, every rank publishes its whole list again (the
+ *                             index still holds the hits) and waits for the world's.  Synchronises.
+ *   tav_sharded_range_merge   tav_merge_range over the inbox into the caller's device outputs (out_offsets [B + 1],
+ *                             out_items / out_scores [sum of the totals]), then this rank acknowledges the round to
+ *                             its peers (also when the merge fails).  No synchronisation.
+ *   tav_sharded_range_abort   closes an open search without a merge: this rank acknowledges its last round, so that
+ *                             no peer's next publish waits for it.  For a caller that cannot merge (its output
+ *                             buffers could not be allocated, say); its peers merge as usual.  No-op when nothing is
+ *                             open.
+ *
+ * A search stays open from tav_sharded_range_search to its merge or abort: no other range search, and no search on
+ * the index that would replace its hits, may run in between (a tav_sharded_range_search finding one open closes it
+ * as tav_sharded_range_abort does).  Every rank calls the steps with the same n_queries and flags.
+ *
+ * Failures.  A threshold search whose local part fails on a rank (an error of the local tav_range_search* other than
+ * TAV_ERR_CUDA: an argument it rejects, a missing mask, an allocation; or the allocation of the positions' device
+ * copy) still publishes its header, with status 1 and no hits, and returns that rank's own error; every rank adds up
+ * the world's status words, and every other rank gets TAV_ERR_PEER from tav_sharded_range_search.  Each rank
+ * acknowledges such a round itself and the search is closed.  Not published, so that the peers' waits trap after
+ * about 4 s: a local TAV_ERR_CUDA, and the checks tav_sharded_range_search makes before its local search (NULL or
+ * malformed arguments, no connected inbox, more queries than it holds).  Those checks see only replicated state and
+ * arguments, so a caller that makes every rank's call alike, and checks its arguments on every rank first (as
+ * ShardedVectorBase does), never reaches them on one rank alone.
+ */
+int tav_group_range_reserve(tav_group* g, int max_queries, int64_t capacity);
+int tav_group_range_handle(tav_group* g, void* handle_out /* tav_group_handle_bytes() */);
+int tav_group_range_connect(tav_group* g, const void* handles /* world x tav_group_handle_bytes() */);
+int tav_group_range_capacity(const tav_group* g, int* max_queries, int64_t* capacity);
+int tav_sharded_range_search(tav_index* ix, tav_group* g, const float* queries, int n_queries, float min_score,
+                             int flags, const int64_t* subset, int64_t subset_len, const int64_t* offsets,
+                             const int64_t* positions, int64_t item_offset, int64_t expected_hits,
+                             int64_t* world_headers, void* stream);
+int tav_sharded_range_republish(tav_group* g, void* stream);
+int tav_sharded_range_abort(tav_group* g, void* stream);
+int tav_sharded_range_merge(tav_group* g, int ties_low_first, int64_t* out_offsets, int64_t* out_items,
+                            float* out_scores, void* stream);
+
+/*
  * Rebalance of row-sharded indexes (ShardedVectorBase.rebalance): every rank's new block is copied from the
  * ranks' current row allocations over CUDA IPC, in the storage dtype, byte for byte, by the copy engines.
  *

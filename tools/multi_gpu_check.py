@@ -9,14 +9,16 @@ Every rank builds the same seeded corpus on the host, keeps its own row block on
 peer-memory publish/merge over NVLink, and the NCCL all-gather form), merge kernel — is BIT-IDENTICAL to
 the single-GPU lookup over the whole corpus on that rank's GPU, for the float32 row-scan path, the
 float32 split form and the bf16 / fp16 tensor-core paths, and agrees with the CPU oracle.  The sharded
-threshold search (``search_range``: offsets and hits all-gathered, ``tav_merge_range``) must equal the
+threshold search (``search_range``, merged by ``tav_merge_range``) must equal the
 single-GPU ``search_range`` bit for bit on every rank: float32 row scan, bf16 tensor cores, float32 split form.
 Filtered and subset lookups (row masks, predicates, subsets; top-k and threshold) must equal the single-GPU
 ``VectorBase`` bit for bit on every rank.  The same filtered, per-query-mask and per-query-subset top-k lookups go
 through the peer exchange (``tav_sharded_search`` / ``tav_sharded_search_subset``) with ``exchange="peer"``, also
 deferred on the device (``search_tensors(..., defer_check=True)`` and one ``finish()``), and through the NCCL
-exchange with ``exchange="nccl"``: both must equal the single-GPU lookup.  These peer-exchange cases have not been
-run on two or more GPUs.
+exchange with ``exchange="nccl"``: both must equal the single-GPU lookup.  Threshold searches (plain, every row,
+row and per-query masks, subsets, per-query subsets) through the peer exchange's range inbox and through the process
+group must equal the single-GPU ``search_range``.  These peer-exchange cases, top-k and threshold, have not been run
+on two or more GPUs.
 """
 import os
 import sys
@@ -102,7 +104,7 @@ def main():
         if rank == 0:
             print(f"multi-gpu ok: world={world} exact fallback through finish(), one and three outstanding, "
                   f"exchange={exchange}", flush=True)
-    # threshold search (search_range: offsets + hits all-gathered, tav_merge_range): bit-identical to the single-GPU
+    # threshold search (search_range, merged by tav_merge_range): bit-identical to the single-GPU
     # search_range over the whole corpus, at sizes where every rank takes the same path as the whole-corpus search
     for storage, n, d, b, ms, path in (("float32", 70001, 96, 5, 0.55, "scan"),
                                        ("bfloat16", 160001, 128, 32, 0.6, "mma"),
@@ -190,6 +192,30 @@ def main():
         if rank == 0:
             print(f"multi-gpu ok: world={world} filtered, subset and per-query-mask lookups {storage} n={n} d={d} "
                   f"b={b}, synchronous and deferred, peer and nccl exchanges", flush=True)
+    # threshold searches through either exchange (exchange="peer": the range inbox over NVLink, with a grow when
+    # min_score 0 returns every row): equal to the single-GPU search_range bit for bit on every rank
+    n, d, b = 120001, 128, 24
+    v, q = O.make_corpus(n, d, seed=n + 3, n_queries=b)
+    whole = tab.VectorBase(settings, device=local, storage_dtype="bfloat16")
+    whole.add_embeddings(None, v)
+    rng = np.random.default_rng(n)
+    sub = np.concatenate([rng.permutation(n)[:3000], np.arange(500), [-1, -n, 0]])
+    subsets = [rng.permutation(n)[: 200 + 50 * i].astype(np.int64) for i in range(b)]
+    searches = [(q, 0.6, {}), (q[:2], 0.0, {}), (q, 0.6, dict(allowed=rng.random(n) < 0.3, ties_low_first=True)),
+                (q, 0.5, dict(allowed=rng.random((b, n)) < 0.3)), (q, 0.4, dict(subset=sub)),
+                (q, 0.4, dict(subsets=subsets, ties_low_first=True))]
+    for exchange in ("peer", "nccl"):
+        shx = ShardedVectorBase(settings, device=local, storage_dtype="bfloat16", exchange=exchange)
+        shx.deserialize(v)
+        for qq, ms, kw in searches:
+            for g, w in zip(shx.search_range(qq, ms, **kw), whole.search_range(qq, ms, **kw)):
+                np.testing.assert_array_equal(g.view(np.uint32) if g.dtype == np.float32 else g,
+                                              w.view(np.uint32) if w.dtype == np.float32 else w)
+        shx.close()
+    dist.barrier()
+    if rank == 0:
+        print(f"multi-gpu ok: world={world} threshold searches bfloat16 n={n} d={d} b={b}, peer and nccl exchanges",
+              flush=True)
     dist.destroy_process_group()
 
 

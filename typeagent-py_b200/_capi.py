@@ -74,6 +74,16 @@ SIGNATURES = {
                                             C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p]),
     "tav_sharded_finish": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
+    "tav_group_range_reserve": (C.c_int, [C.c_void_p, C.c_int, C.c_int64]),
+    "tav_group_range_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "tav_group_range_connect": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "tav_group_range_capacity": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), _i64p]),
+    "tav_sharded_range_search": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int,
+                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                           C.c_void_p, C.c_void_p]),
+    "tav_sharded_range_republish": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "tav_sharded_range_abort": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "tav_sharded_range_merge": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tav_rows_handle_bytes": (C.c_int, []),
     "tav_rows_export": (C.c_int, [C.c_void_p, C.c_void_p, _i64p]),
     "tav_rows_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,

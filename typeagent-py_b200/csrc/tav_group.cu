@@ -31,11 +31,26 @@
 // host word per slot, and every rank reports TAV_ERR_PEER for a search whose sum is not zero: a synchronous call
 // on return, a deferred one at tav_sharded_finish.  A CUDA error cannot be published (the device may be unusable):
 // the call returns without publishing and its peers' waits end in the ~4 s trap of spin_until.
+//
+// Threshold searches (tav_sharded_range_*) have results whose size is known only after the local search, so they
+// use a second allocation of the group, the "range inbox", with its own IPC handle and its own sequence numbers:
+//   range_arrive[world] u32 | range_ack[world] u32 |
+//   hdr[world][hdr_stride] int64      rank r's CSR offsets [B + 1], then a word: status | hits-included << 1
+//   items[world][cap] int64 | scores[world][cap] float32
+// Section r of every rank's inbox is written only by rank r, so tav_merge_range merges the world's lists in place.
+// A round: the local search (it synchronises), this rank's header and (when they fit in `cap`) its hits stored into
+// every peer's section r, range_arrive[me] = seq released at system scope; a one-CTA wait spins on the arrive words
+// and copies the world's headers to the host, which sizes the result.  When some rank's hits did not fit, the host
+// side reserves larger inboxes on every rank (tav_group_range_reserve: the totals are replicated, so every rank
+// takes that branch) and every rank republishes its whole list, still held by the index.  After the merge an ack
+// kernel stores range_ack[me] = seq into every peer's inbox; a publish first waits for every peer's ack of the
+// previous round.  A reserve starts the sequence numbers of the new inbox from 0, as its arrive / ack words do.
 
 #include <stdio.h>
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
 #include <new>
 #include <string>
 #include <vector>
@@ -124,6 +139,84 @@ publish_kernel(PeerTable peers, int me, int world, size_t off_ack, size_t off_sl
     }
 }
 
+// Where rank r's section lies in every range inbox (byte offsets; strides in elements)
+struct RangeLayout {
+    size_t off_ack, off_hdr, off_items, off_scores;
+    int64_t hdr_stride, cap;
+};
+
+// Range publish: this rank's section of its own inbox — n_hdr16 16-byte vectors of header, n_items16 of items,
+// n_scores16 of scores — into the same section of every peer's inbox, then range_arrive[me] = seq everywhere.  Waits
+// first until every peer acknowledged the previous round (range_ack[w] >= seq - 1 in this rank's inbox).
+__global__ void __launch_bounds__(256)
+range_publish_kernel(PeerTable inbox, int me, int world, RangeLayout L, int64_t n_hdr16, int64_t n_items16,
+                     int64_t n_scores16, uint32_t seq, uint32_t* ticket) {
+    __shared__ int s_last;
+    if (blockIdx.x == 0 && threadIdx.x < world && threadIdx.x != me)
+        spin_until(reinterpret_cast<const uint32_t*>(inbox.region[me] + L.off_ack) + threadIdx.x, seq - 1);
+    if (blockIdx.x == 0) {  // the other CTAs wait for CTA 0's acks through the ticket's high bit (publish_kernel)
+        __syncthreads();
+        if (threadIdx.x == 0) atomicOr(ticket, 0x80000000u);
+    } else if (threadIdx.x == 0) {
+        const long long t0 = clock64();
+        while (!(atomicAdd(ticket, 0u) & 0x80000000u)) {
+            if (clock64() - t0 > kSpinLimit) __trap();
+            __nanosleep(32);
+        }
+    }
+    __syncthreads();
+    const size_t hdr = L.off_hdr + static_cast<size_t>(me) * L.hdr_stride * 8;
+    const size_t items = L.off_items + static_cast<size_t>(me) * L.cap * 8;
+    const size_t scores = L.off_scores + static_cast<size_t>(me) * L.cap * 4;
+    const int64_t n = n_hdr16 + n_items16 + n_scores16;
+    for (int w = 0; w < world; ++w) {
+        if (w == me) continue;
+        for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+             i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+            size_t off;
+            if (i < n_hdr16) off = hdr + 16 * i;
+            else if (i < n_hdr16 + n_items16) off = items + 16 * (i - n_hdr16);
+            else off = scores + 16 * (i - n_hdr16 - n_items16);
+            *reinterpret_cast<uint4*>(inbox.region[w] + off) = *reinterpret_cast<const uint4*>(inbox.region[me] + off);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence_system();
+        const uint32_t t = atomicAdd(ticket, 1u) & 0x7FFFFFFFu;
+        s_last = t == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (s_last) {
+        if (threadIdx.x < world) {
+            __threadfence_system();
+            st_release_sys(reinterpret_cast<uint32_t*>(inbox.region[threadIdx.x]) + me, seq);  // range_arrive[me]
+        }
+        if (threadIdx.x == 0) *ticket = 0;
+    }
+}
+
+// Range wait: every rank's round `seq` arrived in this inbox; its headers (n_words each) -> out [world][n_words]
+// (mapped pinned host memory)
+__global__ void __launch_bounds__(256)
+range_wait_kernel(const char* inbox, int world, RangeLayout L, uint32_t seq, int n_words, int64_t* out) {
+    if (threadIdx.x < world) spin_until(reinterpret_cast<const uint32_t*>(inbox) + threadIdx.x, seq);
+    __syncthreads();
+    const int64_t* hdr = reinterpret_cast<const int64_t*>(inbox + L.off_hdr);
+    for (int i = threadIdx.x; i < world * n_words; i += blockDim.x) {
+        const int r = i / n_words;
+        out[i] = __ldcg(hdr + r * L.hdr_stride + (i - r * n_words));
+    }
+}
+
+// Range ack: this rank no longer reads round `seq` of its inbox: range_ack[me] = seq in every peer's inbox
+__global__ void range_ack_kernel(PeerTable inbox, int me, int world, size_t off_ack, uint32_t seq) {
+    if (threadIdx.x < world && threadIdx.x != me) {
+        __threadfence_system();
+        st_release_sys(reinterpret_cast<uint32_t*>(inbox.region[threadIdx.x] + off_ack) + me, seq);
+    }
+}
+
 }  // namespace
 
 }  // namespace tav
@@ -159,7 +252,30 @@ struct tav_group {
     };
     std::vector<OpenSearch> open;     // ascending, consecutive sequence numbers ending at `seq`
     int outstanding = 0;              // deferred sharded searches since the last finish
+    // threshold searches (tav_group_range_*, tav_sharded_range_*): the range inbox
+    char* rin = nullptr;              // this rank's range inbox (cudaMalloc), or none
+    PeerTable rpeers{};               // range inbox of every rank, as mapped here
+    RangeLayout rl{};
+    size_t rin_bytes = 0;
+    int rin_queries = 0;              // queries a header holds
+    bool rin_connected = false;
+    int64_t rin_limit = -1;           // tests: the largest inbox a reserve may allocate (-1: no cap)
+    uint32_t rseq = 0;                // rounds published into the current inbox
+    uint32_t* rticket = nullptr;      // device counter of the range publish kernel
+    int64_t* rhdr_host = nullptr;     // pinned, mapped: the world's headers of the last round
+    struct OpenRange {                // the range search between tav_sharded_range_search and its merge
+        bool open = false;
+        tav_index* ix = nullptr;
+        int nq = 0;
+        int64_t total = 0;
+        bool positions_form = false;
+        int64_t* positions = nullptr;  // device copy of the caller's positions (stream-ordered), until the close
+        int64_t positions_len = 0;
+        std::vector<int64_t> hdr;     // this rank's header: offsets [nq + 1], status | included << 1
+    } rs;
 };
+
+static std::atomic<int64_t> g_range_bytes{0};  // range inbox bytes held by every group of the process
 
 static inline size_t a16(size_t v) { return (v + 15) & ~size_t(15); }
 static inline size_t a8(size_t v) { return (v + 7) & ~size_t(7); }
@@ -254,10 +370,40 @@ int tav_group_connect(tav_group* g, const void* handles) {
     return TAV_OK;
 }
 
+// the device copy of an open range search's positions, freed (the device is idle or the call synchronises)
+static void range_drop_positions(tav_group* g) {
+    if (g->rs.positions) cudaFree(g->rs.positions);
+    g->rs.positions = nullptr;
+}
+
+// the range inbox and its peers' mappings, gone: the next threshold search needs a reserve
+static void range_free(tav_group* g) {
+    for (int r = 0; r < g->world; ++r) {
+        if (r != g->rank && g->rpeers.region[r]) cudaIpcCloseMemHandle(g->rpeers.region[r]);
+        g->rpeers.region[r] = nullptr;
+    }
+    if (g->rin) {
+        cudaFree(g->rin);
+        g_range_bytes -= static_cast<int64_t>(g->rin_bytes);
+    }
+    if (g->rhdr_host) cudaFreeHost(g->rhdr_host);
+    g->rin = nullptr;
+    g->rhdr_host = nullptr;
+    g->rin_bytes = 0;
+    g->rin_queries = 0;
+    g->rl = RangeLayout{};
+    g->rin_connected = false;
+    g->rseq = 0;
+    g->rs.open = false;
+}
+
 int tav_group_destroy(tav_group* g) {
     if (!g) return TAV_OK;
     cudaSetDevice(g->device);
     cudaDeviceSynchronize();
+    range_free(g);
+    range_drop_positions(g);
+    if (g->rticket) cudaFree(g->rticket);
     for (int r = 0; r < g->world; ++r)
         if (r != g->rank && g->peers.region[r]) cudaIpcCloseMemHandle(g->peers.region[r]);
     if (g->region) cudaFree(g->region);
@@ -548,6 +694,301 @@ int tav_sharded_finish(tav_index* ix, tav_group* g, void* stream, int* redone_to
         return TAV_ERR_PEER;
     }
     return TAV_OK;
+}
+
+// ---- threshold searches through the range inbox ----------------------------------------------------------------
+
+int tav_group_range_reserve(tav_group* g, int max_queries, int64_t capacity) {
+    if (!g || max_queries < 0 || capacity < 0) {
+        set_error("tav_group_range_reserve: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    TAVG_CUDA(cudaSetDevice(g->device));
+    const bool open = g->rs.open;  // a grow between the rounds of a search keeps it open (its state is host-side)
+    range_free(g);
+    if (max_queries == 0 || capacity == 0) {
+        range_drop_positions(g);
+        return TAV_OK;
+    }
+    RangeLayout L{};
+    L.hdr_stride = (static_cast<int64_t>(max_queries) + 2 + 1) & ~int64_t(1);  // 16-byte rows
+    L.cap = (capacity + 15) & ~int64_t(15);                                    // 16-byte item and score sections
+    const size_t W = static_cast<size_t>(g->world);
+    L.off_ack = a16(W * 4);
+    L.off_hdr = (L.off_ack + a16(W * 4) + 255) & ~size_t(255);
+    L.off_items = (L.off_hdr + W * L.hdr_stride * 8 + 255) & ~size_t(255);
+    L.off_scores = (L.off_items + W * L.cap * 8 + 255) & ~size_t(255);
+    const size_t bytes = L.off_scores + W * L.cap * 4;
+    if (g->rin_limit >= 0 && bytes > static_cast<size_t>(g->rin_limit)) {
+        range_drop_positions(g);
+        set_error("tav_group_range_reserve: an inbox of %zu bytes exceeds the test cap of %lld", bytes,
+                  static_cast<long long>(g->rin_limit));
+        return TAV_ERR_OOM;
+    }
+    cudaError_t e = cudaSuccess;
+    if (!g->rticket) {
+        e = cudaMalloc(reinterpret_cast<void**>(&g->rticket), 64);
+        if (e == cudaSuccess) e = cudaMemset(g->rticket, 0, 64);
+    }
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&g->rin), bytes);
+    if (e == cudaSuccess) {
+        g->rin_bytes = bytes;
+        g_range_bytes += static_cast<int64_t>(bytes);
+        e = cudaMemset(g->rin, 0, L.off_hdr);  // arrive and ack words
+    }
+    if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&g->rhdr_host), W * L.hdr_stride * 8);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();  // the words are zero before a peer can map them
+    if (e != cudaSuccess) {
+        set_error("tav_group_range_reserve: %s (an inbox of %zu bytes)", cudaGetErrorString(e), bytes);
+        range_free(g);
+        range_drop_positions(g);
+        return e == cudaErrorMemoryAllocation ? TAV_ERR_OOM : TAV_ERR_CUDA;
+    }
+    g->rl = L;
+    g->rin_queries = max_queries;
+    g->rpeers.region[g->rank] = g->rin;
+    g->rin_connected = g->world == 1;
+    g->rs.open = open;
+    return TAV_OK;
+}
+
+int tav_group_range_handle(tav_group* g, void* handle_out) {
+    if (!g || !handle_out || !g->rin) {
+        set_error("tav_group_range_handle: no range inbox (tav_group_range_reserve)");
+        return TAV_ERR_STATE;
+    }
+    TAVG_CUDA(cudaSetDevice(g->device));
+    cudaIpcMemHandle_t h;
+    TAVG_CUDA(cudaIpcGetMemHandle(&h, g->rin));
+    memcpy(handle_out, &h, sizeof(h));
+    return TAV_OK;
+}
+
+int tav_group_range_connect(tav_group* g, const void* handles) {
+    if (!g || !handles || !g->rin) {
+        set_error("tav_group_range_connect: no range inbox (tav_group_range_reserve)");
+        return TAV_ERR_STATE;
+    }
+    TAVG_CUDA(cudaSetDevice(g->device));
+    for (int r = 0; r < g->world; ++r) {
+        if (r == g->rank || g->rpeers.region[r]) continue;
+        cudaIpcMemHandle_t h;
+        memcpy(&h, static_cast<const char*>(handles) + static_cast<size_t>(r) * sizeof(h), sizeof(h));
+        void* p = nullptr;
+        TAVG_CUDA(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
+        g->rpeers.region[r] = static_cast<char*>(p);
+    }
+    g->rin_connected = true;
+    return TAV_OK;
+}
+
+int tav_group_range_capacity(const tav_group* g, int* max_queries, int64_t* capacity) {
+    if (!g) return TAV_ERR_INVALID;
+    if (max_queries) *max_queries = g->rin_connected ? g->rin_queries : 0;
+    if (capacity) *capacity = g->rin_connected ? g->rl.cap : 0;
+    return TAV_OK;
+}
+
+int tav_internal_range_bytes(const tav_group* g, int64_t* group_bytes, int64_t* process_bytes) {
+    if (!g) return TAV_ERR_INVALID;
+    if (group_bytes) *group_bytes = static_cast<int64_t>(g->rin_bytes);
+    if (process_bytes) *process_bytes = g_range_bytes.load();
+    return TAV_OK;
+}
+
+int tav_internal_range_cap(tav_group* g, int64_t max_bytes) {
+    if (!g || max_bytes < -1) return TAV_ERR_INVALID;
+    g->rin_limit = max_bytes;
+    return TAV_OK;
+}
+
+}  // extern "C"
+
+// One round of the open range search: this rank's header, and its hits when `hits` (fetched from the index into its
+// own section, mapped to the caller's positions for the subset forms), published into every peer's inbox; then the
+// wait for every rank's round and the world's headers on the host.  Synchronises `s`.
+static int range_round(tav_group* g, bool hits, cudaStream_t s) {
+    tav_group::OpenRange& o = g->rs;
+    const RangeLayout& L = g->rl;
+    const uint32_t seq = ++g->rseq;
+    char* hdr = g->rin + L.off_hdr + static_cast<size_t>(g->rank) * L.hdr_stride * 8;
+    int64_t* items = reinterpret_cast<int64_t*>(g->rin + L.off_items + static_cast<size_t>(g->rank) * L.cap * 8);
+    float* scores = reinterpret_cast<float*>(g->rin + L.off_scores + static_cast<size_t>(g->rank) * L.cap * 4);
+    const int n_words = o.nq + 2;
+    TAVG_CUDA(cudaMemcpyAsync(hdr, o.hdr.data(), static_cast<size_t>(n_words) * 8, cudaMemcpyHostToDevice, s));
+    const int64_t n = hits ? o.total : 0;
+    if (n > 0) {
+        if (int rc = tav_range_fetch(o.ix, 0, n, items, scores, TAV_OUTPUTS_ON_DEVICE, s)) return rc;
+        if (o.positions_form) TAVG_CUDA(launch_map_items(n, o.positions, o.positions_len, items, s));
+    }
+    if (g->world > 1) {
+        int64_t n_items16 = (n * 8 + 15) / 16, n_scores16 = (n * 4 + 15) / 16;
+        if (TAV_PEER_RANGE_MUTANT == 1 && n_items16 > 0) n_items16 -= 1;
+        if (TAV_PEER_RANGE_MUTANT == 2 && g->rs.hdr[o.nq + 1] & 4) n_items16 = n_scores16 = 0;
+        const size_t bytes = static_cast<size_t>(n_words) * 8 + static_cast<size_t>(n) * 12;
+        const int grid = static_cast<int>(std::min<size_t>(128, std::max<size_t>(1, bytes / 2048)));
+        range_publish_kernel<<<grid, 256, 0, s>>>(g->rpeers, g->rank, g->world, L, (n_words * 8 + 15) / 16, n_items16,
+                                                  n_scores16, seq, g->rticket);
+        TAVG_CUDA(cudaGetLastError());
+    }
+    // (one rank publishes nothing: its wait only copies its own header out)
+    range_wait_kernel<<<1, 256, 0, s>>>(g->rin, g->world, L, g->world > 1 ? seq : 0u, n_words, g->rhdr_host);
+    TAVG_CUDA(cudaGetLastError());
+    TAVG_CUDA(cudaStreamSynchronize(s));
+    return TAV_OK;
+}
+
+// Close the open range search: this rank acknowledges its last round to every peer (nobody will wait for this rank
+// at the next publish) and frees the search's positions.
+static int range_close(tav_group* g, cudaStream_t s) {
+    g->rs.open = false;
+    if (g->rs.positions) {
+        cudaError_t e = cudaFreeAsync(g->rs.positions, s);
+        g->rs.positions = nullptr;
+        TAVG_CUDA(e);
+    }
+    if (g->world == 1 || !g->rin_connected) return TAV_OK;
+    range_ack_kernel<<<1, 32, 0, s>>>(g->rpeers, g->rank, g->world, g->rl.off_ack, g->rseq);
+    TAVG_CUDA(cudaGetLastError());
+    return TAV_OK;
+}
+
+extern "C" {
+
+int tav_sharded_range_search(tav_index* ix, tav_group* g, const float* queries, int n_queries, float min_score,
+                             int flags, const int64_t* subset, int64_t subset_len, const int64_t* offsets,
+                             const int64_t* positions, int64_t item_offset, int64_t expected_hits,
+                             int64_t* world_headers, void* stream) {
+    const bool positions_form = (flags & TAV_ITEMS_AS_POSITIONS) != 0;
+    if (!ix || !g || n_queries < 1 || !queries || !world_headers || subset_len < 0 || expected_hits < 0 ||
+        (positions_form && subset_len > 0 && (!subset || !positions)) ||
+        (offsets && (!positions_form || offsets[0] != 0 || offsets[n_queries] != subset_len))) {
+        set_error("tav_sharded_range_search: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    if (!g->rin_connected) {
+        set_error("tav_sharded_range_search: no connected range inbox (tav_group_range_reserve / _connect)");
+        return TAV_ERR_STATE;
+    }
+    if (n_queries > g->rin_queries) {
+        set_error("tav_sharded_range_search: %d queries exceed the range inbox's %d", n_queries, g->rin_queries);
+        return TAV_ERR_INVALID;
+    }
+    TAVG_CUDA(cudaSetDevice(g->device));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (g->rs.open)  // a search the caller left open (neither merged nor aborted) is closed first
+        if (int rc = range_close(g, s)) return rc;
+    tav_group::OpenRange& o = g->rs;
+    o.ix = ix;
+    o.nq = n_queries;
+    o.positions_form = positions_form;
+    o.positions_len = subset_len;
+    o.hdr.assign(static_cast<size_t>(n_queries) + 2, 0);
+    int lrc = TAV_OK;
+    const bool local = tav_size(ix) > 0 && !(positions_form && subset_len == 0);
+    if (local && positions_form) {
+        // the positions on the device, for tav_map_items at each round; a failure here is published like the
+        // search's own allocations
+        const size_t bytes = static_cast<size_t>(subset_len) * sizeof(int64_t);
+        cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&o.positions), bytes, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(o.positions, positions, bytes, cudaMemcpyHostToDevice, s);
+        if (e == cudaErrorMemoryAllocation) {
+            o.positions = nullptr;
+            set_error("tav_sharded_range_search: %zu bytes of positions: %s", bytes, cudaGetErrorString(e));
+            lrc = TAV_ERR_OOM;
+        } else {
+            TAVG_CUDA(e);
+        }
+    }
+    if (local && lrc == TAV_OK) {
+        const int ties = flags & TAV_TIES_LOW_FIRST;
+        if (offsets)
+            lrc = tav_range_search_subsets(ix, queries, n_queries, min_score, TAV_ITEMS_AS_POSITIONS | ties, offsets,
+                                           subset, o.hdr.data(), stream);
+        else
+            lrc = tav_range_search(ix, queries, n_queries, min_score,
+                                   flags & (TAV_FORCE_SCAN | TAV_FORCE_MMA | TAV_USE_ROW_MASK | TAV_USE_QUERY_MASKS |
+                                            TAV_TIES_LOW_FIRST | TAV_ITEMS_AS_POSITIONS),
+                                   positions_form ? subset : nullptr, positions_form ? subset_len : 0,
+                                   positions_form ? 0 : item_offset, expected_hits, o.hdr.data(), stream);
+    }
+    if (lrc == TAV_ERR_CUDA) {  // not published (the failure protocol of the top-k exchange)
+        range_drop_positions(g);
+        return lrc;
+    }
+    std::string error;
+    if (lrc != TAV_OK) {  // published as status 1 with no hits, so that no peer waits for this rank
+        error = tav_last_error();
+        cudaGetLastError();  // a failed allocation inside the search is not sticky (sharded_run)
+        std::fill(o.hdr.begin(), o.hdr.end(), 0);
+    }
+    o.total = o.hdr[n_queries];
+    const bool included = o.total <= g->rl.cap;
+    o.hdr[n_queries + 1] = (lrc != TAV_OK ? 1 : 0) | (included ? 2 : 0);
+    o.open = true;
+    if (int rc = range_round(g, included, s)) return rc;
+    const int n_words = n_queries + 2;
+    memcpy(world_headers, g->rhdr_host, static_cast<size_t>(g->world) * n_words * 8);
+    int failed = 0;
+    for (int r = 0; r < g->world; ++r)
+        if (TAV_PEER_RANGE_MUTANT != 3 || r == g->rank)
+            failed += static_cast<int>(world_headers[r * n_words + n_queries + 1] & 1);
+    if (lrc != TAV_OK || failed) {  // nobody merges this round: acknowledge it now
+        if (int rc = range_close(g, s)) return rc;
+        if (lrc != TAV_OK) {
+            set_error("%s", error.c_str());
+            return lrc;
+        }
+        set_error("tav_sharded_range_search: a rank's local search failed (%d of %d ranks)", failed, g->world);
+        return TAV_ERR_PEER;
+    }
+    return TAV_OK;
+}
+
+int tav_sharded_range_republish(tav_group* g, void* stream) {
+    if (!g || !g->rs.open || !g->rin_connected) {
+        set_error("tav_sharded_range_republish: no open range search, or no connected range inbox");
+        return TAV_ERR_STATE;
+    }
+    tav_group::OpenRange& o = g->rs;
+    if (o.nq > g->rin_queries || o.total > g->rl.cap) {
+        set_error("tav_sharded_range_republish: %d queries, %lld hits exceed the range inbox (%d, %lld)", o.nq,
+                  static_cast<long long>(o.total), g->rin_queries, static_cast<long long>(g->rl.cap));
+        range_close(g, static_cast<cudaStream_t>(stream));
+        return TAV_ERR_INVALID;
+    }
+    TAVG_CUDA(cudaSetDevice(g->device));
+    o.hdr[o.nq + 1] = 2 | 4;  // hits included (a failed search never gets here); 4: a republish (not read by the merge)
+    return range_round(g, true, static_cast<cudaStream_t>(stream));
+}
+
+int tav_sharded_range_merge(tav_group* g, int ties_low_first, int64_t* out_offsets, int64_t* out_items,
+                            float* out_scores, void* stream) {
+    if (!g || !g->rs.open) {
+        set_error("tav_sharded_range_merge: no open range search");
+        return TAV_ERR_STATE;
+    }
+    TAVG_CUDA(cudaSetDevice(g->device));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const RangeLayout& L = g->rl;
+    const int rc = tav_merge_range(g->device, g->world, g->rs.nq, reinterpret_cast<const int64_t*>(g->rin + L.off_hdr),
+                                   L.hdr_stride, reinterpret_cast<const int64_t*>(g->rin + L.off_items), L.cap,
+                                   reinterpret_cast<const float*>(g->rin + L.off_scores), L.cap, ties_low_first,
+                                   out_offsets, out_items, out_scores, stream);
+    std::string error = rc != TAV_OK ? tav_last_error() : "";
+    const int arc = range_close(g, s);  // also after a failed merge: no peer may wait for this round
+    if (rc != TAV_OK) {
+        set_error("%s", error.c_str());
+        return rc;
+    }
+    return arc;
+}
+
+int tav_sharded_range_abort(tav_group* g, void* stream) {
+    if (!g) return TAV_ERR_INVALID;
+    if (!g->rs.open) return TAV_OK;
+    TAVG_CUDA(cudaSetDevice(g->device));
+    return range_close(g, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -234,6 +234,15 @@ cudaError_t launch_map_items(int64_t n, const int64_t* table, int64_t table_len,
 #define TAV_PEER_FILTER_MUTANT 0
 #endif
 
+// TAV_PEER_RANGE_MUTANT (tests only, never set by build.py): 1..3 compile one deliberate defect each into the
+// threshold search of the peer exchange (tav_sharded_range_*), so that tests/test_gpu_peer_range.py can show its
+// checks catch it: 1 a publish stores one 16-byte vector fewer of the items into the peers, 2 a republish after a grow
+// stores the header (and raises the flag) but no hits, 3 a rank adds up only its own status word (a peer's failure is
+// not reported).  Every wait of the protocol stays satisfiable and nothing is read outside an allocation.
+#ifndef TAV_PEER_RANGE_MUTANT
+#define TAV_PEER_RANGE_MUTANT 0
+#endif
+
 // ---- compaction after a removal (tav_compact.cu) -----------------------------------------
 // keys: device [m], keys[i] = rem[i] - i over the sorted distinct removed ordinals.  Destinations
 // [d_begin, d_end) of the compacted rows: dst row (d - d_base) = src row (d + #{keys <= d}).  src and dst
@@ -346,6 +355,12 @@ extern "C" int tav_internal_search_alloc_fail(tav_index* ix, int on);
 // library-internal: bytes of this index's library-owned row allocation and staged block, and bytes held in such row
 // blocks by every index of the process.  Tests use it to see that a rebalance frees the block it replaced.
 extern "C" int tav_internal_row_bytes(tav_index* ix, int64_t* index_bytes, int64_t* process_bytes);
+// library-internal: bytes of this group's range inbox, and bytes held in range inboxes by every group of the process.
+// Tests use it to see what a group keeps between threshold searches.
+extern "C" int tav_internal_range_bytes(const tav_group* g, int64_t* group_bytes, int64_t* process_bytes);
+// Tests only: tav_group_range_reserve fails with TAV_ERR_OOM, as a failed allocation does, for an inbox of more than
+// max_bytes bytes (-1: no cap), so that one rank's grow can fail without a device fault.
+extern "C" int tav_internal_range_cap(tav_group* g, int64_t max_bytes);
 
 // TAV_REBALANCE_MUTANT (tests only, never set by build.py): 1..3 compile one deliberate defect each into the
 // rebalance (tav_rows_stage / tav_rows_commit), so that tests/test_gpu_rebalance.py can show its exact checks catch

@@ -18,8 +18,10 @@ Two exchanges:
     drive over ``gloo`` with an injected engine).
 
 Threshold searches (``search_range``; ``max_hits=0`` lookups and ``search_arrays`` with k >= rows > 8192) have
-results whose size is known only after the local searches: they exchange over the process group (offsets, then
-the hits padded to the largest rank's total) and merge with ``tav_merge_range``.
+results whose size is known only after the local searches.  With ``exchange="peer"`` they go through the group's
+range inbox (``tav_sharded_range_*``: every rank's offsets and hits stored into its peers' inboxes, the inboxes
+grown collectively when a rank's hits do not fit); otherwise they exchange over the process group (offsets, then
+the hits padded to the largest rank's total).  Either way ``tav_merge_range`` merges them.
 
 Filtered and subset lookups (``predicate=``, ``fuzzy_lookup_embedding_in_subset``, ``subset=`` / ``allowed=`` /
 ``ties_low_first=``) return what ``VectorBase`` returns for the whole corpus, tie order included.  With
@@ -103,6 +105,57 @@ def rebalance_plan(old_starts, new_starts) -> list[tuple[int, int, int, int]]:
 MIRROR_ROUND_BYTES = 256 << 20
 
 
+RANGE_MIN_HITS = 1 << 12       # the smallest range inbox: hits per rank
+RANGE_RETAIN_BYTES = 64 << 20  # the most hit capacity a group keeps in its range inbox between threshold searches
+
+
+def pow2_at_least(n: int, floor: int) -> int:
+    """The smallest power of two that is at least ``n`` and ``floor``."""
+    return 1 << (max(int(n), int(floor), 1) - 1).bit_length()
+
+
+def range_retain_hits(world: int, retain_bytes: int = RANGE_RETAIN_BYTES) -> int:
+    """Hits per rank the range inbox keeps between threshold searches: the largest power of two whose hits from
+    every rank (12 bytes each) fit in ``retain_bytes``, and at least ``RANGE_MIN_HITS``."""
+    per = max(int(retain_bytes) // (12 * max(world, 1)), 1)
+    return max(1 << (per.bit_length() - 1), RANGE_MIN_HITS)
+
+
+def range_capacity_plan(totals, capacity: int, retain: int) -> tuple[int | None, int | None]:
+    """(grow, keep) of one threshold search through the range inbox, from every rank's total (replicated, so
+    every rank plans alike) and the inbox's capacity in hits per rank: ``grow`` is the capacity to reserve before
+    round 2 (the next power of two of the largest total), None when round 1 held every rank's hits; ``keep`` the
+    capacity to give the excess back to at the end of the call, None when the inbox is within ``retain``."""
+    t_max = int(np.max(totals)) if len(totals) else 0
+    grow = pow2_at_least(t_max, RANGE_MIN_HITS) if t_max > capacity else None
+    after = capacity if grow is None else grow
+    return grow, (retain if after > retain else None)
+
+
+def reserve_everywhere(dist, process_group, world: int, reserve, release) -> list[bytes]:
+    """Collective: ``reserve()`` on every rank (an allocation; returns its handle), then every rank's (status,
+    handle) through ``all_gather_object``.  If any rank failed, every rank runs ``release()`` and raises: its own
+    error, else MemoryError when some rank ran out of memory, else RuntimeError.  Returns the handles in rank
+    order."""
+    status, handle, error = 0, b"", None
+    try:
+        handle = reserve()
+    except Exception as e:  # noqa: BLE001
+        status, error = (2 if isinstance(e, MemoryError) else 1), e
+    got = [(status, handle)]
+    if world > 1:
+        got = [None] * world
+        dist.all_gather_object(got, (status, handle), group=process_group)
+    worst = max(st for st, _ in got)
+    if worst:
+        release()
+        if error is not None:
+            raise error
+        raise (MemoryError if worst == 2 else RuntimeError)("search_range: another rank failed to reserve its "
+                                                            "range inbox")
+    return [h for _, h in got]
+
+
 def packed_layout(n_queries: int, k: int) -> tuple[int, int, int]:
     """Byte offsets (scores, counts) and total size of one rank's packed candidate buffer:
     [items int64 B*k | scores float32 B*k | counts int32 B], each section 8-byte aligned."""
@@ -124,6 +177,8 @@ class CudaShardEngine:
         self.base = VectorBase(settings, device=device, storage_dtype=storage_dtype)
         self._group = None        # tav_group handle (peer exchange)
         self._group_keep = []     # outputs of deferred group searches, alive until finish
+        self._range_cap_hint = RANGE_MIN_HITS  # range inbox capacity the last threshold search needed
+        self.last_range_rounds = 0  # rounds (1, or 2 after a grow) of the last threshold search through the inbox
 
     # ---- peer exchange (tav_group) --------------------------------------------------------
     GROUP_DEPTH = 8
@@ -206,6 +261,125 @@ class CudaShardEngine:
             raise error
         _capi.check(rc)
         return items, scores, counts
+
+    # ---- threshold search through the peer exchange (the group's range inbox) ---------------------------------
+    RANGE_RETAIN_BYTES = RANGE_RETAIN_BYTES
+
+    def range_capacity(self) -> tuple[int, int]:
+        """(queries, hits per rank) the group's connected range inbox holds; (0, 0) without one."""
+        if self._group is None:
+            return 0, 0
+        mq, cap = C.c_int(0), C.c_int64(0)
+        _capi.check(_capi.load().tav_group_range_capacity(self._group, C.byref(mq), C.byref(cap)))
+        return mq.value, cap.value
+
+    def _range_reserve(self, dist, process_group, world: int, n_queries: int, capacity: int) -> None:
+        """Collective: every rank's range inbox replaced by one for ``n_queries`` queries and ``capacity`` hits per
+        rank, as ``_ensure_group`` makes a region: quiesce and wait for every rank, reserve, exchange (status,
+        handle), connect.  If any rank fails (MemoryError for an allocation), every rank frees its inbox and raises,
+        so that all ranks hold none and the next search reserves again; so does a failed connect."""
+        lib = _capi.load()
+        self.torch.cuda.synchronize(self.device)
+        dist.barrier(group=process_group)       # nobody still reads or publishes into an inbox about to die
+
+        def reserve() -> bytes:
+            _capi.check(lib.tav_group_range_reserve(self._group, n_queries, capacity))
+            buf = C.create_string_buffer(lib.tav_group_handle_bytes())
+            _capi.check(lib.tav_group_range_handle(self._group, buf))
+            return bytes(buf.raw)
+
+        release = lambda: lib.tav_group_range_reserve(self._group, 0, 0)  # noqa: E731
+        handles = reserve_everywhere(dist, process_group, world, reserve, release)
+        # the connect is agreed too (its gather is the barrier after it): every rank holds a connected inbox, or none
+        reserve_everywhere(dist, process_group, world,
+                           lambda: _capi.check(lib.tav_group_range_connect(self._group, b"".join(handles))) or b"",
+                           release)
+
+    def group_range(self, dist, process_group, rank: int, world: int, queries: np.ndarray, min_score: float,
+                    item_offset: int, ties_low_first: bool, mask=None, mask_key=None, mask_owner=None, subset=None,
+                    positions=None, subsets=None):
+        """One threshold search through the peer exchange (``tav_sharded_range_*``), collective.  Local arguments as
+        ``range_local`` takes them; returns device tensors (offsets int64 [B + 1], items int64 [T], scores float32
+        [T]), items being positions in the caller's subset(s) for the subset forms.  Round 1 publishes every rank's
+        header, and its hits when they fit in the inbox; if some rank's did not, every rank reserves an inbox for
+        the largest total and publishes again (``range_capacity_plan``).  A local failure (a mask upload here, or the
+        local search) is still published, so that every peer raises too.  A failure after round 1 (the output
+        allocation, say) closes the round on this rank (``tav_sharded_range_abort``: its peers' next publish does
+        not wait for it) and raises on this rank only, after the give-back every rank runs; the peers' results are
+        complete.  A failed grow raises on every rank."""
+        torch = self.torch
+        b = len(queries)
+        group = self._ensure_group(dist, process_group, rank, world, 1, 1)
+        retain = range_retain_hits(world, self.RANGE_RETAIN_BYTES)
+        mq, cap = self.range_capacity()
+        if b > mq:
+            mq, cap = pow2_at_least(b, 64), min(max(cap, self._range_cap_hint), retain)
+            self._range_reserve(dist, process_group, world, mq, cap)
+        base = self.base
+        lib, ix = base._ensure_device()
+        q = np.ascontiguousarray(queries, np.float32)
+        flags = (base._flags() & ~_capi.TAV_NO_FUSED_SCAN) | (_capi.TAV_TIES_LOW_FIRST if ties_low_first else 0)
+        error, sub, offs, pos = None, None, None, None
+        if mask is not None:
+            flags |= _capi.TAV_USE_QUERY_MASKS if np.ndim(mask) == 2 else _capi.TAV_USE_ROW_MASK
+        if subset is not None or subsets is not None:
+            flags |= _capi.TAV_ITEMS_AS_POSITIONS
+            sub = np.ascontiguousarray(subset if subsets is None else subsets[1], np.int64)
+            offs = None if subsets is None else np.ascontiguousarray(subsets[0], np.int64)
+            pos = np.ascontiguousarray(positions, np.int64)  # the library copies them (a failure there is published)
+        headers = np.zeros((world, b + 2), np.int64)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        keep, totals, out = None, None, None
+        base._single_lock.acquire()  # the index holds the hits until the last round has published them
+        try:
+            if mask is not None:
+                try:
+                    self.upload_mask((mask, mask_key, mask_owner), b)
+                except Exception as e:  # noqa: BLE001
+                    error = e
+                    self._drop_masks(lib, ix)  # the local search then fails and publishes this rank's failure
+            rc = lib.tav_sharded_range_search(
+                ix, group, q.ctypes.data_as(C.c_void_p), b, C.c_float(min_score), flags,
+                None if sub is None else sub.ctypes.data_as(C.c_void_p), 0 if sub is None else len(sub),
+                None if offs is None else offs.ctypes.data_as(C.c_void_p),
+                None if pos is None else pos.ctypes.data_as(C.c_void_p), item_offset, base._range_hint,
+                headers.ctypes.data_as(C.c_void_p), C.c_void_p(stream))
+            if error is not None:
+                raise error
+            _capi.check(rc)  # a failure of any rank's local search: raised on every rank, the round closed
+            totals = headers[:, b]
+            base._range_hint = int(totals[rank])
+            grow, keep = range_capacity_plan(totals, cap, retain)
+            self.last_range_rounds = 1
+            if grow is not None:
+                try:
+                    self._range_reserve(dist, process_group, world, mq, grow)
+                except Exception:
+                    keep = None  # every rank raised and holds no inbox: nothing to give back
+                    raise
+                _capi.check(lib.tav_sharded_range_republish(group, C.c_void_p(stream)))
+                self.last_range_rounds = 2
+            total = int(totals.sum())
+            out_offsets = torch.empty(b + 1, dtype=torch.int64, device=self.device)
+            items = torch.empty(max(total, 1), dtype=torch.int64, device=self.device)
+            scores = torch.empty(max(total, 1), dtype=torch.float32, device=self.device)
+            _capi.check(lib.tav_sharded_range_merge(group, int(ties_low_first), C.c_void_p(out_offsets.data_ptr()),
+                                                    C.c_void_p(items.data_ptr()), C.c_void_p(scores.data_ptr()),
+                                                    C.c_void_p(stream)))
+            out = out_offsets, items[:total], scores[:total]
+        except Exception as e:  # noqa: BLE001
+            error = e
+            # a round still open on this rank is acknowledged, so that no peer's next publish waits for it
+            lib.tav_sharded_range_abort(group, C.c_void_p(stream))
+        finally:
+            base._single_lock.release()
+        if totals is not None:
+            self._range_cap_hint = min(pow2_at_least(int(totals.max()), RANGE_MIN_HITS), retain)
+        if keep is not None:  # give the excess back, on every rank alike (the totals are replicated)
+            self._range_reserve(dist, process_group, world, mq, keep)
+        if error is not None:
+            raise error
+        return out
 
     def upload_mask(self, mask, n_queries: int) -> None:
         """Put this block's mask (words, key, owner) on the device unless it is there already."""
@@ -1095,7 +1269,7 @@ class ShardedVectorBase:
         per query: bool [B, N] or packed words [B, ceil(N / 32)]), with its results and
         errors.  With ``exchange="peer"`` such lookups go through the peer exchange (``tav_sharded_search`` /
         ``tav_sharded_search_subset``), otherwise over the process group; threshold routes (k >= rows > 8192, per-query
-        subsets with k > 2048) always exchange over the process group."""
+        subsets with k > 2048) exchange as ``search_range`` does."""
         if subsets is not None:
             return self._search_arrays_subsets(queries, k, min_score, subsets, subset, allowed, ties_low_first)
         if subset is not None or allowed is not None or ties_low_first:
@@ -1363,9 +1537,8 @@ class ShardedVectorBase:
         """The threshold search of validated per-query subsets: flat positions merged, then decoded."""
         lo, hi = self.local_range
         positions, local_offsets, local_ordinals = subsets_share(offsets, ordinals, len(self), lo, hi)
-        return self._range_exchange(q, floor, ties_low_first, lambda: self._engine.range_local(
-            q, float(floor), lo, bool(ties_low_first), subsets=(local_offsets, local_ordinals), positions=positions),
-            decode=ordinals)
+        return self._range_exchange(q, floor, ties_low_first, dict(subsets=(local_offsets, local_ordinals),
+                                                                   positions=positions), decode=ordinals)
 
     def search_range(self, queries, min_score: float = 0.0, ties_low_first: bool = False, subset=None, allowed=None,
                      subsets=None):
@@ -1381,7 +1554,8 @@ class ShardedVectorBase:
         collective), a second one every rank's hits, padded to the largest rank's total (after a one-word
         all-reduce that makes a failure to stage them raise on every rank); ``tav_merge_range`` merges them on
         every rank.  A subset search merges positions in the subset and decodes them through the caller's list
-        afterwards.  The exchanges go through the process group whatever ``exchange`` says.  At most
+        afterwards.  With ``exchange="peer"`` the exchange is the group's range inbox instead (``group_range``:
+        no process-group collective unless the inbox must be reserved or grown).  At most
         ``MAX_RANGE_RANKS`` (32) ranks: larger groups get ValueError on every rank before any exchange.
         ``subsets`` (one integer sequence per query) as ``VectorBase.search_range`` takes it."""
         if subsets is not None:
@@ -1415,9 +1589,7 @@ class ShardedVectorBase:
             return np.zeros(b + 1, np.int64), np.empty(0, np.int64), np.empty(0, np.float32)
         if q.shape[1] != self._embedding_size:
             raise ValueError("query width does not match the embedding size")
-        lo, _ = self.local_range
-        return self._range_exchange(q, floor, ties_low_first,
-                                    lambda: self._engine.range_local(q, float(floor), lo, bool(ties_low_first)))
+        return self._range_exchange(q, floor, ties_low_first)
 
     def _search_range_filtered(self, q, floor, ties_low_first, sub, mask):
         """The threshold search of validated arguments with a subset (int64, in range), this block's mask, or
@@ -1425,28 +1597,39 @@ class ShardedVectorBase:
         lo, hi = self.local_range
         if sub is not None:
             positions, local_sub = subset_share(sub, len(self), lo, hi)
-            return self._range_exchange(q, floor, ties_low_first, lambda: self._engine.range_local(
-                q, float(floor), lo, bool(ties_low_first), subset=local_sub, positions=positions), decode=sub)
+            return self._range_exchange(q, floor, ties_low_first, dict(subset=local_sub, positions=positions),
+                                        decode=sub)
         if mask is None:
-            return self._range_exchange(q, floor, ties_low_first, lambda: self._engine.range_local(
-                q, float(floor), lo, bool(ties_low_first)))
+            return self._range_exchange(q, floor, ties_low_first)
         self.finish()  # the mask upload finishes this rank's deferred searches; their exchange is redone here
         words, key, owner = mask
-        return self._range_exchange(q, floor, ties_low_first, lambda: self._engine.range_local(
-            q, float(floor), lo, bool(ties_low_first), mask=words, mask_key=key, mask_owner=owner))
+        return self._range_exchange(q, floor, ties_low_first, dict(mask=words, mask_key=key, mask_owner=owner),
+                                    mask=mask)
 
-    def _range_exchange(self, q, floor, ties_low_first, search, decode=None):
-        """Both exchanges and the merge of a threshold search whose local part is ``search()`` (a LocalRange);
-        ``decode``: merged items are positions in this list, replaced by its entries on the device."""
+    def _range_exchange(self, q, floor, ties_low_first, local_args=None, decode=None, mask=None):
+        """The exchange and the merge of a threshold search whose local part is ``range_local`` with
+        ``local_args``; ``decode``: merged items are positions in this list, replaced by its entries on the device;
+        ``mask``: this block's mask (words, key, owner) when ``local_args`` carries one.  Through the peer exchange
+        (``group_range``) when the lookups use it, otherwise over the process group."""
         import torch
 
         b = len(q)
         empty = (np.zeros(b + 1, np.int64), np.empty(0, np.int64), np.empty(0, np.float32))
         if self.world > MAX_RANGE_RANKS:
             raise ValueError(f"search_range merges at most {MAX_RANGE_RANKS} ranks (tav_merge_range), not {self.world}")
+        local_args = local_args or {}
+        lo, _ = self.local_range
+        if self._peer() and hasattr(self._engine, "group_range"):
+            if mask is not None:
+                self._agree_mask(mask, b)
+            out = self._engine.group_range(self._dist, self._group, self.rank, self.world, q, float(floor), lo,
+                                           bool(ties_low_first), **local_args)
+            if decode is not None:
+                self._engine.map_items(out[1], decode)  # subset positions -> the caller's ordinals, as given
+            return tuple(np.asarray(t.cpu().numpy() if hasattr(t, "cpu") else t) for t in out)
         error, local = None, None
         try:
-            local = search()
+            local = self._engine.range_local(q, float(floor), lo, bool(ties_low_first), **local_args)
             offsets = np.asarray(local.offsets, np.int64)
         except Exception as e:  # noqa: BLE001
             error, offsets = e, np.zeros(b + 1, np.int64)
