@@ -202,9 +202,43 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
                      const int64_t* subset, int64_t subset_len, int64_t item_offset,
                      int64_t expected_hits, int64_t* out_offsets, void* stream);
 /* Copy hits [first, first + n) of the last range search (items = row + item_offset, or the
- * subset ordinal + item_offset; scores float32) to host or device (TAV_OUTPUTS_ON_DEVICE) memory. */
+ * subset ordinal + item_offset; scores float32) to host or device (TAV_OUTPUTS_ON_DEVICE) memory.
+ * After a tav_range_search_into, TAV_ERR_STATE until the next tav_range_search. */
 int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items, float* out_scores,
                     int flags, void* stream);
+
+/* Threshold search into the caller's device memory, sized on the device: the result of tav_range_search (same
+ * order, score map, float32 compare, item_offset, shared subset of host ordinals, masks, NaN rules, path choice
+ * and fp16-range fallback) without reading the hit counts back to the host first.
+ *   out_offsets [n_queries + 1] int64   the full CSR offsets, also when out_offsets[n_queries] > capacity
+ *   out_items   [capacity]      int64   every hit whose CSR position is below capacity; positions at or
+ *   out_scores  [capacity]      float32 beyond it are never touched (the written hits are a prefix of the result)
+ * Positions between the total and capacity are not written either, with one exception: when a tensor-core
+ * re-pass (below) does not count what the first pass counted, the search is redone whole by the row scan, and
+ * hits of the first pass may remain between the new total and capacity.  A caller that finds the total above
+ * capacity can search again with enough room.  expected_hits sizes the collect regions as in tav_range_search
+ * (0 = library default, 16384 per query); device scratch of about 2 x 8 bytes per key of the regions (1.5 x the
+ * per-query share + 32, or twice that on the tensor cores) is held by the index.  Flags: QUERIES_ON_DEVICE,
+ * FORCE_SCAN, FORCE_MMA, USE_ROW_MASK, USE_QUERY_MASKS, TIES_LOW_FIRST, DEFER_RETRY; any other flag,
+ * capacity < 0 or a NULL output that is needed (items / scores with capacity > 0): TAV_ERR_INVALID.
+ * A query whose collect region (row scan) or segment (tensor cores) overflowed is flagged and searched again at
+ * the finish: all flagged queries of the search together, in one more pass of the collection that flagged them
+ * (gathered queries, regions of their counted size; the tensor cores with the same plan, so the re-pass must
+ * count what the first pass counted), sorted into these outputs at their offsets.  A split-form (float32 on the
+ * tensor cores) search that met a value beyond the fp16 range writes no hits and is searched again whole by the
+ * row scan, offsets included, as tav_range_search falls back.  Every search so redone counts its queries in
+ * *redone.  Without TAV_DEFER_RETRY the call finishes itself before it returns (like tav_search, with the other
+ * outstanding deferred searches): one synchronisation, and three or four when queries are searched again.
+ * With TAV_DEFER_RETRY the call makes no host synchronisation (growing a device buffer may allocate; a repeat call
+ * of the same shape does not) and joins the deferred searches tav_finish_search completes (at most 64
+ * outstanding, shared with tav_search); until then only the flagged queries' outputs (the whole search's, when
+ * flagged whole) are not final.  The caller keeps the device queries and the outputs alive until the finish (host
+ * queries, normalised queries and the subset are held by the library).  The hits of the last tav_range_search
+ * are given up (see tav_range_fetch); a finish never touches them. */
+int tav_range_search_into(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
+                          const int64_t* subset, int64_t subset_len, int64_t item_offset,
+                          int64_t expected_hits, int64_t capacity,
+                          int64_t* out_offsets, int64_t* out_items, float* out_scores, void* stream);
 
 /*
  * Per-query subsets: one batched lookup in which query q scores only its own entries
@@ -240,7 +274,9 @@ int tav_range_search_subsets(tav_index* ix, const float* queries, int n_queries,
  * then.  Up to 64 searches may be outstanding (a 65th finishes the earlier ones first, and the
  * queries redone then are not counted in *redone).  On a TAV_NORMALIZE index each outstanding
  * search keeps its normalised queries in device memory of its own (grown as needed, never by
- * finishing searches early) until this call.  No-op when nothing is pending. */
+ * finishing searches early) until this call.  Deferred tav_range_search_into searches are completed
+ * here too (their flagged queries searched again into their outputs at their offsets).  No-op when
+ * nothing is pending. */
 int tav_finish_search(tav_index* ix, void* stream, int* redone);
 
 /* Row mask for TAV_USE_ROW_MASK: `n_rows` bits (bit r of word r/32 = row r allowed), host or

@@ -57,6 +57,9 @@ SIGNATURES = {
     "tav_range_search_subsets": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p]),
     "tav_range_fetch": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "tav_range_search_into": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_int64,
+                                        C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p]),
     "tav_finish_search": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
     "tav_set_row_mask": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "tav_set_query_masks": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p]),

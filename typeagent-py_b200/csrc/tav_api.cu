@@ -122,6 +122,16 @@ struct Pending {
     bool split;
     const uint32_t* mask;  // the row mask, or query 0's per-query mask (query q's: mask + q * mask_stride)
     int64_t mask_stride;   // 0 for the row mask
+    // a threshold search into the caller's buffers (tav_range_search_into; k == 0): `items` / `scores` hold
+    // its first `cap` hits, `offsets` its CSR offsets
+    int64_t* offsets = nullptr;
+    int64_t cap = 0;
+    const int64_t* subset = nullptr;  // device ordinals (held, like normalised queries), or nullptr
+    int64_t n_scan = 0;
+    int ties_low = 0;
+    int64_t expected_hits = 0;
+    QueryMasks qm{};                  // per-query masks of the whole search (nq > 1)
+    int per_chunk = 0, n_seg = 0;     // the tensor-core collection plan a re-pass repeats (0: the row scan)
 };
 
 }  // namespace tav
@@ -205,6 +215,7 @@ struct tav_index {
     DevBuf range_mmaws, range_mmaws2, range_mmaaux;  // tensor-core collection: workspaces, scratch
     DevBuf range_items, range_scores;
     int64_t range_total = 0;     // hits of the last range search held in range_items / range_scores
+    bool range_replaced = false; // a tav_range_search_into ran after it: tav_range_fetch has nothing to copy
     // per-query subsets: device [offsets | work-item starts | CSR offsets of the hits], each n_queries + 1
     DevBuf subsets_meta;
 
@@ -970,6 +981,8 @@ static int ensure_split_planes(tav_index* ix, TimedSearch* ts, cudaStream_t s) {
     return TAV_OK;
 }
 
+static int range_into_redo(tav_index* ix, const Pending& p, bool redo_all, int* n_redone, cudaStream_t s);
+
 static inline int32_t* retry_totals(tav_index* ix, int slot) { return static_cast<int32_t*>(ix->retry.p) + 2 * slot; }
 static inline int32_t* retry_flags(tav_index* ix, int slot) {
     return static_cast<int32_t*>(ix->retry.p) + 2 * kMaxPending + static_cast<size_t>(slot) * ix->retry_cap;
@@ -1000,6 +1013,10 @@ static int finish_pending(tav_index* ix, cudaStream_t s, int* redone) {
         const bool redo_all = p.split && (corpus_overflow != 0 || q_overflow != 0);
         dirty |= flagged != 0 || q_overflow != 0;
         if (flagged == 0 && !redo_all) continue;
+        if (p.k == 0) {  // a threshold search into the caller's buffers
+            if (int rc = range_into_redo(ix, p, redo_all, &n_redone, s)) return rc;
+            continue;
+        }
         host.assign(static_cast<size_t>(p.nq), 1);
         if (!redo_all) {
             TAV_CUDA(cudaMemcpyAsync(host.data(), retry_flags(ix, p.slot), static_cast<size_t>(p.nq) * sizeof(int32_t),
@@ -1500,6 +1517,390 @@ static int range_core(tav_index* ix, TimedSearch* ts, bool timing, const float* 
                               expected_hits, offsets, s, positions, qm);
 }
 
+// ---- threshold search into caller buffers (tav_range_search_into) ----------------------------------------
+// The hits land in the caller's device memory: CSR offsets [nq + 1] always complete, items / scores at the CSR
+// positions below cap.  No host synchronisation: the plan kernel sizes the result on the device, the sort is
+// launched over upper bounds known on the host, and a query whose region overflowed is flagged for
+// tav_finish_search (finish_pending -> range_into_redo) instead of being re-collected now.  Nothing here touches
+// range_items / range_scores: the hits of the last tav_range_search stay as they were until the next call that
+// replaces them (tav_range_search_into itself gives them up on entry).
+struct RangeOut {
+    int64_t* offsets;
+    int64_t* items;
+    float* scores;
+    int64_t cap;
+};
+
+// The "redo exactly" bookkeeping for searches of up to `need` queries, sized for `cap` when it grows (which
+// finishes the outstanding searches first).
+static int ensure_retry(tav_index* ix, int need, int cap, cudaStream_t s) {
+    if (need <= ix->retry_cap && ix->retry.p && !ix->alloc_fail) return TAV_OK;
+    if (int rc = finish_pending(ix, s, nullptr)) return rc;
+    cap = std::max(cap, 1024);
+    const size_t bytes = (static_cast<size_t>(2) * kMaxPending + static_cast<size_t>(kMaxPending) * cap) * sizeof(int32_t);
+    TAV_CUDA(ix->retry.ensure(ix->alloc_fail ? ~size_t(0) >> 4 : bytes));
+    TAV_CUDA(cudaMemsetAsync(ix->retry.p, 0, 2 * kMaxPending * sizeof(int32_t), s));
+    TAV_CUDA(ix->retry_host.ensure(2 * kMaxPending * sizeof(int32_t)));
+    memset(ix->retry_host.p, 0, 2 * kMaxPending * sizeof(int32_t));
+    ix->retry_cap = cap;
+    return TAV_OK;
+}
+
+// A deferred search re-reads its queries (and subset) at tav_finish_search, after later searches on this index have
+// restaged ix->queries: `bytes` of held_queries stay its own until then (*out; *end = the region's end).  When they
+// do not fit, a buffer of at least twice the size takes over and the old one is kept (not freed) until the
+// searches that read it are finished: no search is finished early.
+static int hold_region(tav_index* ix, size_t bytes, void** out, size_t* end) {
+    bytes = (bytes + 255) & ~size_t(255);
+    const size_t need = ix->held_used + bytes;
+    if (need > ix->held_queries.bytes) {
+        const size_t want = std::max(need, 2 * ix->held_queries.bytes);
+        if (ix->held_used > 0) {  // pending searches read the current buffer
+            ix->held_retired.push_back(std::move(ix->held_queries));
+            ix->held_used = 0;
+        }
+        TAV_CUDA(ix->held_queries.ensure(want));
+    }
+    *out = static_cast<char*>(ix->held_queries.p) + ix->held_used;
+    ix->held_used += bytes;
+    *end = ix->held_used;
+    return TAV_OK;
+}
+
+// Where a plan's results go besides the sort setup (see RangePlanArgs): a first pass scans the counts into
+// `offsets` and flags its overflowed queries; a re-pass puts query i's hits at base[i] (host, nq entries).
+struct PlanDest {
+    int64_t* offsets = nullptr;
+    const int64_t* base = nullptr;
+    int32_t* flags = nullptr;
+    int32_t* n_flagged = nullptr;
+    int32_t* n_flagged_host = nullptr;
+    const int* abandon[2] = {nullptr, nullptr};
+};
+
+// The device plan of nq queries whose counters are count / fill (see RangePlanArgs), at most `region` keys per
+// query that did not overflow, then the sort setup: *sa for launch_segmented_sort_dev, *sizes its counts, and
+// (packed keys) *dst_off the gather offsets.
+static int range_plan(tav_index* ix, TimedSearch* ts, int nq, const uint32_t* count, const uint32_t* fill, uint32_t cap,
+                      int64_t region, int64_t key_stride, uint64_t* keys, const int64_t* d_subset, int64_t item_offset,
+                      int ties_low, const RangeOut& out, const PlanDest& dest, SortArgs* sa, const int** sizes,
+                      int64_t** dst_off, cudaStream_t s) {
+    const bool any_large = region > kSmallSortMax;
+    const int n_large_max = any_large ? nq : 0;
+    const int64_t tiles_max = any_large ? static_cast<int64_t>(nq) * ((region + kRadixTile - 1) / kRadixTile) : 0;
+    uint64_t* tmp = nullptr;
+    if (any_large) {
+        if (int rc = range_alloc(ix->range_tmp, static_cast<size_t>(nq) * region * sizeof(uint64_t), "the sort scratch"))
+            return rc;
+        tmp = static_cast<uint64_t*>(ix->range_tmp.p);
+    }
+    // sort workspace: segs | large | tile_seg | minmax | hist | offs | sizes | dst_off | base
+    auto up = [](size_t o) { return (o + 15) & ~size_t(15); };
+    const size_t o_large = up(static_cast<size_t>(nq) * sizeof(SortSeg));
+    const size_t o_tiles = up(o_large + static_cast<size_t>(n_large_max) * sizeof(int));
+    const size_t o_minmax = up(o_tiles + static_cast<size_t>(tiles_max) * sizeof(int));
+    const size_t o_hist = o_minmax + static_cast<size_t>(n_large_max) * 2 * sizeof(uint64_t);
+    const size_t o_offs = o_hist + static_cast<size_t>(tiles_max) * 256 * sizeof(uint32_t);
+    const size_t o_sizes = o_offs + static_cast<size_t>(tiles_max) * 256 * sizeof(uint32_t);
+    const size_t o_dst = up(o_sizes + 2 * sizeof(int));
+    const size_t o_base = o_dst + static_cast<size_t>(nq) * sizeof(int64_t);
+    const size_t ws_bytes = o_base + (dest.base ? static_cast<size_t>(nq) * sizeof(int64_t) : 0);
+    if (int rc = range_alloc(ix->range_sortws, ws_bytes, "the sort workspace")) return rc;
+    char* ws = static_cast<char*>(ix->range_sortws.p);
+    if (dest.base)  // from pageable memory: consumed when the call returns
+        TAV_CUDA(cudaMemcpyAsync(ws + o_base, dest.base, static_cast<size_t>(nq) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+
+    RangePlanArgs pa{};
+    pa.nq = nq;
+    pa.count = count;
+    pa.fill = fill;
+    pa.cap = cap;
+    pa.key_stride = key_stride;
+    pa.keys = keys;
+    pa.tmp = tmp;
+    pa.out_offsets = dest.offsets;
+    pa.out_base = dest.base ? reinterpret_cast<const int64_t*>(ws + o_base) : nullptr;
+    pa.abandon[0] = dest.abandon[0];
+    pa.abandon[1] = dest.abandon[1];
+    pa.dst_off = key_stride ? nullptr : reinterpret_cast<int64_t*>(ws + o_dst);
+    pa.flags = dest.flags;
+    pa.n_flagged = dest.n_flagged;
+    pa.n_flagged_host = dest.n_flagged_host;
+    pa.segs = reinterpret_cast<SortSeg*>(ws);
+    pa.large = reinterpret_cast<int*>(ws + o_large);
+    pa.tile_seg = reinterpret_cast<int*>(ws + o_tiles);
+    pa.minmax = reinterpret_cast<uint64_t*>(ws + o_minmax);
+    pa.sizes = reinterpret_cast<int*>(ws + o_sizes);
+    TAV_CUDA(launch_range_plan(pa, s));
+    ts->launches += 1;
+
+    *sa = SortArgs{};
+    sa->segs = pa.segs;
+    sa->n_segs = nq;
+    sa->large = pa.large;
+    sa->n_large = n_large_max;
+    sa->tile_seg = pa.tile_seg;
+    sa->n_tiles = tiles_max;
+    sa->minmax = pa.minmax;
+    sa->hist = reinterpret_cast<uint32_t*>(ws + o_hist);
+    sa->offs = reinterpret_cast<uint32_t*>(ws + o_offs);
+    sa->subset = d_subset;
+    sa->item_offset = item_offset;
+    sa->ties_low = ties_low;
+    sa->out_items = out.items;
+    sa->out_scores = out.scores;
+    *sizes = pa.sizes;
+    *dst_off = pa.dst_off;
+    return TAV_OK;
+}
+
+static int range_sort_dev(tav_index* ix, TimedSearch* ts, bool timing, const SortArgs& sa, const int* sizes, int64_t cap,
+                          cudaStream_t s) {
+    TAV_CUDA(timed_launch(ix, ts, timing, 2, s, [&] { return launch_segmented_sort_dev(sa, sizes, cap, s, &ts->launches); }));
+    return TAV_OK;
+}
+
+// the tensor-core collection plan of a threshold search: segments sized from expected_hits as in range_collect_mma
+static MmaCollect range_mma_plan(const MmaArgs& m, int64_t expected_hits, int nq, int64_t n_rows) {
+    const int64_t per = range_per_query(expected_hits, nq, n_rows);
+    const MmaCollect shape = mma_collect_plan(m, 0, 1);
+    return mma_collect_plan(m, shape.per_chunk, 2 * ((per + shape.n_seg - 1) / shape.n_seg) + 8);
+}
+
+// A first pass: collection (the row scan, or the tensor cores with the split form's planes), device plan and sort
+// of a threshold search into `out`, all queued on s.  The plan's flags go to bookkeeping slot `slot` (and, with
+// `count_flags`, their number).  *per_chunk / *n_seg: the tensor-core plan (0 for the row scan), which a re-pass
+// must repeat.  Returns kRangeUseScan when the split planes cannot be allocated (the row scan then serves the
+// search, as in range_collect_mma).
+static int range_into_core(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
+                           const int64_t* d_subset, int64_t n_scan, int64_t item_offset, const uint32_t* d_mask,
+                           QueryMasks qm, int ties_low, int64_t expected_hits, bool use_mma, int slot, bool count_flags,
+                           const RangeOut& out, int* per_chunk, int* n_seg, cudaStream_t s) {
+    SortArgs sa;
+    const int* sizes = nullptr;
+    int64_t* dst_off = nullptr;
+    PlanDest dest;
+    dest.offsets = out.offsets;
+    dest.flags = retry_flags(ix, slot);
+    if (count_flags) {
+        dest.n_flagged = retry_totals(ix, slot);
+        dest.n_flagged_host = static_cast<int32_t*>(ix->retry_host.p) + 2 * slot;
+    }
+    *per_chunk = *n_seg = 0;
+    if (!use_mma) {
+        const int64_t per = range_per_query(expected_hits, nq, n_scan);
+        if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(nq) * per * sizeof(uint64_t), "the hit regions")) return rc;
+        if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(nq) * sizeof(uint32_t), "the hit counters")) return rc;
+        uint32_t* d_counts = static_cast<uint32_t*>(ix->range_counts.p);
+        uint64_t* keys = static_cast<uint64_t*>(ix->range_keys.p);
+        TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(nq) * sizeof(uint32_t), s));
+        if (int rc = collect_scans(ix, ts, timing, d_queries, nq, floor, d_subset, n_scan, d_mask, ties_low, keys, per,
+                                   d_counts, s, qm))
+            return rc;
+        if (int rc = range_plan(ix, ts, nq, d_counts, d_counts, static_cast<uint32_t>(per), per, per, keys, d_subset,
+                                item_offset, ties_low, out, dest, &sa, &sizes, &dst_off, s))
+            return rc;
+    } else {
+        const bool split = ix->dtype == TAV_F32;
+        if (split) {
+            const int rc = ensure_split_planes(ix, ts, s);
+            if (rc == TAV_ERR_OOM) return kRangeUseScan;
+            if (rc != TAV_OK) return rc;
+        }
+        if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(nq) * 2 * sizeof(uint32_t), "the hit counters")) return rc;
+        uint32_t* d_tot = static_cast<uint32_t*>(ix->range_counts.p);
+        uint32_t* d_max = d_tot + nq;
+        if (timing)
+            if (int rc = create_events(ts)) return rc;
+        MmaArgs m = mma_args(ix, split);
+        // a query value beyond the fp16 range flags the whole search (finish_pending reads the mapped twin)
+        m.split_overflow = split ? retry_totals(ix, slot) + 1 : nullptr;
+        m.split_overflow_host = split ? static_cast<int*>(ix->retry_host.p) + 2 * slot + 1 : nullptr;
+        m.queries = d_queries;
+        m.nq = nq;
+        m.floor_score = floor;
+        m.k = 1;
+        m.item_offset = item_offset;
+        m.retry_flags = retry_flags(ix, slot);  // scratch of the query prep; the plan writes the flags after it
+        m.row_mask = d_mask;
+        m.qmask = qm;
+        int ev_used = ts->used;
+        m.ev = timing ? ts->ev : nullptr;
+        m.ev_kind = ts->kind;
+        m.ev_max = kMaxTimedKernels;
+        m.ev_used = &ev_used;
+        const MmaCollect c = range_mma_plan(m, expected_hits, nq, ix->size);
+        if (int rc = range_alloc(ix->range_mmaws, c.ws_bytes, "the tensor-core workspace")) return rc;
+        TAV_CUDA(launch_mma_collect(m, c, ix->range_mmaws.p, d_tot, d_max, s, &ts->launches));
+        ts->used = ev_used;
+        // a query that did not overflow has at most every segment full of keys
+        const int64_t region = static_cast<int64_t>(c.n_seg) * c.cap_seg;
+        if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(nq) * region * sizeof(uint64_t), "the hit keys")) return rc;
+        uint64_t* keys = static_cast<uint64_t*>(ix->range_keys.p);
+        if (split) {  // the split form's overflow: nothing of this pass may reach the outputs (it is redone whole)
+            dest.abandon[0] = m.split_overflow;
+            dest.abandon[1] = static_cast<const int*>(ix->split_flag.p);
+        }
+        if (int rc = range_plan(ix, ts, nq, d_tot, d_max, c.cap_seg, region, 0, keys, nullptr, item_offset, ties_low, out,
+                                dest, &sa, &sizes, &dst_off, s))
+            return rc;
+        TAV_CUDA(launch_mma_gather(m, c, ix->range_mmaws.p, dst_off, keys, ties_low, s));
+        ts->launches += 1;
+        *per_chunk = c.per_chunk;
+        *n_seg = c.n_seg;
+    }
+    return range_sort_dev(ix, ts, timing, sa, sizes, out.cap, s);
+}
+
+// The filter of a re-pass over the queries `over` of a deferred search: its row mask, or its per-query masks
+// through a map (each gathered query keeps its own mask).
+static int repass_masks(tav_index* ix, const Pending& p, const std::vector<int>& over, const uint32_t** d_mask,
+                        QueryMasks* qm, cudaStream_t s) {
+    *d_mask = p.qm.bits ? nullptr : p.mask;
+    *qm = QueryMasks{};
+    if (p.qm.bits) return gather_mask_map(ix, over, p.qm, *qm, s);
+    return TAV_OK;
+}
+
+// Row-scan re-pass of the flagged queries `over` of a deferred search, gathered, in one collect pass with regions
+// of the largest count (nothing can overflow: the same kernel counts the same rows), sorted into the search's
+// outputs at their offsets `off` (host, the search's CSR offsets).
+static int range_repass_scan(tav_index* ix, const Pending& p, const std::vector<int>& over, const std::vector<int64_t>& off,
+                             cudaStream_t s) {
+    TimedSearch ts;
+    const int no = static_cast<int>(over.size());
+    int64_t per = 1;
+    std::vector<int64_t> base(static_cast<size_t>(no));
+    for (int i = 0; i < no; ++i) {
+        per = std::max(per, off[over[i] + 1] - off[over[i]]);
+        base[i] = off[over[i]];
+    }
+    if (int rc = gather_repass_queries(ix, p.queries, over, s)) return rc;
+    const uint32_t* d_mask;
+    QueryMasks qm;
+    if (int rc = repass_masks(ix, p, over, &d_mask, &qm, s)) return rc;
+    if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(no) * per * sizeof(uint64_t), "the re-pass regions")) return rc;
+    if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(no) * sizeof(uint32_t), "the hit counters")) return rc;
+    uint32_t* d_counts = static_cast<uint32_t*>(ix->range_counts.p);
+    uint64_t* keys = static_cast<uint64_t*>(ix->range_keys.p);
+    TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(no) * sizeof(uint32_t), s));
+    if (int rc = collect_scans(ix, &ts, false, static_cast<const float*>(ix->range_qgather.p), no, p.floor, p.subset,
+                               p.n_scan, d_mask, p.ties_low, keys, per, d_counts, s, qm))
+        return rc;
+    SortArgs sa;
+    const int* sizes = nullptr;
+    int64_t* dst_off = nullptr;
+    PlanDest dest;
+    dest.base = base.data();
+    const RangeOut out{nullptr, p.items, p.scores, p.cap};
+    if (int rc = range_plan(ix, &ts, no, d_counts, d_counts, static_cast<uint32_t>(per), per, per, keys, p.subset,
+                            p.item_offset, p.ties_low, out, dest, &sa, &sizes, &dst_off, s))
+        return rc;
+    return range_sort_dev(ix, &ts, false, sa, sizes, p.cap, s);
+}
+
+// Tensor-core re-pass of the flagged queries `over` (fill = each one's fullest segment) of a deferred search, as
+// range_collect_mma re-passes: gathered, through the same units per query chunk (every segment receives the rows
+// it received before) with segments of the fullest size.  Its counts are checked against the first pass's (one
+// synchronisation) before anything is written; on a mismatch it returns kRangeUseScan and writes nothing.
+static int range_repass_mma(tav_index* ix, const Pending& p, const std::vector<int>& over, uint32_t over_seg,
+                            const std::vector<int64_t>& off, cudaStream_t s) {
+    TimedSearch ts;
+    const int no = static_cast<int>(over.size());
+    if (int rc = gather_repass_queries(ix, p.queries, over, s)) return rc;
+    MmaArgs m = mma_args(ix, p.split);
+    m.split_overflow = p.split ? retry_totals(ix, p.slot) + 1 : nullptr;
+    m.queries = static_cast<const float*>(ix->range_qgather.p);
+    m.nq = no;
+    m.floor_score = p.floor;
+    m.k = 1;
+    m.item_offset = p.item_offset;
+    m.retry_flags = retry_flags(ix, p.slot);  // scratch (the flags were read)
+    if (int rc = repass_masks(ix, p, over, &m.row_mask, &m.qmask, s)) return rc;
+    const MmaCollect c = mma_collect_plan(m, p.per_chunk, over_seg);
+    if (c.n_seg != p.n_seg || c.cap_seg < over_seg) return kRangeUseScan;
+    if (int rc = range_alloc(ix->range_mmaws2, c.ws_bytes, "the tensor-core re-pass workspace")) return rc;
+    if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(no) * 2 * sizeof(uint32_t), "the hit counters")) return rc;
+    uint32_t* d_tot = static_cast<uint32_t*>(ix->range_counts.p);
+    uint32_t* d_max = d_tot + no;
+    TAV_CUDA(launch_mma_collect(m, c, ix->range_mmaws2.p, d_tot, d_max, s, &ts.launches));
+    std::vector<uint32_t> host(2 * static_cast<size_t>(no));
+    TAV_CUDA(cudaMemcpyAsync(host.data(), d_tot, host.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaStreamSynchronize(s));
+    int64_t most = 1;
+    std::vector<int64_t> base(static_cast<size_t>(no));
+    for (int i = 0; i < no; ++i) {
+        const int64_t n = off[over[i] + 1] - off[over[i]];
+        if (host[i] != static_cast<uint64_t>(n) || host[no + i] > c.cap_seg) return kRangeUseScan;
+        most = std::max(most, n);
+        base[i] = off[over[i]];
+    }
+    if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(no) * most * sizeof(uint64_t), "the hit keys")) return rc;
+    uint64_t* keys = static_cast<uint64_t*>(ix->range_keys.p);
+    SortArgs sa;
+    const int* sizes = nullptr;
+    int64_t* dst_off = nullptr;
+    PlanDest dest;
+    dest.base = base.data();
+    const RangeOut out{nullptr, p.items, p.scores, p.cap};
+    if (int rc = range_plan(ix, &ts, no, d_tot, d_max, c.cap_seg, most, 0, keys, nullptr, p.item_offset, p.ties_low, out,
+                            dest, &sa, &sizes, &dst_off, s))
+        return rc;
+    TAV_CUDA(launch_mma_gather(m, c, ix->range_mmaws2.p, dst_off, keys, p.ties_low, s));
+    return range_sort_dev(ix, &ts, false, sa, sizes, p.cap, s);
+}
+
+// What a deferred threshold search into caller buffers left for tav_finish_search (finish_pending, after its
+// synchronisation).  Its flagged queries are searched again, gathered, by the collection that flagged them (a
+// row-scan re-pass, or a tensor-core re-pass with the same plan) and sorted into their places.  The whole search is
+// searched again by the row scan, offsets included, when the split form met a value beyond the fp16 range (its
+// first pass then wrote no hits) or a tensor-core re-pass does not count what the first pass counted (a safeguard,
+// as in range_collect_mma; the first pass's hits may then remain between the new total and the capacity).
+static int range_into_redo(tav_index* ix, const Pending& p, bool redo_all, int* n_redone, cudaStream_t s) {
+    std::vector<int64_t> off(static_cast<size_t>(p.nq) + 1);
+    std::vector<int32_t> flag(static_cast<size_t>(p.nq));
+    auto read_plan = [&]() -> int {
+        TAV_CUDA(cudaMemcpyAsync(off.data(), p.offsets, off.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+        TAV_CUDA(cudaMemcpyAsync(flag.data(), retry_flags(ix, p.slot), flag.size() * sizeof(int32_t),
+                                 cudaMemcpyDeviceToHost, s));
+        TAV_CUDA(cudaStreamSynchronize(s));
+        return TAV_OK;
+    };
+    auto flagged = [&](uint32_t* most) {
+        std::vector<int> over;
+        *most = 0;
+        for (int q = 0; q < p.nq; ++q)
+            if (flag[q]) {
+                over.push_back(q);
+                *most = std::max(*most, static_cast<uint32_t>(flag[q]));
+            }
+        return over;
+    };
+    uint32_t over_seg = 0;
+    if (!redo_all) {
+        if (int rc = read_plan()) return rc;
+        const std::vector<int> over = flagged(&over_seg);
+        *n_redone += static_cast<int>(over.size());
+        if (over.empty()) return TAV_OK;
+        if (p.per_chunk == 0) return range_repass_scan(ix, p, over, off, s);
+        const int rc = range_repass_mma(ix, p, over, over_seg, off, s);
+        if (rc != kRangeUseScan) return rc;
+        *n_redone -= static_cast<int>(over.size());  // counted below with the whole search
+    }
+    // the whole search by the row scan, into the same outputs; what overflows its regions gets a row-scan re-pass
+    TimedSearch ts;
+    int per_chunk, n_seg;
+    const RangeOut out{p.offsets, p.items, p.scores, p.cap};
+    if (int rc = range_into_core(ix, &ts, false, p.queries, p.nq, p.floor, p.subset, p.n_scan, p.item_offset,
+                                 p.qm.bits ? nullptr : p.mask, p.qm, p.ties_low, p.expected_hits, false, p.slot, false,
+                                 out, &per_chunk, &n_seg, s))
+        return rc;
+    *n_redone += p.nq;
+    if (int rc = read_plan()) return rc;
+    const std::vector<int> over = flagged(&over_seg);
+    return over.empty() ? TAV_OK : range_repass_scan(ix, p, over, off, s);
+}
+
 // ---- removal and overwrite (tav_remove_rows, tav_write_rows) -----------------------------------------------
 constexpr size_t kCompactScratchBytes = size_t(256) << 20;  // window buffer of the in-place compaction
 
@@ -1984,6 +2385,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             return rc;
         std::vector<int64_t> offsets;
         ix->range_total = 0;
+        ix->range_replaced = false;
         if (int rc = range_core(ix, ts, timing, d_q, n_queries, min_score, d_sub, n_scan, item_offset, d_mask, ties_low,
                                 static_cast<int64_t>(n_queries) * n_scan, false, offsets, s, positions, qm))
             return rc;
@@ -2144,18 +2546,9 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     float* held = nullptr;
     size_t held_end = 0;
     if (use_mma && defer && (ix->flags & TAV_NORMALIZE)) {
-        const size_t q_bytes = (static_cast<size_t>(n_queries) * ix->dim * sizeof(float) + 255) & ~size_t(255);
-        const size_t need = ix->held_used + q_bytes;
-        if (need > ix->held_queries.bytes) {
-            const size_t want = std::max(need, 2 * ix->held_queries.bytes);
-            if (ix->held_used > 0) {  // pending searches read the current buffer
-                ix->held_retired.push_back(std::move(ix->held_queries));
-                ix->held_used = 0;
-            }
-            TAV_CUDA(ix->held_queries.ensure(want));
-        }
-        held = reinterpret_cast<float*>(static_cast<char*>(ix->held_queries.p) + ix->held_used);
-        held_end = ix->held_used + q_bytes;
+        void* r = nullptr;
+        if (int rc = hold_region(ix, static_cast<size_t>(n_queries) * ix->dim * sizeof(float), &r, &held_end)) return rc;
+        held = static_cast<float*>(r);
     }
 
     const int64_t* d_subset = nullptr;
@@ -2175,16 +2568,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
 
     if (use_mma) {
         ts->path = use_split ? 3 : 2;
-        if (n_queries > ix->retry_cap || !ix->retry.p || ix->alloc_fail) {
-            if (int rc = finish_pending(ix, s, nullptr)) return rc;
-            const int cap = std::max(std::min(n_queries, kMmaMaxQueries), 1024);
-            const size_t bytes = (static_cast<size_t>(2) * kMaxPending + static_cast<size_t>(kMaxPending) * cap) * sizeof(int32_t);
-            TAV_CUDA(ix->retry.ensure(ix->alloc_fail ? ~size_t(0) >> 4 : bytes));
-            TAV_CUDA(cudaMemsetAsync(ix->retry.p, 0, 2 * kMaxPending * sizeof(int32_t), s));
-            TAV_CUDA(ix->retry_host.ensure(2 * kMaxPending * sizeof(int32_t)));
-            memset(ix->retry_host.p, 0, 2 * kMaxPending * sizeof(int32_t));
-            ix->retry_cap = cap;
-        }
+        if (int rc = ensure_retry(ix, n_queries, std::min(n_queries, kMmaMaxQueries), s)) return rc;
         if (timing)
             if (int rc = create_events(ts)) return rc;
         // one launch sequence per slab of kMmaMaxQueries queries (in practice: one)
@@ -2272,6 +2656,7 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
     if (int rc = enter_stream(ix, s)) return rc;  // (also: a queued tav_range_fetch reads the hits replaced here)
     const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
     ix->range_total = 0;
+    ix->range_replaced = false;
     std::vector<int64_t> offsets(static_cast<size_t>(n_queries) + 1, 0);
     const uint32_t* d_mask = nullptr;
     QueryMasks qm;
@@ -2316,6 +2701,10 @@ int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items,
         return TAV_ERR_INVALID;
     }
     std::lock_guard<std::mutex> lock(ix->mu);
+    if (ix->range_replaced) {
+        set_error("tav_range_fetch: a tav_range_search_into replaced the hits of the last range search");
+        return TAV_ERR_STATE;
+    }
     if (first + n > ix->range_total) {
         set_error("tav_range_fetch: hits [%lld, %lld) out of range (the last range search has %lld)", (long long)first,
                   (long long)(first + n), (long long)ix->range_total);
@@ -2333,6 +2722,113 @@ int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items,
     TAV_CUDA(cudaStreamSynchronize(s));
     mark_done(ix);
     return TAV_OK;
+}
+
+int tav_range_search_into(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
+                          const int64_t* subset, int64_t subset_len, int64_t item_offset, int64_t expected_hits,
+                          int64_t capacity, int64_t* out_offsets, int64_t* out_items, float* out_scores, void* stream) {
+    constexpr int kAccepted = TAV_QUERIES_ON_DEVICE | TAV_FORCE_SCAN | TAV_FORCE_MMA | TAV_USE_ROW_MASK |
+                              TAV_USE_QUERY_MASKS | TAV_TIES_LOW_FIRST | TAV_DEFER_RETRY;
+    if (!ix || n_queries < 0 || expected_hits < 0 || capacity < 0 || (flags & ~kAccepted) || !out_offsets ||
+        (n_queries > 0 && !queries) || (capacity > 0 && (!out_items || !out_scores))) {
+        set_error("tav_range_search_into: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    if (int rc = check_subset_args("tav_range_search_into", flags, subset, subset_len, false)) return rc;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = enter_stream(ix, s)) return rc;
+    const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, defer = flags & TAV_DEFER_RETRY;
+    ix->range_total = 0;  // the hits of the last tav_range_search are given up (the sort scratch is reused)
+    ix->range_replaced = true;
+    const uint32_t* d_mask = nullptr;
+    QueryMasks qm;
+    if (int rc = resolve_masks(ix, "tav_range_search_into", n_queries, flags, subset != nullptr, &d_mask, &qm)) return rc;
+    const int64_t n_scan = subset ? subset_len : ix->size;
+    // NaN min_score, empty corpus or empty subset: no hits
+    if (n_queries == 0 || n_scan == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score) {
+        TAV_CUDA(cudaMemsetAsync(out_offsets, 0, (static_cast<size_t>(n_queries) + 1) * sizeof(int64_t), s));
+        return mark_queued(ix, s);
+    }
+    if (n_scan > 0xFFFFFFFFll) {
+        set_error("tav_range_search_into: more than 2^32 rows per index are not supported; shard the corpus");
+        return TAV_ERR_INVALID;
+    }
+    if (int rc = check_subset_ordinals(ix, subset, subset_len)) return rc;
+    // path choice as in tav_range_search
+    const bool mma_able = (mma_supported(ix->dtype, ix->dim) || (ix->dtype == TAV_F32 && mma_split_supported(ix->dim))) &&
+                          !subset && n_queries <= kMmaMaxQueries && ix->size < (1ll << 31);
+    bool use_mma = !(flags & TAV_FORCE_SCAN) && mma_able &&
+                   ((flags & TAV_FORCE_MMA) || (n_queries >= 16 && ix->size >= 4096));
+    if ((flags & TAV_FORCE_MMA) && !use_mma) {
+        set_error("tav_range_search_into: TAV_FORCE_MMA needs dim %% 8 == 0, no subset, at most %d queries", kMmaMaxQueries);
+        return TAV_ERR_INVALID;
+    }
+    // bookkeeping slot (flags and flagged count of the plan), as for deferred top-k searches
+    if (int rc = ensure_retry(ix, n_queries, n_queries, s)) return rc;
+    if (static_cast<int>(ix->pending.size()) >= kMaxPending)
+        if (int rc = finish_pending(ix, s, nullptr)) return rc;
+    // a deferred search reads its queries and subset again at tav_finish_search: staged ones are held until then
+    float* held_q = nullptr;
+    int64_t* held_sub = nullptr;
+    size_t held_end = 0;
+    if (defer && (!q_dev || (ix->flags & TAV_NORMALIZE))) {
+        void* r = nullptr;
+        if (int rc = hold_region(ix, static_cast<size_t>(n_queries) * ix->dim * sizeof(float), &r, &held_end)) return rc;
+        held_q = static_cast<float*>(r);
+    }
+    if (defer && subset) {
+        void* r = nullptr;
+        if (int rc = hold_region(ix, static_cast<size_t>(subset_len) * sizeof(int64_t), &r, &held_end)) return rc;
+        held_sub = static_cast<int64_t*>(r);
+    }
+    TimedSearch* ts = begin_search(ix, use_mma ? (ix->dtype == TAV_F32 ? 3 : 2) : 1);
+    const bool timing = ts != &ix->untimed;
+    const float* d_queries = nullptr;
+    const int64_t* d_subset = nullptr;
+    if (int rc = stage_inputs(ix, ts, timing, queries, n_queries, q_dev, true, subset, subset_len, &d_queries, &d_subset, s,
+                              held_q))
+        return rc;
+    if (held_sub) {
+        TAV_CUDA(cudaMemcpyAsync(held_sub, d_subset, static_cast<size_t>(subset_len) * sizeof(int64_t),
+                                 cudaMemcpyDeviceToDevice, s));
+        d_subset = held_sub;
+    }
+    const int slot = ix->next_slot++;
+    const int ties_low = (flags & TAV_TIES_LOW_FIRST) ? 1 : 0;
+    const RangeOut out{out_offsets, out_items, out_scores, capacity};
+    int per_chunk = 0, n_seg = 0;
+    int rc = range_into_core(ix, ts, timing, d_queries, n_queries, min_score, d_subset, n_scan, item_offset, d_mask, qm,
+                             ties_low, expected_hits, use_mma, slot, true, out, &per_chunk, &n_seg, s);
+    if (rc == kRangeUseScan) {
+        use_mma = false;
+        ts->path = 1;
+        rc = range_into_core(ix, ts, timing, d_queries, n_queries, min_score, d_subset, n_scan, item_offset, d_mask, qm,
+                             ties_low, expected_hits, false, slot, true, out, &per_chunk, &n_seg, s);
+    }
+    if (rc == TAV_OK) rc = end_search(ix, ts, s);
+    if (rc != TAV_OK) {
+        // the slot goes back, clean: a kernel this call queued may have written its totals (the error stands)
+        cudaStreamSynchronize(s);
+        cudaMemset(retry_totals(ix, slot), 0, 2 * sizeof(int32_t));
+        static_cast<int32_t*>(ix->retry_host.p)[2 * slot] = static_cast<int32_t*>(ix->retry_host.p)[2 * slot + 1] = 0;
+        --ix->next_slot;
+        return rc;
+    }
+    Pending p{d_queries, n_queries, 0, min_score, item_offset, out_items, out_scores, nullptr, slot,
+              use_mma && ix->dtype == TAV_F32, qm.bits ? qm.bits : d_mask, qm.bits ? qm.stride : 0};
+    p.offsets = out_offsets;
+    p.cap = capacity;
+    p.subset = d_subset;
+    p.n_scan = n_scan;
+    p.ties_low = ties_low;
+    p.expected_hits = expected_hits;
+    p.qm = qm;
+    p.per_chunk = per_chunk;
+    p.n_seg = n_seg;
+    ix->pending.push_back(p);
+    if (!defer) return finish_pending(ix, s, nullptr);  // redoes what the plan flagged now; synchronises s
+    return mark_queued(ix, s);
 }
 
 }  // extern "C"
@@ -2474,6 +2970,7 @@ int tav_search_subsets(tav_index* ix, const float* queries, int n_queries, int k
     const bool timing = ts != &ix->untimed;
     std::vector<int64_t> csr;
     ix->range_total = 0;  // the hits land in the threshold search's buffers
+    ix->range_replaced = false;
     if (int rc = subsets_core(ix, ts, timing, queries, n_queries, flags, min_score, offsets, ordinals, csr, s))
         return rc;
     ix->range_total = csr[n_queries];
@@ -2514,6 +3011,7 @@ int tav_range_search_subsets(tav_index* ix, const float* queries, int n_queries,
         if (int rc = check_subset_ordinals(ix, ordinals, total)) return rc;
     std::vector<int64_t> csr(static_cast<size_t>(n_queries) + 1, 0);
     ix->range_total = 0;
+    ix->range_replaced = false;
     if (!none) {
         TimedSearch* ts = begin_search(ix, 1);
         const bool timing = ts != &ix->untimed;

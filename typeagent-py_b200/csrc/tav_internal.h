@@ -169,6 +169,35 @@ struct SortArgs {
 // returns the number of kernels launched in *launches
 cudaError_t launch_segmented_sort(const SortArgs& a, cudaStream_t s, int* launches);
 
+// The device plan of a threshold search into caller buffers (tav_range_search_into): the collect counters ->
+// the CSR offsets, the overflow flags and everything the segmented sort needs, with no host round trip.
+struct RangePlanArgs {
+    int nq;
+    const uint32_t* count;   // [nq] rows admitted (exact, also past a full region)
+    const uint32_t* fill;    // [nq] compared with cap: > cap = the query's region or fullest segment overflowed
+    uint32_t cap;
+    int64_t key_stride;      // > 0: query q's keys at keys + q * key_stride (row scan); 0: packed in query order
+                             // with the overflowed queries left out (tensor cores, gathered to dst_off)
+    uint64_t* keys;
+    uint64_t* tmp;           // radix scratch, laid out like keys
+    int64_t* out_offsets;    // [nq + 1] the CSR offsets of the result, or nullptr (a re-pass: out_base)
+    const int64_t* out_base; // [nq] a re-pass: where each query's hits go (its offset in the search it redoes)
+    const int* abandon[2];   // words (or nullptr): either set -> nothing is sorted or gathered
+    int64_t* dst_off;        // [nq] packed only: key offset of the query, -1 when not gathered; else nullptr
+    int32_t* flags;          // [nq] or nullptr: 0, or the fill of an overflowed query
+    int32_t* n_flagged;      // or nullptr: the number of flagged queries (device) ...
+    int32_t* n_flagged_host; // ... and its mapped pinned twin, or nullptr
+    SortSeg* segs;           // [nq]
+    int* large;              // [nq] at most
+    int* tile_seg;           // [upper bound of the radix tiles]
+    uint64_t* minmax;        // [2 * nq] at most (initialised here for the large segments)
+    int* sizes;              // [2] large segments, radix tiles
+};
+cudaError_t launch_range_plan(const RangePlanArgs& a, cudaStream_t s);
+// launch_segmented_sort over a device plan: a.n_large / a.n_tiles are upper bounds (the plan's sizes give the
+// counts), and hits at CSR positions >= cap are not written
+cudaError_t launch_segmented_sort_dev(const SortArgs& a, const int* sizes, int64_t cap, cudaStream_t s, int* launches);
+
 struct SelectArgs {
     const uint64_t* cand_keys;   // [nq, cand_stride]
     int cand_stride;

@@ -21,7 +21,9 @@ Additions (not in the reference; all opt-in):
     batched lookup in which every query scores only its own candidate ordinals (the batched form of
     ``fuzzy_lookup_embedding_in_subset``, vectorbase.py:203-230: candidate re-ranking);
   * constructor keywords ``device``, ``storage_dtype``, ``normalize``;
-  * ``from_device_tensor`` / ``search_device`` — torch tensors as device-memory handles.
+  * ``from_device_tensor`` / ``search_device`` / ``search_range_device`` — torch tensors as device-memory
+    handles (the threshold search into caller tensors, sized on the device, optionally without a host
+    synchronisation).
 
 Documented divergences: negative ``max_hits`` raises ``ValueError`` (the reference returns
 an arbitrary slice); among *exactly* equal scores the order is "higher ordinal first" on
@@ -1111,9 +1113,98 @@ class VectorBase:
             self._pending.append((queries, items, scores, counts, stream, allowed))
         return items, scores, counts
 
+    def search_range_device(self, queries, min_score: float = 0.0, capacity: int | None = None, *, out=None,
+                            defer_check: bool = False, allowed=None, ties_low_first: bool = False, subset=None,
+                            expected_hits: int | None = None, item_offset: int = 0):
+        """Threshold search with torch CUDA tensors as handles, enqueued on torch's current stream: every row whose
+        score is >= min_score, per query, as ``search_range`` finds them, into device tensors
+        (offsets int64 [B + 1], items int64 [capacity], scores float32 [capacity]).  The offsets are always
+        complete; hits at CSR positions >= ``capacity`` are not written (those slots keep what they held), so when
+        ``offsets[-1] > capacity`` the caller may search again with more room.  ``out`` may supply the three
+        tensors (``capacity`` then defaults to the room they have).  Items are row ordinals (or subset ordinals)
+        + ``item_offset``, as in ``search_device``.  ``queries``: a contiguous float32 CUDA tensor
+        [B, D]; ``allowed`` as in ``search_device``; ``subset``: host ordinals as in ``search_range``.
+        ``expected_hits`` (default ``capacity``) sizes the device collect regions; it never changes the result.
+        The call synchronises once (more when a query overflowed its region); with ``defer_check=True`` it does
+        not synchronise at all, and ``finish_search()`` must run before the results are trusted."""
+        import torch
+
+        if not (getattr(queries, "is_cuda", False) and queries.dtype == torch.float32 and queries.is_contiguous()):
+            raise ValueError("queries must be a contiguous float32 CUDA tensor")
+        if queries.dim() != 2 or queries.shape[1] != self._embedding_size:
+            raise ValueError("query width does not match the embedding size")
+        b = queries.shape[0]
+        dev = queries.device
+        if out is not None:
+            if len(out) != 3:
+                raise ValueError("out must be (offsets, items, scores)")
+            offsets, items, scores = out
+            for t, dt, what in ((offsets, torch.int64, "offsets"), (items, torch.int64, "items"),
+                                (scores, torch.float32, "scores")):
+                if not (getattr(t, "is_cuda", False) and t.dtype == dt and t.dim() == 1 and t.is_contiguous()):
+                    raise ValueError(f"out {what} must be a contiguous 1-D {dt} CUDA tensor")
+                if t.device != dev:
+                    raise ValueError(f"out {what} is on {t.device}, the queries on {dev}")
+            if offsets.numel() != b + 1:
+                raise ValueError(f"out offsets must have {b + 1} entries, not {offsets.numel()}")
+            if capacity is None:
+                capacity = min(items.numel(), scores.numel())
+        if capacity is None:
+            raise ValueError("capacity is needed when out is not given")
+        if isinstance(capacity, bool) or int(capacity) != capacity or capacity < 0:
+            raise ValueError(f"capacity must be a non-negative integer, not {capacity!r}")
+        capacity = int(capacity)
+        if out is not None and (items.numel() < capacity or scores.numel() < capacity):
+            raise ValueError(f"out items / scores hold fewer than capacity = {capacity} hits")
+        if expected_hits is None:
+            expected_hits = capacity
+        if isinstance(expected_hits, bool) or int(expected_hits) != expected_hits or expected_hits < 0:
+            raise ValueError(f"expected_hits must be a non-negative integer, not {expected_hits!r}")
+        sub = None
+        if subset is not None:
+            if allowed is not None:
+                raise ValueError("allowed= and subset= cannot be combined")
+            sub = np.ascontiguousarray(subset)
+            if sub.size and not np.issubdtype(sub.dtype, np.integer):
+                raise IndexError("arrays used as indices must be of integer (or boolean) type")
+            sub = sub.astype(np.int64, copy=False).reshape(-1)
+        if out is None:
+            offsets = torch.empty((b + 1,), dtype=torch.int64, device=dev)
+            items = torch.empty((capacity,), dtype=torch.int64, device=dev)
+            scores = torch.empty((capacity,), dtype=torch.float32, device=dev)
+        lib, ix = self._ensure_device()
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        flags = _capi.TAV_QUERIES_ON_DEVICE | (self._flags() & ~_capi.TAV_NO_FUSED_SCAN)
+        if defer_check:
+            flags |= _capi.TAV_DEFER_RETRY
+        if self._is_query_masks(allowed):
+            self._use_query_masks(lib, ix, allowed, b, stream)
+            flags |= _capi.TAV_USE_QUERY_MASKS
+        elif allowed is not None:
+            self._use_row_mask(lib, ix, allowed)
+            flags |= _capi.TAV_USE_ROW_MASK
+        if ties_low_first:
+            flags |= _capi.TAV_TIES_LOW_FIRST
+        floor = float(_as_f32_scalar(min_score))
+        # the call gives up the index's threshold-search hits: not between a search_range and its fetch
+        with self._single_lock:
+            _capi.check(
+                lib.tav_range_search_into(
+                    ix, C.c_void_p(queries.data_ptr()), b, C.c_float(floor), flags,
+                    sub.ctypes.data_as(C.c_void_p) if sub is not None else None, len(sub) if sub is not None else 0,
+                    int(item_offset), int(expected_hits), capacity, C.c_void_p(offsets.data_ptr()),
+                    C.c_void_p(items.data_ptr()), C.c_void_p(scores.data_ptr()), C.c_void_p(stream),
+                )
+            )
+        if defer_check:
+            # the library searches flagged queries again into these very tensors at finish_search(): keep them alive
+            self._pending.append((queries, items, scores, offsets, stream, allowed))
+        return offsets, items, scores
+
     def finish_search(self) -> int:
-        """Complete every outstanding ``search_device(..., defer_check=True)``: synchronise, redo
-        (exactly) the queries the tensor-core path flagged, return how many there were."""
+        """Complete every outstanding ``search_device(..., defer_check=True)`` and
+        ``search_range_device(..., defer_check=True)``: synchronise, redo (exactly) the queries the device search
+        flagged, return how many there were."""
         if not self._pending:
             return 0
         stream = self._pending[-1][4]
