@@ -523,6 +523,58 @@ int tav_rows_stage(tav_index* ix, int world, int rank, const void* handles, int 
 int tav_rows_commit(tav_index* ix, int commit);
 
 /*
+ * Row-sharded search across the devices of ONE process (VectorBase(devices=[...])).  A tav_multi borrows W shard
+ * indexes (1 <= W <= 32, created with tav_create as usual, distinct, any devices, a device may repeat), shard g
+ * holding the contiguous block of global rows [starts[g], starts[g + 1]), in ascending block order.  It owns only the
+ * workspace of the fan-out and the merge: one non-blocking stream and one event per shard on the shard's device, a
+ * stream on `home_device`, and the buffers below.  tav_multi_create enables peer access between the distinct devices
+ * where cudaDeviceCanAccessPeer allows it.  Destroy the tav_multi before its shards.  Calls on one tav_multi are
+ * serialised by a mutex; every call restores the caller's current device.
+ *
+ * `starts` (host int64 [W + 1], starts[0] == 0) must match the shards' sizes (else TAV_ERR_INVALID).  Queries are host
+ * float32 [n_queries, dim], outputs host memory; both calls synchronise once at the end.  Flags: TAV_FORCE_SCAN,
+ * TAV_FORCE_MMA, TAV_USE_ROW_MASK (each shard's block of the mask set on that shard with tav_set_row_mask first; a
+ * shard without rows ignores it) and TAV_TIES_LOW_FIRST; any other flag: TAV_ERR_INVALID.  The result equals, bit for
+ * bit, the same call on one index holding every row: the per-shard searches are the library's searches of the blocks
+ * (ordinals shifted by starts[g]) and the merges keep one index's order.
+ *
+ *   tav_multi_search        the queries are copied once into pinned memory and to each shard's device; every shard's
+ *                           tav_search (both _ON_DEVICE flags, TAV_DEFER_RETRY) is launched before anything waits;
+ *                           tav_finish_search completes each (the exact redo runs before the merge); each [B, k] list
+ *                           is copied into a slab on the home device (cudaMemcpyPeerAsync), the home stream waits on the
+ *                           shards' events and merges with tav_merge_topk_ordered (order 0, 1 with ties-low-first).
+ *                           1 <= k <= 8192 (the merge's limit; tav_multi_range_search serves "every hit").
+ *   tav_multi_range_search  every hit at or above min_score, CSR offsets out_offsets [n_queries + 1] (host).  Each
+ *                           shard runs tav_range_search_into with TAV_DEFER_RETRY into buffers of the tav_multi sized
+ *                           from expected_hits (the whole batch's hint, as tav_range_search takes it); after the
+ *                           finishes a shard whose total exceeds its room is searched again with room enough.  The
+ *                           shards' CSR results are copied to the home device and merged by tav_merge_range.  The hits
+ *                           stay in the tav_multi until the next tav_multi_range_search.
+ *   tav_multi_range_fetch   copies hits [first, first + n) of the last tav_multi_range_search to host memory
+ *                           (TAV_ERR_RANGE beyond its total).
+ *
+ * Subset: the host ordinals are split by block on the host (negative ordinals wrap against the global row count
+ * starts[W]; any ordinal outside [-starts[W], starts[W]): TAV_ERR_RANGE before any work).  Each shard searches its share
+ * with block-local ordinals and TAV_ITEMS_AS_POSITIONS (a threshold search of a share runs tav_range_search, which
+ * synchronises, then tav_range_fetch), the positions are mapped to positions in the caller's subset, merged by
+ * position (top-k order 2, or 3 with ties-low-first) and decoded through the caller's subset (tav_map_items): repeats,
+ * negative ordinals and the subset's tie order come back as one index returns them.
+ *
+ * Errors: a shard that fails fails the call with its status and message; every other shard is still finished and its
+ * stream synchronised, so nothing is left outstanding, and the tav_multi and every index stay usable.
+ */
+typedef struct tav_multi tav_multi;
+int tav_multi_create(int home_device, int n_shards, tav_index* const* shards, tav_multi** out);
+int tav_multi_destroy(tav_multi* m);
+int tav_multi_search(tav_multi* m, const int64_t* starts, const float* queries, int n_queries, int k, float min_score,
+                     int flags, const int64_t* subset, int64_t subset_len, int64_t* out_items, float* out_scores,
+                     int32_t* out_counts);
+int tav_multi_range_search(tav_multi* m, const int64_t* starts, const float* queries, int n_queries, float min_score,
+                           int flags, const int64_t* subset, int64_t subset_len, int64_t expected_hits,
+                           int64_t* out_offsets);
+int tav_multi_range_fetch(tav_multi* m, int64_t first, int64_t n, int64_t* out_items, float* out_scores);
+
+/*
  * Chunk -> message fold of hit lists, on the device, in place (storage/memory/messageindex.py:
  * 185-207 `to_scored_message_ordinals`; the reference folds AFTER the top-k over chunks): walking
  * each query's hits in score order, the first hit of a group keeps its score, later hits of the

@@ -102,6 +102,13 @@ SIGNATURES = {
     "tav_map_items": (C.c_int, [C.c_int, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "tav_merge_range": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                   C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tav_multi_create": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "tav_multi_destroy": (C.c_int, [C.c_void_p]),
+    "tav_multi_search": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int,
+                                   C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tav_multi_range_search": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p,
+                                         C.c_int64, C.c_int64, C.c_void_p]),
+    "tav_multi_range_fetch": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
     "tav_mma_scores": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "tav_set_timing": (C.c_int, [C.c_void_p, C.c_int]),
     "tav_timing_breakdown": (C.c_int, [C.c_void_p, _f32p, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]),

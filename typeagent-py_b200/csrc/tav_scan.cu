@@ -1006,24 +1006,6 @@ merge_kernel(int n_lists, int n_queries, int k, const int64_t* items, const floa
     }
 }
 
-cudaError_t launch_merge(int n_lists, int n_queries, int k, const int64_t* items,
-                         const float* scores, const int32_t* counts, int64_t items_stride,
-                         int64_t scores_stride, int64_t counts_stride, int64_t* out_items,
-                         float* out_scores, int32_t* out_counts, cudaStream_t s) {
-    if (items_stride == 0) items_stride = static_cast<int64_t>(n_queries) * k;
-    if (scores_stride == 0) scores_stride = static_cast<int64_t>(n_queries) * k;
-    if (counts_stride == 0) counts_stride = n_queries;
-    const size_t smem = static_cast<size_t>(select_cap(k)) * sizeof(uint64_t);
-    static int granted[16] = {};
-    cudaError_t e = ensure_dynamic_smem(merge_kernel<0>, smem, granted);
-    if (e != cudaSuccess) return e;
-    merge_kernel<0><<<n_queries, kSelectThreads, smem, s>>>(n_lists, n_queries, k, items, scores,
-                                                            counts, items_stride, scores_stride,
-                                                            counts_stride, out_items, out_scores,
-                                                            out_counts, MergeSync{});
-    return cudaGetLastError();
-}
-
 template <int ORDER>
 static cudaError_t launch_merge_t(int n_lists, int n_queries, int k, const int64_t* items, const float* scores,
                                   const int32_t* counts, int64_t items_stride, int64_t scores_stride,
@@ -1061,6 +1043,19 @@ cudaError_t launch_merge_ordered(int n_lists, int n_queries, int k, const int64_
                                          counts_stride, out_items, out_scores, out_counts, s, sync ? *sync : none);
     }
     return cudaErrorInvalidValue;
+}
+
+// tav_merge_topk's merge is order 0 of the ordered merge: one launch path, so that merge_kernel<0> has one record
+// of the shared memory it was granted (two records of one kernel's attribute could lower it under the other's feet)
+cudaError_t launch_merge(int n_lists, int n_queries, int k, const int64_t* items,
+                         const float* scores, const int32_t* counts, int64_t items_stride,
+                         int64_t scores_stride, int64_t counts_stride, int64_t* out_items,
+                         float* out_scores, int32_t* out_counts, cudaStream_t s) {
+    if (items_stride == 0) items_stride = static_cast<int64_t>(n_queries) * k;
+    if (scores_stride == 0) scores_stride = static_cast<int64_t>(n_queries) * k;
+    if (counts_stride == 0) counts_stride = n_queries;
+    return launch_merge_t<0>(n_lists, n_queries, k, items, scores, counts, items_stride, scores_stride, counts_stride,
+                             out_items, out_scores, out_counts, s, MergeSync{});
 }
 
 // ---- items[i] = table[items[i]] (subset positions -> global positions -> the caller's ordinals) --------

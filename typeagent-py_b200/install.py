@@ -77,8 +77,9 @@ def _patch(mod_name: str, owner, name: str, value, patched: list[str], label: st
 
 
 def install(**vectorbase_options) -> list[str]:
-    """Rebind the names; ``vectorbase_options`` (device=, storage_dtype=, normalize=) become
-    the defaults of every VectorBase typeagent constructs afterwards."""
+    """Rebind the names; ``vectorbase_options`` (device=, storage_dtype=, normalize=, or devices= for the rows
+    of every index in blocks over several GPUs of this process) become the defaults of every VectorBase typeagent
+    constructs afterwards."""
     from . import vectorbase
 
     if vectorbase_options:

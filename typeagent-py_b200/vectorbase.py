@@ -21,6 +21,8 @@ Additions (not in the reference; all opt-in):
     batched lookup in which every query scores only its own candidate ordinals (the batched form of
     ``fuzzy_lookup_embedding_in_subset``, vectorbase.py:203-230: candidate re-ranking);
   * constructor keywords ``device``, ``storage_dtype``, ``normalize``;
+  * ``devices=[...]`` — the rows in contiguous blocks over several GPUs of this process, every lookup fanned out to
+    all of them and merged on the first (``multi.py``, ``tav_multi_*``);
   * ``from_device_tensor`` / ``search_device`` / ``search_range_device`` — torch tensors as device-memory
     handles (the threshold search into caller tensors, sized on the device, optionally without a host
     synchronisation).
@@ -131,16 +133,30 @@ class VectorBase:
         self,
         settings: TextEmbeddingIndexSettings,
         *,
-        device: int = 0,
+        device: int | None = None,
         storage_dtype: str = "float32",
         normalize: bool = False,
+        devices: Sequence[int] | None = None,
     ):
+        """``device``: the CUDA ordinal of the index (default 0).  ``devices``: CUDA ordinals (1 to 32, repeats
+        allowed) to hold the rows in contiguous blocks, one per entry, every lookup searching all of them and merging
+        on the first; exclusive with ``device``.  Per-query masks and subsets and the device-tensor forms are not
+        available with ``devices`` (NotImplementedError)."""
         if storage_dtype not in _capi.DTYPE_CODES:
             raise ValueError(f"storage_dtype must be one of {sorted(_capi.DTYPE_CODES)}")
+        self._multi = None
+        if devices is not None:
+            if device is not None:
+                raise ValueError("device= and devices= cannot be combined")
+            from .multi import MultiDevice, check_devices
+
+            devices = check_devices(devices)
+            self._multi = MultiDevice(devices, storage_dtype, normalize)
+            device = devices[0]
         self.settings = settings
         self._model = settings.embedding_model
         self._embedding_size = 0
-        self._device = int(device)
+        self._device = 0 if device is None else int(device)
         self._storage_dtype = storage_dtype
         self._normalize = bool(normalize)
         # host mirror: growable float32 buffer, `_count` rows valid
@@ -339,7 +355,10 @@ class VectorBase:
         removed = removal_ordinals(ordinals, n)
         if removed.size == 0:
             return
-        if self._device_in_sync():
+        if self._multi is not None:
+            if self._multi.in_sync(self._generation):
+                self._multi.remove(_capi.load(), removed)
+        elif self._device_in_sync():
             on_device = np.ascontiguousarray(removed[removed < self._ix_rows])
             if len(on_device):
                 _capi.check(_capi.load().tav_remove_rows(self._ix, on_device.ctypes.data_as(C.c_void_p),
@@ -398,7 +417,10 @@ class VectorBase:
             )
         if n == 0:
             return
-        if self._device_in_sync() and first < self._ix_rows:
+        if self._multi is not None:
+            if self._multi.in_sync(self._generation):
+                self._multi.write(_capi.load(), first, rows)
+        elif self._device_in_sync() and first < self._ix_rows:
             m = min(n, self._ix_rows - first)
             _capi.check(_capi.load().tav_write_rows(self._ix, first, rows.ctypes.data_as(C.c_void_p), m,
                                                     self._embedding_size, _capi.TAV_F32, 0, None))
@@ -416,6 +438,8 @@ class VectorBase:
 
     # ------------------------------------------------------------------ device plumbing
     def _drop_device(self) -> None:
+        if self._multi is not None and self._multi.shards is not None:
+            self._multi.close(_capi.load())
         if self._ix is not None:
             lib = _capi.load()
             lib.tav_destroy(self._ix)
@@ -425,6 +449,10 @@ class VectorBase:
     def _ensure_device(self):
         """Bring the device copy up to date with the host mirror; returns (lib, handle)."""
         lib = _capi.load()
+        if self._multi is not None:
+            if self._multi.sync(lib, self._buf[: self._count], self._generation, self._embedding_size):
+                self._mask_key = None
+            return lib, None
         if self._ix is None:
             handle = C.c_void_p()
             flags = _capi.TAV_NORMALIZE if self._normalize else 0
@@ -498,7 +526,10 @@ class VectorBase:
         if len(words) != (n + 31) // 32:
             raise ValueError(f"row mask has {len(words) * 32} bits for {n} rows")
         words = np.ascontiguousarray(words)
-        _capi.check(lib.tav_set_row_mask(ix, words.ctypes.data_as(C.c_void_p), n, 0, None))
+        if self._multi is not None:
+            self._multi.set_row_mask(lib, words, n)
+        else:
+            _capi.check(lib.tav_set_row_mask(ix, words.ctypes.data_as(C.c_void_p), n, 0, None))
         self._mask_key = key
         self._mask_ref = (allowed, owner)
 
@@ -555,6 +586,17 @@ class VectorBase:
         self._qmask_key = key
         self._qmask_ref = allowed
 
+    def _single_device_only(self, what: str) -> None:
+        """NotImplementedError, before any device work, for what a multi-device index does not offer yet."""
+        if self._multi is not None:
+            raise NotImplementedError(f"{what} is not available on a VectorBase over several devices (devices=)")
+
+    def _refuse_multi(self, allowed, subsets) -> None:
+        if subsets is not None:
+            self._single_device_only("subsets= (per-query subsets)")
+        if self._is_query_masks(allowed):
+            self._single_device_only("a 2-D allowed= (per-query masks)")
+
     def _check_queries(self, queries) -> np.ndarray:
         q = np.ascontiguousarray(queries, dtype=np.float32)
         if q.ndim == 1:
@@ -587,6 +629,7 @@ class VectorBase:
         search; ``ties_low_first`` orders exactly equal scores by ascending ordinal (row-scan path).
         ``subsets`` (B one-dimensional integer sequences) gives every query its own subset, in one batched
         search: row b equals the one-query search with ``subset=subsets[b]``; `k` is clamped to the longest."""
+        self._refuse_multi(allowed, subsets)
         q = self._check_queries(queries)
         b = len(q)
         if k < 1:
@@ -648,6 +691,9 @@ class VectorBase:
         if ties_low_first:
             flags |= _capi.TAV_TIES_LOW_FIRST
         with self._single_lock:
+            if self._multi is not None:
+                self._multi.topk(lib, q, k_eff, floor, flags, sub, items, scores, counts)
+                return items, scores, counts
             _capi.check(
                 lib.tav_search(
                     ix, q.ctypes.data_as(C.c_void_p), b, k_eff, C.c_float(float(floor)), flags,
@@ -674,6 +720,7 @@ class VectorBase:
         equal scores higher ordinal first, or lower first with ``ties_low_first``).  ``subset``, ``subsets`` and
         ``allowed`` (1-D, or 2-D: one mask per query) as in ``search_arrays``.  Batches run on the tensor cores (16-bit storage, or float32
         through its fp16 planes), like ``search_arrays``.  The previous call's total sizes the device buffers."""
+        self._refuse_multi(allowed, subsets)
         q = self._check_queries(queries)
         b = len(q)
         n_rows = len(self)
@@ -725,6 +772,10 @@ class VectorBase:
             flags |= _capi.TAV_USE_ROW_MASK
         if ties_low_first:
             flags |= _capi.TAV_TIES_LOW_FIRST
+        if self._multi is not None:
+            _, items, scores = self._multi.range(lib, q, floor, flags, sub, self._range_hint, offsets)
+            self._range_hint = int(offsets[-1])
+            return offsets, items, scores
         _capi.check(
             lib.tav_range_search(
                 ix, q.ctypes.data_as(C.c_void_p), b, C.c_float(float(floor)), flags,
@@ -881,9 +932,13 @@ class VectorBase:
             qp = C.addressof(C.c_char.from_buffer(q))
         except (TypeError, ValueError):      # read-only query buffer
             qp = q.ctypes.data
-        rc = lib.tav_search(ix, qp, 1, k_eff, floor, self._flags(), sub_ptr, sub_len, 0, ip, sp, cp, None)
-        if rc < 0:
-            _capi.check(rc)
+        if self._multi is not None:
+            self._multi.topk(lib, q.reshape(1, -1), k_eff, floor, self._flags(),
+                             sub[:sub_len] if sub is not None else None, items, scores, counts)
+        else:
+            rc = lib.tav_search(ix, qp, 1, k_eff, floor, self._flags(), sub_ptr, sub_len, 0, ip, sp, cp, None)
+            if rc < 0:
+                _capi.check(rc)
         c = int(counts[0])
         return [ScoredInt(i, s_) for i, s_ in zip(items[0, :c].tolist(), scores[0, :c].tolist())]
 
@@ -989,6 +1044,7 @@ class VectorBase:
     ) -> list[list[ScoredInt]]:
         """One batched GPU search in which query b scores only ``ordinals_of_subsets[b]``; element b equals
         ``fuzzy_lookup_embedding_in_subset(embeddings[b], ordinals_of_subsets[b], max_hits, min_score)``."""
+        self._single_device_only("fuzzy_lookup_embeddings_in_subsets (per-query subsets)")
         if min_score is None:
             min_score = 0.0
         q = np.asarray(embeddings, dtype=np.float32)
@@ -1041,6 +1097,9 @@ class VectorBase:
     def from_device_tensor(cls, settings, tensor, **kw) -> "VectorBase":
         """Wrap a CUDA tensor [N, D] (float32 / bfloat16 / float16, contiguous) as the
         corpus without copying it and without a host mirror (benchmark-scale corpora)."""
+        if kw.get("devices") is not None:
+            raise NotImplementedError("from_device_tensor is not available on a VectorBase over several devices "
+                                      "(devices=)")
         import torch
 
         if not (tensor.is_cuda and tensor.dim() == 2 and tensor.is_contiguous()):
@@ -1067,6 +1126,7 @@ class VectorBase:
         tensor [B, ceil(N / 32)] of packed words, copied on the current stream).  ``row_to_group``: int32 CUDA tensor [N];
         the hits are then folded on the device like the reference's chunk -> message fold
         (storage/memory/messageindex.py:185-207): first hit per group, items = group ordinals."""
+        self._single_device_only("search_device")
         import torch
 
         if not (queries.is_cuda and queries.dtype == torch.float32 and queries.is_contiguous()):
@@ -1127,6 +1187,7 @@ class VectorBase:
         ``expected_hits`` (default ``capacity``) sizes the device collect regions; it never changes the result.
         The call synchronises once (more when a query overflowed its region); with ``defer_check=True`` it does
         not synchronise at all, and ``finish_search()`` must run before the results are trusted."""
+        self._single_device_only("search_range_device")
         import torch
 
         if not (getattr(queries, "is_cuda", False) and queries.dtype == torch.float32 and queries.is_contiguous()):
@@ -1205,6 +1266,7 @@ class VectorBase:
         """Complete every outstanding ``search_device(..., defer_check=True)`` and
         ``search_range_device(..., defer_check=True)``: synchronise, redo (exactly) the queries the device search
         flagged, return how many there were."""
+        self._single_device_only("finish_search")
         if not self._pending:
             return 0
         stream = self._pending[-1][4]
