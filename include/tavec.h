@@ -267,6 +267,43 @@ int tav_search_subsets(tav_index* ix, const float* queries, int n_queries, int k
 int tav_range_search_subsets(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
                              const int64_t* offsets, const int64_t* ordinals, int64_t* out_offsets, void* stream);
 
+/*
+ * Per-query subsets from device memory: tav_search_subsets / tav_range_search_subsets for callers whose candidate
+ * lists are already on the GPU, checked, planned and searched on the device with no host round trip.  Every pointer
+ * is device memory on the index's device: queries float32 [n_queries, dim], offsets int64 [n_queries + 1], ordinals
+ * int64 [n_ordinals], and the outputs.  Row q of the result equals, bit for bit, the host form's on the same CSR:
+ * the same items, score bits, counts or offsets, order, repeats, negative ordinals returned as given and tie order.
+ *
+ * Flags: TAV_DEFER_RETRY, TAV_TIES_LOW_FIRST, TAV_ITEMS_AS_POSITIONS; TAV_QUERIES_ON_DEVICE and
+ * TAV_OUTPUTS_ON_DEVICE are accepted and change nothing; any other flag: TAV_ERR_INVALID.  Checked on the host
+ * before any work (TAV_ERR_INVALID): n_ordinals outside [0, 2^32 - 1], capacity < 0, k < 1, a NULL pointer that is
+ * needed.  Checked on the device before any access: the offsets must start at 0, never decrease and end at
+ * n_ordinals (else TAV_ERR_INVALID, and no work is planned); every ordinal must lie in [-size, size) (else
+ * TAV_ERR_RANGE; the row of an ordinal outside is never read).  A refused search leaves counts 0, items -1 and
+ * scores 0 (top-k form), or all offsets 0 with the items and scores untouched (threshold form).  No queries, no
+ * entries, an empty index or a NaN min_score give no hits, and the ordinals are not looked at.
+ *
+ * Without TAV_DEFER_RETRY the call synchronises `stream` once, to read the device checks' status, and returns
+ * their error.  With it the call makes no host synchronisation (growing a device buffer may allocate) and joins the
+ * deferred searches tav_finish_search completes (at most 64 outstanding, shared with tav_search); the finish reports
+ * a refusal after it has completed every other outstanding search, with the first such error.  The caller keeps
+ * the queries, offsets, ordinals and outputs alive until then; on a TAV_NORMALIZE index the normalised queries are
+ * held by the library.  The calls join the index's call order across streams, replace the hits of the last range
+ * search (tav_range_fetch gives TAV_ERR_STATE afterwards, as after tav_range_search_into) and are timed as path 1.
+ *
+ * tav_search_subsets_into: out_items / out_scores [n_queries, k], out_counts [n_queries], padding item -1 and
+ * score 0.  k is not clamped.
+ * tav_range_search_subsets_into: the contract of tav_range_search_into's outputs.  out_offsets [n_queries + 1] is
+ * always complete; hits at CSR positions >= capacity are not written, and those slots keep what they held.
+ */
+int tav_search_subsets_into(tav_index* ix, const float* queries, int n_queries, int k, float min_score, int flags,
+                            const int64_t* offsets, const int64_t* ordinals, int64_t n_ordinals,
+                            int64_t* out_items, float* out_scores, int32_t* out_counts, void* stream);
+int tav_range_search_subsets_into(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
+                                  const int64_t* offsets, const int64_t* ordinals, int64_t n_ordinals,
+                                  int64_t capacity, int64_t* out_offsets, int64_t* out_items, float* out_scores,
+                                  void* stream);
+
 /* Completes EVERY outstanding TAV_DEFER_RETRY search of the index, whatever stream each was issued
  * on: waits until they have run (`stream` first waits for them, then is synchronised), redoes
  * each search's flagged queries exactly on `stream` into that search's own outputs and reports how many

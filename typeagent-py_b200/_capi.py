@@ -56,6 +56,11 @@ SIGNATURES = {
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tav_range_search_subsets": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tav_search_subsets_into": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p,
+                                          C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tav_range_search_subsets_into": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p,
+                                                C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p]),
     "tav_range_fetch": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "tav_range_search_into": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_int64,
                                         C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -17,6 +17,7 @@
 #include <atomic>
 #include <mutex>
 #include <new>
+#include <string>
 #include <vector>
 
 #include "tav_common.cuh"
@@ -132,6 +133,9 @@ struct Pending {
     int64_t expected_hits = 0;
     QueryMasks qm{};                  // per-query masks of the whole search (nq > 1)
     int per_chunk = 0, n_seg = 0;     // the tensor-core collection plan a re-pass repeats (0: the row scan)
+    // per-query subsets from device memory (tav_search_subsets_into / _range_): the search's status word (device),
+    // read at the finish; nothing is redone
+    const int* subsets_status = nullptr;
 };
 
 }  // namespace tav
@@ -218,6 +222,11 @@ struct tav_index {
     bool range_replaced = false; // a tav_range_search_into ran after it: tav_range_fetch has nothing to copy
     // per-query subsets: device [offsets | work-item starts | CSR offsets of the hits], each n_queries + 1
     DevBuf subsets_meta;
+    // per-query subsets from device memory: the status words, [kMaxPending] of deferred searches by bookkeeping slot
+    // and one of the synchronous form; the first refusal a finish met, reported by tav_finish_search
+    DevBuf subsets_status;
+    int deferred_rc = TAV_OK;
+    std::string deferred_msg;
 
     // call order on the device (join_stream / mark_queued / wait_queued): ev_last marks the end of the work
     // of the calls so far while `outstanding`; last_stream is ordered after it
@@ -319,6 +328,17 @@ static int check_subset_ordinals(const tav_index* ix, const int64_t* ordinals, i
             return TAV_ERR_RANGE;
         }
     return TAV_OK;
+}
+
+// The error of a per-query subset search from device memory that its status word `st` (non-zero) refused, with its
+// message; `size` is the index's row count when the search was issued.
+static int subsets_status_error(int st, int64_t size) {
+    if (st & kSubsetBadOffsets) {
+        set_error("per-query subsets: offsets must be n_queries + 1 values from 0 to n_ordinals, never decreasing");
+        return TAV_ERR_INVALID;
+    }
+    set_error("per-query subsets: an ordinal is out of bounds for axis 0 with size %lld", (long long)size);
+    return TAV_ERR_RANGE;
 }
 
 static void destroy_history(tav_index* ix) {
@@ -996,10 +1016,16 @@ static int finish_pending(tav_index* ix, cudaStream_t s, int* redone) {
     if (int rc = join_stream(ix, s)) return rc;  // the searches may have been issued on other streams
     int32_t totals[2 * kMaxPending];
     int corpus_overflow = 0;
-    bool any_split = false;
-    for (const Pending& p : ix->pending) any_split |= p.split;
+    bool any_split = false, any_subsets = false;
+    for (const Pending& p : ix->pending) {
+        any_split |= p.split;
+        any_subsets |= p.subsets_status != nullptr;
+    }
     if (any_split)
         TAV_CUDA(cudaMemcpyAsync(&corpus_overflow, ix->split_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+    int status[kMaxPending];
+    if (any_subsets)
+        TAV_CUDA(cudaMemcpyAsync(status, ix->subsets_status.p, sizeof(status), cudaMemcpyDeviceToHost, s));
     TAV_CUDA(cudaStreamSynchronize(s));
     memcpy(totals, ix->retry_host.p, sizeof(totals));  // written by the kernels through the mapping; current after the sync
     std::vector<Pending> todo;
@@ -1009,6 +1035,13 @@ static int finish_pending(tav_index* ix, cudaStream_t s, int* redone) {
     int n_redone = 0;
     std::vector<int32_t> host;
     for (const Pending& p : todo) {
+        if (p.subsets_status && TAV_SUBSETS_DEVICE_MUTANT != 2) {  // refused on the device: its outputs say no hits
+            const int st = status[p.slot];
+            if (st && ix->deferred_rc == TAV_OK) {
+                ix->deferred_rc = subsets_status_error(st, p.n_scan);
+                ix->deferred_msg = tav_last_error();
+            }
+        }
         const int flagged = totals[2 * p.slot], q_overflow = totals[2 * p.slot + 1];
         const bool redo_all = p.split && (corpus_overflow != 0 || q_overflow != 0);
         dirty |= flagged != 0 || q_overflow != 0;
@@ -1576,6 +1609,9 @@ struct PlanDest {
     int32_t* n_flagged = nullptr;
     int32_t* n_flagged_host = nullptr;
     const int* abandon[2] = {nullptr, nullptr};
+    // per-query subsets: query q's keys at keys + key_off[q] (device), total_keys in all (region, key_stride unused)
+    const int64_t* key_off = nullptr;
+    int64_t total_keys = 0;
 };
 
 // The device plan of nq queries whose counters are count / fill (see RangePlanArgs), at most `region` keys per
@@ -1585,12 +1621,19 @@ static int range_plan(tav_index* ix, TimedSearch* ts, int nq, const uint32_t* co
                       int64_t region, int64_t key_stride, uint64_t* keys, const int64_t* d_subset, int64_t item_offset,
                       int ties_low, const RangeOut& out, const PlanDest& dest, SortArgs* sa, const int** sizes,
                       int64_t** dst_off, cudaStream_t s) {
-    const bool any_large = region > kSmallSortMax;
-    const int n_large_max = any_large ? nq : 0;
-    const int64_t tiles_max = any_large ? static_cast<int64_t>(nq) * ((region + kRadixTile - 1) / kRadixTile) : 0;
+    const bool var = dest.key_off != nullptr;
+    const bool any_large = (var ? dest.total_keys : region) > kSmallSortMax;
+    // variable bases: at most total / (kSmallSortMax + 1) large segments, whose tiles number at most
+    // total / kRadixTile + one partial tile each
+    const int n_large_max =
+        !any_large ? 0 : var ? static_cast<int>(std::min<int64_t>(nq, dest.total_keys / (kSmallSortMax + 1))) : nq;
+    const int64_t tiles_max = !any_large ? 0
+                              : var      ? dest.total_keys / kRadixTile + n_large_max
+                                         : static_cast<int64_t>(nq) * ((region + kRadixTile - 1) / kRadixTile);
     uint64_t* tmp = nullptr;
     if (any_large) {
-        if (int rc = range_alloc(ix->range_tmp, static_cast<size_t>(nq) * region * sizeof(uint64_t), "the sort scratch"))
+        const int64_t tmp_keys = var ? dest.total_keys : static_cast<int64_t>(nq) * region;
+        if (int rc = range_alloc(ix->range_tmp, static_cast<size_t>(tmp_keys) * sizeof(uint64_t), "the sort scratch"))
             return rc;
         tmp = static_cast<uint64_t*>(ix->range_tmp.p);
     }
@@ -1622,7 +1665,7 @@ static int range_plan(tav_index* ix, TimedSearch* ts, int nq, const uint32_t* co
     pa.out_base = dest.base ? reinterpret_cast<const int64_t*>(ws + o_base) : nullptr;
     pa.abandon[0] = dest.abandon[0];
     pa.abandon[1] = dest.abandon[1];
-    pa.dst_off = key_stride ? nullptr : reinterpret_cast<int64_t*>(ws + o_dst);
+    pa.dst_off = key_stride || var ? nullptr : reinterpret_cast<int64_t*>(ws + o_dst);
     pa.flags = dest.flags;
     pa.n_flagged = dest.n_flagged;
     pa.n_flagged_host = dest.n_flagged_host;
@@ -1631,7 +1674,7 @@ static int range_plan(tav_index* ix, TimedSearch* ts, int nq, const uint32_t* co
     pa.tile_seg = reinterpret_cast<int*>(ws + o_tiles);
     pa.minmax = reinterpret_cast<uint64_t*>(ws + o_minmax);
     pa.sizes = reinterpret_cast<int*>(ws + o_sizes);
-    TAV_CUDA(launch_range_plan(pa, s));
+    TAV_CUDA(var ? launch_range_plan_subsets(pa, dest.key_off, s) : launch_range_plan(pa, s));
     ts->launches += 1;
 
     *sa = SortArgs{};
@@ -2307,9 +2350,15 @@ int tav_finish_search(tav_index* ix, void* stream, int* redone) {
     if (!ix) return TAV_ERR_INVALID;
     std::lock_guard<std::mutex> lock(ix->mu);
     if (redone) *redone = 0;
-    if (ix->pending.empty()) return TAV_OK;  // nothing deferred (row-scan path, or already finished)
-    if (int rc = set_device(ix)) return rc;
-    return finish_pending(ix, static_cast<cudaStream_t>(stream), redone);
+    if (!ix->pending.empty()) {  // (else nothing deferred: row-scan path, or already finished)
+        if (int rc = set_device(ix)) return rc;
+        if (int rc = finish_pending(ix, static_cast<cudaStream_t>(stream), redone)) return rc;
+    }
+    // a deferred subset search refused on the device, here or in an earlier finish the library ran itself
+    const int rc = ix->deferred_rc;
+    if (rc != TAV_OK) set_error("%s", ix->deferred_msg.c_str());
+    ix->deferred_rc = TAV_OK;
+    return rc;
 }
 
 int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float min_score,
@@ -2934,6 +2983,136 @@ static int subsets_core(tav_index* ix, TimedSearch* ts, bool timing, const float
     return range_sort(ix, ts, timing, segs, csr[nq], positions ? nullptr : d_ordinals, 0, ties_low, s);
 }
 
+// ---- per-query subsets from device memory (tav_search_subsets_into, tav_range_search_subsets_into) -----------
+// The same gather and sort as above with no host round trip: the offsets are checked and the work items planned on
+// the device (subset_plan_kernel), the gather runs over an upper bound of the items and range-checks every ordinal,
+// and the sort is planned on the device (range_plan_subsets_kernel) and launched over upper bounds.  A refusal sets
+// the search's status word: no work is planned (offsets) or no row address is formed from the ordinal, and the plan
+// of the sort then gives every query 0 hits.
+constexpr int kSubsetsIntoFlags = kSubsetsFlags | TAV_DEFER_RETRY;
+
+// k > 0: the top-k form (its CSR hits in ix->range_items / range_scores, laid out into items / scores / counts);
+// k == 0: the threshold form into `out`.  The caller has checked the arguments and entered s; B, the entries, the
+// rows and min_score are not empty.
+static int subsets_into(tav_index* ix, const char* fn, const float* queries, int nq, int k, float floor, int flags,
+                        const int64_t* offsets, const int64_t* ordinals, int64_t n_ord, RangeOut out, int64_t* items,
+                        float* scores, int32_t* counts, cudaStream_t s) {
+    if (scan_collect_max_queries(ix->dim) < 1) {  // one query row in shared memory, as the row scan stages it
+        set_error("%s: embedding size %d too large for the row-scan kernel", fn, ix->dim);
+        return TAV_ERR_INVALID;
+    }
+    const bool defer = flags & TAV_DEFER_RETRY;
+    const int ties_low = (flags & TAV_TIES_LOW_FIRST) ? 1 : 0;
+    const int positions = (flags & TAV_ITEMS_AS_POSITIONS) ? 1 : 0;
+    if (!ix->subsets_status.p) {
+        TAV_CUDA(ix->subsets_status.ensure((kMaxPending + 1) * sizeof(int)));
+        TAV_CUDA(cudaMemsetAsync(ix->subsets_status.p, 0, (kMaxPending + 1) * sizeof(int), s));
+    }
+    int slot = kMaxPending;  // the synchronous form's word
+    float* held = nullptr;
+    if (defer) {
+        // a bookkeeping slot (its status word), as for the other deferred searches; nothing is redone at the finish
+        if (int rc = ensure_retry(ix, 0, 0, s)) return rc;
+        if (static_cast<int>(ix->pending.size()) >= kMaxPending)
+            if (int rc = finish_pending(ix, s, nullptr)) return rc;
+        if (ix->flags & TAV_NORMALIZE) {  // the normalised queries stay the search's own until the finish
+            void* r = nullptr;
+            size_t end = 0;
+            if (int rc = hold_region(ix, static_cast<size_t>(nq) * ix->dim * sizeof(float), &r, &end)) return rc;
+            held = static_cast<float*>(r);
+        }
+        slot = ix->next_slot++;
+    }
+    int* status = static_cast<int*>(ix->subsets_status.p) + slot;
+    auto run = [&]() -> int {
+        TimedSearch* ts = begin_search(ix, 1);
+        const bool timing = ts != &ix->untimed;
+        const float* d_queries = nullptr;
+        const int64_t* no_subset = nullptr;
+        if (int rc = stage_inputs(ix, ts, timing, queries, nq, true, true, nullptr, 0, &d_queries, &no_subset, s, held))
+            return rc;
+        ix->range_total = 0;  // the hits of the last tav_range_search are given up (the sort scratch is reused)
+        ix->range_replaced = true;
+        // device [work0 | CSR offsets of the top-k form's hits | planned work items]
+        const size_t n1 = static_cast<size_t>(nq) + 1;
+        if (int rc = range_alloc(ix->subsets_meta, (2 * n1 + 1) * sizeof(int64_t), "the subset plan")) return rc;
+        int64_t* work0 = static_cast<int64_t*>(ix->subsets_meta.p);
+        int64_t* n_work = work0 + 2 * n1;
+        if (k > 0) {
+            if (int rc = range_alloc(ix->range_items, static_cast<size_t>(n_ord) * sizeof(int64_t), "the hits")) return rc;
+            if (int rc = range_alloc(ix->range_scores, static_cast<size_t>(n_ord) * sizeof(float), "the hit scores"))
+                return rc;
+            out = RangeOut{work0 + n1, static_cast<int64_t*>(ix->range_items.p), static_cast<float*>(ix->range_scores.p),
+                           n_ord};
+        }
+        if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(n_ord) * sizeof(uint64_t), "the hit regions")) return rc;
+        if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(nq) * sizeof(uint32_t), "the hit counters")) return rc;
+        uint32_t* d_counts = static_cast<uint32_t*>(ix->range_counts.p);
+        uint64_t* keys = static_cast<uint64_t*>(ix->range_keys.p);
+        TAV_CUDA(cudaMemsetAsync(status, 0, sizeof(int), s));
+        TAV_CUDA(cudaMemsetAsync(d_counts, 0, static_cast<size_t>(nq) * sizeof(uint32_t), s));
+
+        const SubsetPlanArgs pl{nq, offsets, n_ord, work0, n_work, status};
+        TAV_CUDA(timed_launch(ix, ts, timing, 2, s, [&] { return launch_subset_plan(pl, s); }));
+        ts->launches += 1;
+        SubsetArgs a{};
+        a.corpus = ix->rows;
+        a.dtype = ix->dtype;
+        a.n_corpus = ix->size;
+        a.dim = ix->dim;
+        a.queries = d_queries;
+        a.nq = nq;
+        a.ordinals = ordinals;
+        a.offsets = offsets;
+        a.work0 = work0;
+        a.n_work = (n_ord + kSubsetTile - 1) / kSubsetTile + nq;  // >= the planned items (one partial tile per query)
+        a.floor_score = floor;
+        a.ties_low = ties_low;
+        a.keys = keys;
+        a.counts = d_counts;
+        TAV_CUDA(timed_launch(ix, ts, timing, 0, s, [&] { return launch_subset_gather_dev(a, n_work, status, s); }));
+        ts->launches += 1;
+
+        PlanDest dest;
+        dest.offsets = out.offsets;
+        dest.abandon[0] = status;
+        dest.key_off = offsets;
+        dest.total_keys = n_ord;
+        SortArgs sa;
+        const int* sizes = nullptr;
+        int64_t* dst_off = nullptr;
+        // regions never overflow: fill = count, cap = every count
+        if (int rc = range_plan(ix, ts, nq, d_counts, d_counts, 0xFFFFFFFFu, 0, 0, keys, positions ? nullptr : ordinals, 0,
+                                ties_low, out, dest, &sa, &sizes, &dst_off, s))
+            return rc;
+        if (int rc = range_sort_dev(ix, ts, timing, sa, sizes, out.cap, s)) return rc;
+        if (k > 0) {
+            TAV_CUDA(launch_subset_topk_layout(nq, k, out.offsets, out.items, out.scores, items, scores, counts, s));
+            ts->launches += 1;
+        }
+        return end_search(ix, ts, s);
+    };
+    if (int rc = run()) {
+        if (defer) --ix->next_slot;  // the slot goes back (its status word is cleared by the next search that takes it)
+        return rc;
+    }
+    if (defer) {
+        // (the queries as the search read them: normalised into the held region, or the caller's)
+        Pending p{held ? held : queries, nq, k, floor, 0, items, scores, counts, slot, false, nullptr, 0};
+        p.offsets = k > 0 ? nullptr : out.offsets;
+        p.cap = out.cap;
+        p.n_scan = ix->size;
+        p.subsets_status = status;
+        ix->pending.push_back(p);
+        return mark_queued(ix, s);
+    }
+    int st = 0;
+    TAV_CUDA(cudaMemcpyAsync(&st, status, sizeof(int), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaStreamSynchronize(s));
+    mark_done(ix);
+    return st ? subsets_status_error(st, ix->size) : TAV_OK;
+}
+
 extern "C" {
 
 int tav_search_subsets(tav_index* ix, const float* queries, int n_queries, int k, float min_score, int flags,
@@ -3021,6 +3200,53 @@ int tav_range_search_subsets(tav_index* ix, const float* queries, int n_queries,
         ix->range_total = csr[n_queries];
     }
     return deliver_offsets(ix, csr, out_offsets, flags & TAV_OUTPUTS_ON_DEVICE, s);
+}
+
+int tav_search_subsets_into(tav_index* ix, const float* queries, int n_queries, int k, float min_score, int flags,
+                            const int64_t* offsets, const int64_t* ordinals, int64_t n_ordinals, int64_t* out_items,
+                            float* out_scores, int32_t* out_counts, void* stream) {
+    if (!ix || n_queries < 0 || k < 1 || (flags & ~kSubsetsIntoFlags) || n_ordinals < 0 || n_ordinals > 0xFFFFFFFFll ||
+        !offsets || (n_ordinals > 0 && !ordinals) ||
+        (n_queries > 0 && (!queries || !out_items || !out_scores || !out_counts))) {
+        set_error("tav_search_subsets_into: invalid argument (k >= 1, 0 <= n_ordinals < 2^32, accepted flags)");
+        return TAV_ERR_INVALID;
+    }
+    if (n_queries == 0) return TAV_OK;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = enter_stream(ix, s)) return rc;
+    // no entries, no rows or a NaN min_score: no hits (the ordinals are not looked at)
+    if (n_ordinals == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score) {
+        const size_t nk = static_cast<size_t>(n_queries) * k;
+        TAV_CUDA(cudaMemsetAsync(out_items, 0xFF, nk * sizeof(int64_t), s));
+        TAV_CUDA(cudaMemsetAsync(out_scores, 0, nk * sizeof(float), s));
+        TAV_CUDA(cudaMemsetAsync(out_counts, 0, static_cast<size_t>(n_queries) * sizeof(int32_t), s));
+        return mark_queued(ix, s);
+    }
+    return subsets_into(ix, "tav_search_subsets_into", queries, n_queries, k, min_score, flags, offsets, ordinals,
+                        n_ordinals, RangeOut{}, out_items, out_scores, out_counts, s);
+}
+
+int tav_range_search_subsets_into(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
+                                  const int64_t* offsets, const int64_t* ordinals, int64_t n_ordinals, int64_t capacity,
+                                  int64_t* out_offsets, int64_t* out_items, float* out_scores, void* stream) {
+    if (!ix || n_queries < 0 || (flags & ~kSubsetsIntoFlags) || n_ordinals < 0 || n_ordinals > 0xFFFFFFFFll ||
+        capacity < 0 || !offsets || (n_ordinals > 0 && !ordinals) || !out_offsets || (n_queries > 0 && !queries) ||
+        (capacity > 0 && (!out_items || !out_scores))) {
+        set_error("tav_range_search_subsets_into: invalid argument (0 <= n_ordinals < 2^32, capacity >= 0, accepted "
+                  "flags)");
+        return TAV_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(ix->mu);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = enter_stream(ix, s)) return rc;
+    // no queries, no entries, no rows or a NaN min_score: no hits (the ordinals are not looked at)
+    if (n_queries == 0 || n_ordinals == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score) {
+        TAV_CUDA(cudaMemsetAsync(out_offsets, 0, (static_cast<size_t>(n_queries) + 1) * sizeof(int64_t), s));
+        return mark_queued(ix, s);
+    }
+    return subsets_into(ix, "tav_range_search_subsets_into", queries, n_queries, 0, min_score, flags, offsets, ordinals,
+                        n_ordinals, RangeOut{out_offsets, out_items, out_scores, capacity}, nullptr, nullptr, nullptr, s);
 }
 
 int tav_mma_scores(tav_index* ix, const float* queries, int n_queries, int flags, float* out_device,

@@ -129,6 +129,32 @@ cudaError_t launch_subset_topk_layout(int nq, int k, const int64_t* csr_offsets,
 #define TAV_SUBSETS_MUTANT 0
 #endif
 
+// Per-query subsets from device memory (tav_search_subsets_into / tav_range_search_subsets_into): the offsets are
+// checked and the work items planned on the device.  The status word: bit 0 malformed offsets (the planner plans
+// no work), bit 1 an ordinal outside [-n_corpus, n_corpus) (the gather never forms that row's address).
+constexpr int kSubsetBadOffsets = 1, kSubsetBadOrdinal = 2;
+struct SubsetPlanArgs {
+    int nq;
+    const int64_t* offsets;   // device [nq + 1], the caller's
+    int64_t n_ordinals;       // offsets[nq] must equal it
+    int64_t* work0;           // device [nq + 1]
+    int64_t* n_work;          // device [1]: work0[nq], 0 when the offsets are refused
+    int* status;
+};
+cudaError_t launch_subset_plan(const SubsetPlanArgs& a, cudaStream_t s);
+// the gather over a device plan: a.n_work is an upper bound (ceil(n_ordinals / kSubsetTile) + nq), the items at or
+// past *n_work return at once, and each ordinal is range-checked before its row is read
+cudaError_t launch_subset_gather_dev(const SubsetArgs& a, const int64_t* n_work, int* status, cudaStream_t s);
+
+// TAV_SUBSETS_DEVICE_MUTANT (tests only, never set by build.py): 1..3 compile one deliberate defect each into the
+// device form, so that tests/test_gpu_subsets_device.py can show its checks catch it: 1 the planner drops the last
+// tile of a query whose length is a non-zero multiple of kSubsetTile, 2 a deferred finish ignores the status word,
+// 3 the plan of the sort ignores the status word (a refused search keeps its partial offsets).  No variant reads or
+// writes outside a buffer.
+#ifndef TAV_SUBSETS_DEVICE_MUTANT
+#define TAV_SUBSETS_DEVICE_MUTANT 0
+#endif
+
 // TAV_SCALE_MUTANT (tests only, never set by build.py): 1..3 compile one deliberate defect each that only shows on
 // corpora or subsets past 2^24 entries, so that tests/test_gpu_scale_exact.py can show its exact checks catch what
 // the small exact tests cannot: 1 the tensor-core MAIN epilogue keeps 24 bits of the row in its keys, 2 the subset
@@ -194,6 +220,9 @@ struct RangePlanArgs {
     int* sizes;              // [2] large segments, radix tiles
 };
 cudaError_t launch_range_plan(const RangePlanArgs& a, cudaStream_t s);
+// the same plan over per-query subsets: query q's keys (and radix scratch) at keys + key_off[q] (tmp + key_off[q]),
+// key_stride unused; when an abandon word is set every query counts 0 hits (all offsets 0)
+cudaError_t launch_range_plan_subsets(const RangePlanArgs& a, const int64_t* key_off, cudaStream_t s);
 // launch_segmented_sort over a device plan: a.n_large / a.n_tiles are upper bounds (the plan's sizes give the
 // counts), and hits at CSR positions >= cap are not written
 cudaError_t launch_segmented_sort_dev(const SortArgs& a, const int* sizes, int64_t cap, cudaStream_t s, int* launches);

@@ -615,16 +615,24 @@ cudaError_t launch_scan_collect(const ScanArgs& a, cudaStream_t s) {
 // Each (query, entry) dot is computed as the row scan computes it with one query per pass (QB = 1): the same
 // lane-strided loads, fmaf order and warp_transpose_reduce<4> tree, so row b of a batch equals the one-query
 // subset search bit for bit.  A CTA walks work items (query, tile); it stages a query only when the query changes.
-template <typename T, bool VEC>
-__global__ void __launch_bounds__(kScanThreads) subset_gather_kernel(const SubsetArgs a) {
+// The device-planned form (kDev, tav_search_subsets_into) reads the planned item count and checks each ordinal
+// against [-n_corpus, n_corpus) before it forms a row address: an entry outside sets the status word and row 0 is
+// read in its place (the search is refused).  The <false> instantiation is the host-planned kernel, unchanged.
+struct SubsetDev {
+    const int64_t* n_work;  // device: the planned item count
+    int* status;
+};
+template <typename T, bool VEC, bool kDev>
+__device__ __forceinline__ void subset_gather(const SubsetArgs& a, const SubsetDev& d) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* sq = reinterpret_cast<float*>(smem_raw);
     __shared__ int s_q;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int dim = a.dim;
     const T* corpus = reinterpret_cast<const T*>(a.corpus);
+    const int64_t n_work = kDev ? *d.n_work : a.n_work;
     int cur = -1;
-    for (int64_t w = blockIdx.x; w < a.n_work; w += gridDim.x) {
+    for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
         __syncthreads();  // the previous item is done with s_q and sq
         if (tid == 0) {   // the query of item w: the last q with work0[q] <= w
             int lo = 0, hi = a.nq - 1;
@@ -656,6 +664,10 @@ __global__ void __launch_bounds__(kScanThreads) subset_gather_kernel(const Subse
                 int64_t row = 0;
                 if (pos0 + r < end) {
                     row = a.ordinals[pos0 + r];
+                    if (kDev && (row < -a.n_corpus || row >= a.n_corpus)) {
+                        atomicOr(d.status, kSubsetBadOrdinal);
+                        row = 0;
+                    }
                     if (row < 0) row += a.n_corpus;  // numpy-style negative ordinals
                 }
                 rp[r] = corpus + row * dim;
@@ -720,34 +732,61 @@ __global__ void __launch_bounds__(kScanThreads) subset_gather_kernel(const Subse
     }
 }
 
-template <typename T>
-static cudaError_t launch_subset_gather_t(const SubsetArgs& a, cudaStream_t s) {
-    const size_t row_bytes = static_cast<size_t>(a.dim) * sizeof(T);
-    const bool vec = (row_bytes % 16 == 0) && (reinterpret_cast<uintptr_t>(a.corpus) % 16 == 0);
-    const size_t smem = collect_smem_bytes(1, a.dim);
-    auto kern = vec ? subset_gather_kernel<T, true> : subset_gather_kernel<T, false>;
-    static int granted[2][16] = {};
-    cudaError_t e = ensure_dynamic_smem(kern, smem, granted[vec ? 1 : 0]);
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kScanThreads) subset_gather_kernel(const SubsetArgs a) {
+    subset_gather<T, VEC, false>(a, SubsetDev{});
+}
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kScanThreads) subset_gather_dev_kernel(const SubsetArgs a, const SubsetDev d) {
+    subset_gather<T, VEC, true>(a, d);
+}
+
+// one wave of as many CTAs as fit per SM (at most 4, the row scan's occupancy); the items are grid-strided
+template <typename Kern, typename... Args>
+static cudaError_t launch_gather_wave(Kern kern, int (&granted)[16], size_t smem, int64_t n_work, cudaStream_t s,
+                                      Args... args) {
+    cudaError_t e = ensure_dynamic_smem(kern, smem, granted);
     if (e != cudaSuccess) return e;
-    // one wave of as many CTAs as fit per SM (at most 4, the row scan's occupancy); the items are grid-strided
     int device = 0, sms = 132, per_sm = 1;
     if ((e = cudaGetDevice(&device)) != cudaSuccess) return e;
     if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device)) != cudaSuccess) return e;
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kScanThreads, smem)) != cudaSuccess) return e;
     per_sm = std::max(1, std::min(per_sm, 4));
-    const int grid = static_cast<int>(std::min<int64_t>(a.n_work, static_cast<int64_t>(sms) * per_sm));
-    kern<<<grid, kScanThreads, smem, s>>>(a);
+    const int grid = static_cast<int>(std::min<int64_t>(n_work, static_cast<int64_t>(sms) * per_sm));
+    kern<<<grid, kScanThreads, smem, s>>>(args...);
     return cudaGetLastError();
 }
 
-cudaError_t launch_subset_gather(const SubsetArgs& a, cudaStream_t s) {
+// d: the device-planned form (nullptr: the host-planned one)
+template <typename T>
+static cudaError_t launch_subset_gather_t(const SubsetArgs& a, const SubsetDev* d, cudaStream_t s) {
+    const size_t row_bytes = static_cast<size_t>(a.dim) * sizeof(T);
+    const bool vec = (row_bytes % 16 == 0) && (reinterpret_cast<uintptr_t>(a.corpus) % 16 == 0);
+    const size_t smem = collect_smem_bytes(1, a.dim);
+    static int granted[4][16] = {};
+    int (&g)[16] = granted[(vec ? 1 : 0) + (d ? 2 : 0)];
+    if (d)
+        return launch_gather_wave(vec ? subset_gather_dev_kernel<T, true> : subset_gather_dev_kernel<T, false>, g, smem,
+                                  a.n_work, s, a, *d);
+    return launch_gather_wave(vec ? subset_gather_kernel<T, true> : subset_gather_kernel<T, false>, g, smem, a.n_work, s,
+                              a);
+}
+
+static cudaError_t launch_subset_gather_any(const SubsetArgs& a, const SubsetDev* d, cudaStream_t s) {
     if (a.n_work == 0) return cudaSuccess;
     switch (a.dtype) {
-        case TAV_F32: return launch_subset_gather_t<float>(a, s);
-        case TAV_BF16: return launch_subset_gather_t<__nv_bfloat16>(a, s);
-        case TAV_F16: return launch_subset_gather_t<__half>(a, s);
+        case TAV_F32: return launch_subset_gather_t<float>(a, d, s);
+        case TAV_BF16: return launch_subset_gather_t<__nv_bfloat16>(a, d, s);
+        case TAV_F16: return launch_subset_gather_t<__half>(a, d, s);
     }
     return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_subset_gather(const SubsetArgs& a, cudaStream_t s) { return launch_subset_gather_any(a, nullptr, s); }
+
+cudaError_t launch_subset_gather_dev(const SubsetArgs& a, const int64_t* n_work, int* status, cudaStream_t s) {
+    const SubsetDev d{n_work, status};
+    return launch_subset_gather_any(a, &d, s);
 }
 
 // one CTA per query

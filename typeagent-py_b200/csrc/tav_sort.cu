@@ -385,6 +385,107 @@ cudaError_t launch_range_plan(const RangePlanArgs& a, cudaStream_t s) {
     return cudaGetLastError();
 }
 
+// The plan of the sort of per-query subsets (tav_search_subsets_into): as range_plan_kernel over regions that never
+// overflow, query q's keys (and radix scratch) at keys + key_off[q].  When an abandon word (the search's status) is
+// set the search is refused: every query counts 0 hits, so the offsets are all 0 and nothing is sorted.
+__global__ void __launch_bounds__(kPlanThreads, 1) range_plan_subsets_kernel(const RangePlanArgs a, const int64_t* key_off) {
+    __shared__ int64_t s_warp[65];
+    const bool refused = ((a.abandon[0] && *a.abandon[0]) || (a.abandon[1] && *a.abandon[1]));
+    const int per = (a.nq + kPlanThreads - 1) / kPlanThreads;
+    const int q0 = min(a.nq, static_cast<int>(threadIdx.x) * per), q1 = min(a.nq, q0 + per);
+    int64_t hits = 0, large = 0, tiles = 0;
+    for (int q = q0; q < q1; ++q) {
+        if (refused && TAV_SUBSETS_DEVICE_MUTANT != 3) continue;
+        const int64_t n = a.count[q];
+        hits += n;
+        if (!refused && n > kSmallSortMax) {
+            ++large;
+            tiles += (n + kRadixTile - 1) / kRadixTile;
+        }
+    }
+    int64_t t_hits, t_large, t_tiles;
+    int64_t o_hits = plan_scan(hits, s_warp, &t_hits);
+    int64_t o_large = plan_scan(large, s_warp, &t_large);
+    int64_t o_tiles = plan_scan(tiles, s_warp, &t_tiles);
+    for (int q = q0; q < q1; ++q) {
+        const int64_t n = refused && TAV_SUBSETS_DEVICE_MUTANT != 3 ? 0 : a.count[q];
+        SortSeg g;
+        g.keys = a.keys + key_off[q];
+        g.tmp = a.tmp + key_off[q];
+        g.out = o_hits;
+        g.n = refused ? 0 : n;
+        g.tile0 = o_tiles;
+        a.out_offsets[q] = o_hits;
+        if (g.n > kSmallSortMax) {
+            const int64_t nt = (n + kRadixTile - 1) / kRadixTile;
+            a.large[o_large] = q;
+            a.minmax[2 * o_large] = ~0ull;
+            a.minmax[2 * o_large + 1] = 0ull;
+            for (int64_t t = 0; t < nt; ++t) a.tile_seg[o_tiles + t] = static_cast<int>(o_large);
+            ++o_large;
+            o_tiles += nt;
+        }
+        o_hits += n;
+        a.segs[q] = g;
+    }
+    if (threadIdx.x == 0) {
+        a.out_offsets[a.nq] = t_hits;
+        a.sizes[0] = static_cast<int>(t_large);
+        a.sizes[1] = static_cast<int>(t_tiles);
+    }
+}
+
+cudaError_t launch_range_plan_subsets(const RangePlanArgs& a, const int64_t* key_off, cudaStream_t s) {
+    range_plan_subsets_kernel<<<1, kPlanThreads, 0, s>>>(a, key_off);
+    return cudaGetLastError();
+}
+
+// ---- the work plan of per-query subsets from device offsets (tav_search_subsets_into) ----------------------
+// One CTA; thread t owns the queries [t * per, (t + 1) * per).  The offsets must start at 0, never decrease and end
+// at n_ordinals; otherwise the status word is set and no work is planned, so nothing reads the ordinals.  Query q's
+// work items are its tiles of kSubsetTile entries, [work0[q], work0[q + 1]).
+__global__ void __launch_bounds__(kPlanThreads) subset_plan_kernel(const SubsetPlanArgs a) {
+    __shared__ int64_t s_warp[65];
+    const int per = (a.nq + kPlanThreads - 1) / kPlanThreads;
+    const int q0 = min(a.nq, static_cast<int>(threadIdx.x) * per), q1 = min(a.nq, q0 + per);
+    auto tiles_of = [](int64_t len) {
+        int64_t t = (len + kSubsetTile - 1) / kSubsetTile;
+#if TAV_SUBSETS_DEVICE_MUTANT == 1
+        if (len > 0 && len % kSubsetTile == 0) --t;
+#endif
+        return t;
+    };
+    bool bad = threadIdx.x == 0 && (a.offsets[0] != 0 || a.offsets[a.nq] != a.n_ordinals);
+    int64_t tiles = 0;
+    for (int q = q0; q < q1; ++q) {  // each offset in [0, n_ordinals] first: no difference below can wrap
+        const int64_t lo = a.offsets[q], hi = a.offsets[q + 1];
+        if (lo < 0 || hi > a.n_ordinals || hi < lo) bad = true;
+        else tiles += tiles_of(hi - lo);
+    }
+    if (__syncthreads_or(bad)) {  // CTA-uniform
+        if (threadIdx.x == 0) {
+            atomicOr(a.status, kSubsetBadOffsets);
+            *a.n_work = 0;
+        }
+        return;
+    }
+    int64_t total;
+    int64_t w = plan_scan(tiles, s_warp, &total);
+    for (int q = q0; q < q1; ++q) {
+        a.work0[q] = w;
+        w += tiles_of(a.offsets[q + 1] - a.offsets[q]);
+    }
+    if (threadIdx.x == 0) {
+        a.work0[a.nq] = total;
+        *a.n_work = total;
+    }
+}
+
+cudaError_t launch_subset_plan(const SubsetPlanArgs& a, cudaStream_t s) {
+    subset_plan_kernel<<<1, kPlanThreads, 0, s>>>(a);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_segmented_sort_dev(const SortArgs& a, const int* sizes, int64_t cap, cudaStream_t s, int* launches) {
     const SortBound bd{sizes, cap};
     int n = 0;

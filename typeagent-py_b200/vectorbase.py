@@ -1115,8 +1115,26 @@ class VectorBase:
         self._device_only_rows = tensor.shape[0]
         return self
 
+    @staticmethod
+    def _device_subsets(subsets, n_queries: int, device):
+        """``subsets=(offsets, ordinals)`` of the device forms: contiguous 1-D int64 CUDA tensors on the queries'
+        device, offsets of n_queries + 1 entries (their values are checked on the device)."""
+        import torch
+
+        if not (isinstance(subsets, (tuple, list)) and len(subsets) == 2):
+            raise ValueError("subsets must be (offsets, ordinals) device tensors")
+        offsets, ordinals = subsets
+        for t, what in ((offsets, "offsets"), (ordinals, "ordinals")):
+            if not (getattr(t, "is_cuda", False) and t.dtype == torch.int64 and t.dim() == 1 and t.is_contiguous()):
+                raise ValueError(f"subsets {what} must be a contiguous 1-D int64 CUDA tensor")
+            if t.device != device:
+                raise ValueError(f"subsets {what} is on {t.device}, the queries on {device}")
+        if offsets.numel() != n_queries + 1:
+            raise ValueError(f"subsets offsets must have {n_queries + 1} entries, not {offsets.numel()}")
+        return offsets, ordinals
+
     def search_device(self, queries, k: int, min_score: float = 0.0, item_offset: int = 0, out=None,
-                      defer_check: bool = False, allowed=None, row_to_group=None):
+                      defer_check: bool = False, allowed=None, row_to_group=None, subsets=None):
         """Lookup with torch CUDA tensors as handles, enqueued on torch's current stream:
         queries float32 [B, D] -> (items int64 [B,k], scores float32 [B,k], counts int32 [B]) on
         the device.  The tensor-core path normally ends with one host synchronisation (did any
@@ -1125,7 +1143,13 @@ class VectorBase:
         ``allowed``: row bitmask, or one per query (see ``search_arrays``; here also a contiguous int32 CUDA
         tensor [B, ceil(N / 32)] of packed words, copied on the current stream).  ``row_to_group``: int32 CUDA tensor [N];
         the hits are then folded on the device like the reference's chunk -> message fold
-        (storage/memory/messageindex.py:185-207): first hit per group, items = group ordinals."""
+        (storage/memory/messageindex.py:185-207): first hit per group, items = group ordinals.
+        ``subsets=(offsets, ordinals)``: per-query subsets as ``search_arrays(subsets=)`` takes them, in CSR form as
+        contiguous 1-D int64 CUDA tensors on the queries' device (offsets [B + 1], ordinals [offsets[-1]]); row b
+        equals ``search_arrays(..., subsets=)``'s row b, padded to ``k`` (not clamped: the longest subset is not
+        known on the host).  The offsets and ordinals are checked on the device: malformed offsets raise
+        ``ValueError`` and an ordinal outside [-N, N) ``IndexError``, from this call, or with ``defer_check=True``
+        from ``finish_search()`` (the call then makes no host synchronisation)."""
         self._single_device_only("search_device")
         import torch
 
@@ -1133,8 +1157,14 @@ class VectorBase:
             raise ValueError("queries must be a contiguous float32 CUDA tensor")
         if queries.dim() != 2 or queries.shape[1] != self._embedding_size:
             raise ValueError("query width does not match the embedding size")
-        lib, ix = self._ensure_device()
         b = queries.shape[0]
+        if subsets is not None:
+            if allowed is not None or row_to_group is not None or item_offset:
+                raise ValueError("subsets= cannot be combined with allowed=, row_to_group= or an item_offset")
+            if k < 1:
+                raise ValueError("k must be >= 1")
+            subsets = self._device_subsets(subsets, b, queries.device)
+        lib, ix = self._ensure_device()
         if out is None:
             dev = queries.device
             out = (
@@ -1154,6 +1184,23 @@ class VectorBase:
             self._use_row_mask(lib, ix, allowed)
             flags |= _capi.TAV_USE_ROW_MASK
         floor = float(np.float32(min_score))
+        if subsets is not None:
+            offsets, ordinals = subsets
+            flags &= _capi.TAV_QUERIES_ON_DEVICE | _capi.TAV_OUTPUTS_ON_DEVICE | _capi.TAV_DEFER_RETRY
+            # the hits pass through the index's threshold-search buffers
+            with self._single_lock:
+                _capi.check(
+                    lib.tav_search_subsets_into(
+                        ix, C.c_void_p(queries.data_ptr()), b, k, C.c_float(floor), flags,
+                        C.c_void_p(offsets.data_ptr()), C.c_void_p(ordinals.data_ptr()), ordinals.numel(),
+                        C.c_void_p(items.data_ptr()), C.c_void_p(scores.data_ptr()), C.c_void_p(counts.data_ptr()),
+                        C.c_void_p(stream),
+                    )
+                )
+            if flags & _capi.TAV_DEFER_RETRY:
+                # the device works on these tensors until finish_search(): keep them alive
+                self._pending.append((queries, items, scores, counts, stream, subsets))
+            return items, scores, counts
         _capi.check(
             lib.tav_search(ix, C.c_void_p(queries.data_ptr()), b, k, C.c_float(floor),
                            flags, None, 0, item_offset, C.c_void_p(items.data_ptr()),
@@ -1175,7 +1222,7 @@ class VectorBase:
 
     def search_range_device(self, queries, min_score: float = 0.0, capacity: int | None = None, *, out=None,
                             defer_check: bool = False, allowed=None, ties_low_first: bool = False, subset=None,
-                            expected_hits: int | None = None, item_offset: int = 0):
+                            expected_hits: int | None = None, item_offset: int = 0, subsets=None):
         """Threshold search with torch CUDA tensors as handles, enqueued on torch's current stream: every row whose
         score is >= min_score, per query, as ``search_range`` finds them, into device tensors
         (offsets int64 [B + 1], items int64 [capacity], scores float32 [capacity]).  The offsets are always
@@ -1186,7 +1233,10 @@ class VectorBase:
         [B, D]; ``allowed`` as in ``search_device``; ``subset``: host ordinals as in ``search_range``.
         ``expected_hits`` (default ``capacity``) sizes the device collect regions; it never changes the result.
         The call synchronises once (more when a query overflowed its region); with ``defer_check=True`` it does
-        not synchronise at all, and ``finish_search()`` must run before the results are trusted."""
+        not synchronise at all, and ``finish_search()`` must run before the results are trusted.
+        ``subsets=(offsets, ordinals)``: per-query subsets from device tensors as in ``search_device``; the result
+        equals ``search_range(..., subsets=)``'s (``expected_hits`` is not used).  A refused search (malformed
+        offsets: ``ValueError``; an ordinal outside [-N, N): ``IndexError``) leaves all offsets 0."""
         self._single_device_only("search_range_device")
         import torch
 
@@ -1222,6 +1272,10 @@ class VectorBase:
         if isinstance(expected_hits, bool) or int(expected_hits) != expected_hits or expected_hits < 0:
             raise ValueError(f"expected_hits must be a non-negative integer, not {expected_hits!r}")
         sub = None
+        if subsets is not None:
+            if subset is not None or allowed is not None or item_offset:
+                raise ValueError("subsets= cannot be combined with subset=, allowed= or an item_offset")
+            subsets = self._device_subsets(subsets, b, dev)
         if subset is not None:
             if allowed is not None:
                 raise ValueError("allowed= and subset= cannot be combined")
@@ -1247,6 +1301,21 @@ class VectorBase:
         if ties_low_first:
             flags |= _capi.TAV_TIES_LOW_FIRST
         floor = float(_as_f32_scalar(min_score))
+        if subsets is not None:
+            s_offsets, s_ordinals = subsets
+            flags &= _capi.TAV_QUERIES_ON_DEVICE | _capi.TAV_DEFER_RETRY | _capi.TAV_TIES_LOW_FIRST
+            with self._single_lock:
+                _capi.check(
+                    lib.tav_range_search_subsets_into(
+                        ix, C.c_void_p(queries.data_ptr()), b, C.c_float(floor), flags,
+                        C.c_void_p(s_offsets.data_ptr()), C.c_void_p(s_ordinals.data_ptr()), s_ordinals.numel(),
+                        capacity, C.c_void_p(offsets.data_ptr()), C.c_void_p(items.data_ptr()),
+                        C.c_void_p(scores.data_ptr()), C.c_void_p(stream),
+                    )
+                )
+            if defer_check:
+                self._pending.append((queries, items, scores, offsets, stream, subsets))
+            return offsets, items, scores
         # the call gives up the index's threshold-search hits: not between a search_range and its fetch
         with self._single_lock:
             _capi.check(
@@ -1265,7 +1334,8 @@ class VectorBase:
     def finish_search(self) -> int:
         """Complete every outstanding ``search_device(..., defer_check=True)`` and
         ``search_range_device(..., defer_check=True)``: synchronise, redo (exactly) the queries the device search
-        flagged, return how many there were."""
+        flagged, return how many there were.  A deferred ``subsets=`` search that the device checks refused raises
+        here (``ValueError`` / ``IndexError``), after every other outstanding search has been completed."""
         self._single_device_only("finish_search")
         if not self._pending:
             return 0
