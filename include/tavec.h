@@ -621,6 +621,53 @@ int tav_multi_range_fetch(tav_multi* m, int64_t first, int64_t n, int64_t* out_i
 int tav_fold_groups(int device, int n_queries, int k, const int32_t* row_to_group, int64_t n_rows,
                     int64_t item_offset, int64_t* items, float* scores, int32_t* counts, void* stream);
 
+/*
+ * Grouped lookups: the k best GROUPS of rows (messages, when rows are their chunks), each group scored by its best
+ * row.  Exact, unlike tav_fold_groups after a top-k, which returns fewer than k groups when the best rows of a few
+ * groups fill the k slots.  Definition: take query q's hit list of tav_range_search with the same min_score, masks
+ * and tie order; a group's LEADER is its first row in that list; the grouped result is the list of leaders in that
+ * order (group id, the leader's score, the leader's row).  So groups come by score descending, equal scores with
+ * the higher leader row first (the lower with TAV_TIES_LOW_FIRST), a group with no passing row does not appear, and
+ * the grouped top-k is the first k entries of the grouped threshold search.
+ *
+ * tav_set_row_groups: groups[r] (int32 [n_rows], host or device memory) is the group of row r; n_rows must equal
+ * tav_size(), and n_rows == 0 clears the map.  Values must lie in [0, 2^31): a negative one gives TAV_ERR_INVALID
+ * and leaves the index as it was.  The map is copied into library-owned device memory and checked there by a kernel
+ * (one synchronisation).  Lifecycle and call order of the row mask: outstanding TAV_DEFER_RETRY searches are
+ * finished first; tav_clear, tav_adopt_device, tav_remove_rows and a rebalance commit drop the map, appends
+ * invalidate it, tav_write_rows keeps it.
+ *
+ * tav_range_search_groups: every group's leader per query, CSR offsets out_offsets [n_queries + 1] (host, or device
+ * with TAV_OUTPUTS_ON_DEVICE).  The collection, path choice, sizing, hint, re-pass and fp16-range fallback of
+ * tav_range_search, then the leader reduction (each query's keys through an open-addressing table of twice their
+ * count), then the segmented sort over the leaders only.  The leaders stay in the index until the next threshold
+ * search; tav_range_fetch_groups copies leaders [first, first + n) out (host, or device with TAV_OUTPUTS_ON_DEVICE):
+ * out_groups int64, out_scores float32, out_rows int64.  After any other threshold search: TAV_ERR_STATE.
+ * Synchronises twice (the hit counts, then the leader counts).
+ *
+ * tav_search_groups: out_groups / out_scores / out_rows [n_queries, k], out_counts [n_queries]; padding group -1,
+ * score 0, row -1.  It runs tav_search for the top kp rows of each query (kp = k times the rows per run of equal
+ * group ids in the map, at most 2048 and at least k; the path choice of tav_search), reduces that prefix to its
+ * leaders and sorts them.  A prefix's leaders are the first leaders of the whole list, so a query whose prefix is
+ * all its hits, or holds k groups, is exact; every other query is redone by the grouped threshold search of that
+ * query alone and cut to k, and *redone (may be NULL) reports how many.  When kp covers the rows the grouped
+ * threshold search serves the whole call.  Synchronises (to size the leaders and the redo); replaces the hits of
+ * the last threshold search.
+ *
+ * Flags of the three searches: TAV_QUERIES_ON_DEVICE, TAV_OUTPUTS_ON_DEVICE, TAV_FORCE_SCAN, TAV_FORCE_MMA,
+ * TAV_USE_ROW_MASK, TAV_USE_QUERY_MASKS, TAV_TIES_LOW_FIRST; any other flag: TAV_ERR_INVALID.  No current map (none
+ * set, or set for another row count) on a non-empty index: TAV_ERR_STATE.  An empty index or a NaN min_score gives
+ * no hits.
+ */
+int tav_set_row_groups(tav_index* ix, const int32_t* groups, int64_t n_rows, int on_device, void* stream);
+int tav_range_search_groups(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
+                            int64_t expected_hits, int64_t* out_offsets, void* stream);
+int tav_range_fetch_groups(tav_index* ix, int64_t first, int64_t n, int64_t* out_groups, float* out_scores,
+                           int64_t* out_rows, int flags, void* stream);
+int tav_search_groups(tav_index* ix, const float* queries, int n_queries, int k, float min_score, int flags,
+                      int64_t* out_groups, float* out_scores, int64_t* out_rows, int32_t* out_counts, void* stream,
+                      int* redone);
+
 /* Verification aid for the tensor-core path: every raw dot product it computes,
  * out_device[n_queries, size] float32 (device memory); float32 indexes go through their fp16 planes.  `flags` may
  * carry TAV_QUERIES_ON_DEVICE.  On a TAV_NORMALIZE index the queries are normalised first, as a search

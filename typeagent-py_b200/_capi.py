@@ -70,6 +70,13 @@ SIGNATURES = {
     "tav_set_query_masks": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p]),
     "tav_fold_groups": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tav_set_row_groups": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
+    "tav_range_search_groups": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int64, C.c_void_p,
+                                          C.c_void_p]),
+    "tav_range_fetch_groups": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                         C.c_void_p]),
+    "tav_search_groups": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
     "tav_group_handle_bytes": (C.c_int, []),
     "tav_group_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "tav_group_local_handle": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -20,7 +20,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libtavec.so")
 STAMP = os.path.join(HERE, ".libtavec.stamp")
 SOURCES = ["tav_api.cu", "tav_scan.cu", "tav_mma.cu", "tav_group.cu", "tav_sort.cu", "tav_merge_range.cu",
-           "tav_compact.cu", "tav_multi.cu"]
+           "tav_compact.cu", "tav_multi.cu", "tav_leaders.cu"]
 HEADERS = ["tav_common.cuh", "tav_internal.h", "tav_ptx.cuh", "../../include/tavec.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

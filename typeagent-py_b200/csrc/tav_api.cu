@@ -219,6 +219,16 @@ struct tav_index {
     DevBuf range_mmaws, range_mmaws2, range_mmaaux;  // tensor-core collection: workspaces, scratch
     DevBuf range_items, range_scores;
     int64_t range_total = 0;     // hits of the last range search held in range_items / range_scores
+    bool range_grouped = false;  // ... and they are the leaders of a tav_range_search_groups (tav_range_fetch_groups)
+    // grouped lookups (tav_set_row_groups): the group of every row (group_stage holds an upload until it is checked),
+    // and the runs of equal consecutive values, which size the top-k prefix of tav_search_groups
+    DevBuf group_map, group_stage, group_stat;
+    int64_t group_rows = 0;      // 0 = no map
+    int64_t group_runs = 0;
+    // leader reduction: segments, open-addressing tables, leader counters; the top-k prefix and its keys
+    DevBuf group_segs, group_table, group_counts, group_topk, group_keys, group_csr;
+    DevBuf range_groups;         // the groups of the leaders in range_items (tav_range_search_groups)
+    DevBuf group_res;            // tav_search_groups with host outputs: [groups | rows | scores | counts]
     bool range_replaced = false; // a tav_range_search_into ran after it: tav_range_fetch has nothing to copy
     // per-query subsets: device [offsets | work-item starts | CSR offsets of the hits], each n_queries + 1
     DevBuf subsets_meta;
@@ -496,6 +506,7 @@ int tav_clear(tav_index* ix) {
     ix->split_rows = 0;
     ix->row_mask_rows = 0;
     ix->qmask_n = 0;
+    ix->group_rows = 0;
     return TAV_OK;
 }
 
@@ -603,6 +614,7 @@ int tav_adopt_device(tav_index* ix, void* device_rows, int64_t n, int dim) {
     ix->split_rows = 0;  // (the planes' overflow flag is reset where they are rebuilt from row 0)
     ix->row_mask_rows = 0;
     ix->qmask_n = 0;
+    ix->group_rows = 0;
     ix->adopted = true;
     ix->size = n;
     ix->capacity = n;
@@ -1329,6 +1341,56 @@ static int range_sort(tav_index* ix, TimedSearch* ts, bool timing, std::vector<S
     return TAV_OK;
 }
 
+// Grouped lookups: every segment's keys -> the keys of its groups' leaders (tav_leaders.cu), compacted in place;
+// segs[q].n, segs[q].out and offsets become the leaders' counts and CSR offsets.  One synchronisation, to learn the
+// counts.  Scratch: 12 bytes per table slot, a power of two >= twice the segment's keys.
+static int reduce_leaders(tav_index* ix, TimedSearch* ts, bool timing, std::vector<SortSeg>& segs,
+                          std::vector<int64_t>& offsets, int ties_low, cudaStream_t s) {
+    const int nq = static_cast<int>(segs.size());
+    std::vector<LeaderSeg> ls(static_cast<size_t>(nq));
+    int64_t slots = 0, key_tiles = 0, slot_tiles = 0;
+    for (int q = 0; q < nq; ++q) {
+        const int64_t n = segs[q].n;
+        if (n > (int64_t(1) << 31)) {
+            set_error("grouped search: %lld hits of one query are more than the leader reduction takes", (long long)n);
+            return TAV_ERR_INVALID;
+        }
+        int64_t t = n ? 2 : 0;
+        while (t && t < 2 * n) t <<= 1;
+        ls[q] = LeaderSeg{segs[q].keys, n, slots, static_cast<uint32_t>(t - 1), key_tiles, slot_tiles};
+        slots += t;
+        key_tiles += (n + kLeaderTileKeys - 1) / kLeaderTileKeys;
+        slot_tiles += (t + kLeaderTileKeys - 1) / kLeaderTileKeys;
+    }
+    if (int rc = range_alloc(ix->group_segs, ls.size() * sizeof(LeaderSeg), "the leader segments")) return rc;
+    if (int rc = range_alloc(ix->group_table, static_cast<size_t>(slots) * 12, "the leader tables")) return rc;
+    if (int rc = range_alloc(ix->group_counts, static_cast<size_t>(nq) * sizeof(uint32_t), "the leader counters"))
+        return rc;
+    uint64_t* tkey = static_cast<uint64_t*>(ix->group_table.p);
+    int32_t* tgroup = reinterpret_cast<int32_t*>(tkey + slots);
+    uint32_t* d_cnt = static_cast<uint32_t*>(ix->group_counts.p);
+    // from pageable memory: consumed when the call returns
+    TAV_CUDA(cudaMemcpyAsync(ix->group_segs.p, ls.data(), ls.size() * sizeof(LeaderSeg), cudaMemcpyHostToDevice, s));
+    TAV_CUDA(cudaMemsetAsync(tkey, 0, static_cast<size_t>(slots) * sizeof(uint64_t), s));
+    TAV_CUDA(cudaMemsetAsync(tgroup, 0xFF, static_cast<size_t>(slots) * sizeof(int32_t), s));
+    TAV_CUDA(cudaMemsetAsync(d_cnt, 0, static_cast<size_t>(nq) * sizeof(uint32_t), s));
+    TAV_CUDA(timed_launch(ix, ts, timing, 2, s, [&] {
+        return launch_leaders(static_cast<const LeaderSeg*>(ix->group_segs.p), nq, key_tiles, slot_tiles,
+                              static_cast<const int32_t*>(ix->group_map.p), ties_low, tgroup, tkey, d_cnt, s);
+    }));
+    ts->launches += 2;
+    std::vector<uint32_t> cnt(static_cast<size_t>(nq));
+    TAV_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaStreamSynchronize(s));
+    offsets.assign(static_cast<size_t>(nq) + 1, 0);
+    for (int q = 0; q < nq; ++q) {
+        offsets[q + 1] = offsets[q] + cnt[q];
+        segs[q].n = cnt[q];
+        segs[q].out = offsets[q];
+    }
+    return TAV_OK;
+}
+
 // the masks of a re-pass over the gathered queries `over` (indexes into the search whose masks are qm)
 static int gather_mask_map(tav_index* ix, const std::vector<int>& over, const QueryMasks& qm, QueryMasks& out,
                            cudaStream_t s) {
@@ -1358,7 +1420,7 @@ static int gather_repass_queries(tav_index* ix, const float* d_queries, const st
 static int range_collect_scan(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
                               const int64_t* d_subset, int64_t n_scan, int64_t item_offset, const uint32_t* d_mask,
                               int ties_low, int64_t expected_hits, std::vector<int64_t>& offsets, cudaStream_t s,
-                              int positions = 0, QueryMasks qm = QueryMasks{}) {
+                              int positions = 0, QueryMasks qm = QueryMasks{}, bool leaders = false) {
     const int64_t per = range_per_query(expected_hits, nq, n_scan);
     if (int rc = range_alloc(ix->range_keys, static_cast<size_t>(nq) * per * sizeof(uint64_t), "the hit regions")) return rc;
     if (int rc = range_alloc(ix->range_counts, static_cast<size_t>(nq) * sizeof(uint32_t), "the hit counters")) return rc;
@@ -1407,6 +1469,8 @@ static int range_collect_scan(tav_index* ix, TimedSearch* ts, bool timing, const
         segs[q].out = offsets[q];
         segs[q].n = cnt[q];
     }
+    if (leaders)
+        if (int rc = reduce_leaders(ix, ts, timing, segs, offsets, ties_low, s)) return rc;
     return range_sort(ix, ts, timing, segs, offsets[nq], positions ? nullptr : d_subset, item_offset, ties_low, s);
 }
 
@@ -1419,7 +1483,7 @@ constexpr int kRangeUseScan = 1;  // range_collect_mma: the tensor-core form can
 // a value beyond the fp16 range (the exact row scan then serves the search, as it does for top-k searches).
 static int range_collect_mma(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
                              int64_t item_offset, const uint32_t* d_mask, int ties_low, int64_t expected_hits,
-                             std::vector<int64_t>& offsets, cudaStream_t s, QueryMasks qm) {
+                             std::vector<int64_t>& offsets, cudaStream_t s, QueryMasks qm, bool leaders) {
     const bool split = ix->dtype == TAV_F32;
     if (split) {
         const int rc = ensure_split_planes(ix, ts, s);
@@ -1531,23 +1595,26 @@ static int range_collect_mma(tav_index* ix, TimedSearch* ts, bool timing, const 
         segs[q].out = offsets[q];
         segs[q].n = host[q];
     }
-    return range_sort(ix, ts, timing, segs, total, nullptr, item_offset, ties_low, s);
+    if (leaders)
+        if (int rc = reduce_leaders(ix, ts, timing, segs, offsets, ties_low, s)) return rc;
+    return range_sort(ix, ts, timing, segs, offsets[nq], nullptr, item_offset, ties_low, s);
 }
 
 // Every row with score >= floor, for each of nq device queries -> ix->range_items / range_scores in CSR order
 // (offsets[nq + 1], host): collected by the tensor cores (use_mma) or the row scan, then the segmented sort.
+// `leaders` (grouped lookups): only each group's leader is sorted (reduce_leaders), offsets count the leaders.
 static int range_core(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
                       const int64_t* d_subset, int64_t n_scan, int64_t item_offset, const uint32_t* d_mask,
                       int ties_low, int64_t expected_hits, bool use_mma, std::vector<int64_t>& offsets, cudaStream_t s,
-                      int positions = 0, QueryMasks qm = QueryMasks{}) {
+                      int positions = 0, QueryMasks qm = QueryMasks{}, bool leaders = false) {
     if (use_mma) {
         const int rc = range_collect_mma(ix, ts, timing, d_queries, nq, floor, item_offset, d_mask, ties_low,
-                                         expected_hits, offsets, s, qm);
+                                         expected_hits, offsets, s, qm, leaders);
         if (rc != kRangeUseScan) return rc;
         ts->path = 1;  // a value beyond the fp16 range: the exact row scan serves the search
     }
     return range_collect_scan(ix, ts, timing, d_queries, nq, floor, d_subset, n_scan, item_offset, d_mask, ties_low,
-                              expected_hits, offsets, s, positions, qm);
+                              expected_hits, offsets, s, positions, qm, leaders);
 }
 
 // ---- threshold search into caller buffers (tav_range_search_into) ----------------------------------------
@@ -2066,6 +2133,7 @@ int tav_remove_rows(tav_index* ix, const int64_t* ordinals, int64_t n, void* str
     ix->split_recheck = true;
     ix->qmask_n = 0;
     ix->row_mask_rows = 0;  // ordinals changed meaning (a later append can restore the old size)
+    ix->group_rows = 0;
     return TAV_OK;
 }
 
@@ -2330,6 +2398,7 @@ int tav_rows_commit(tav_index* ix, int commit) {
     ix->split_rows = TAV_REBALANCE_MUTANT == 2 ? std::min(ix->split_rows, ix->size) : 0;
     ix->split_recheck = false;
     if (TAV_REBALANCE_MUTANT != 3) ix->row_mask_rows = 0;  // ordinals changed meaning
+    ix->group_rows = 0;
     ix->qmask_n = 0;
     return TAV_OK;
 }
@@ -2361,6 +2430,11 @@ int tav_finish_search(tav_index* ix, void* stream, int* redone) {
     return rc;
 }
 
+// tav_search with the index's mutex held (tav_search_groups runs it as its first step)
+static int search_locked(tav_index* ix, const float* queries, int n_queries, int k, float min_score, int flags,
+                         const int64_t* subset, int64_t subset_len, int64_t item_offset, int64_t* out_items,
+                         float* out_scores, int32_t* out_counts, void* stream);
+
 int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float min_score,
                int flags, const int64_t* subset, int64_t subset_len, int64_t item_offset,
                int64_t* out_items, float* out_scores, int32_t* out_counts, void* stream) {
@@ -2371,6 +2445,13 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     if (int rc = check_subset_args("tav_search", flags, subset, subset_len, false)) return rc;
     if (n_queries == 0) return TAV_OK;
     std::lock_guard<std::mutex> lock(ix->mu);
+    return search_locked(ix, queries, n_queries, k, min_score, flags, subset, subset_len, item_offset, out_items,
+                         out_scores, out_counts, stream);
+}
+
+static int search_locked(tav_index* ix, const float* queries, int n_queries, int k, float min_score, int flags,
+                         const int64_t* subset, int64_t subset_len, int64_t item_offset, int64_t* out_items,
+                         float* out_scores, int32_t* out_counts, void* stream) {
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (int rc = enter_stream(ix, s)) return rc;
     const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
@@ -2434,6 +2515,7 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
             return rc;
         std::vector<int64_t> offsets;
         ix->range_total = 0;
+        ix->range_grouped = false;
         ix->range_replaced = false;
         if (int rc = range_core(ix, ts, timing, d_q, n_queries, min_score, d_sub, n_scan, item_offset, d_mask, ties_low,
                                 static_cast<int64_t>(n_queries) * n_scan, false, offsets, s, positions, qm))
@@ -2692,6 +2774,19 @@ int tav_search(tav_index* ix, const float* queries, int n_queries, int k, float 
     return TAV_OK;
 }
 
+// path choice of the threshold search, as in tav_search: tensor cores for batches (no subset), the row scan otherwise
+static int range_path(const tav_index* ix, const char* fn, int n_queries, int flags, bool has_subset, bool* use_mma) {
+    const bool mma_able = (mma_supported(ix->dtype, ix->dim) || (ix->dtype == TAV_F32 && mma_split_supported(ix->dim))) &&
+                          !has_subset && n_queries <= kMmaMaxQueries && ix->size < (1ll << 31);
+    *use_mma = !(flags & TAV_FORCE_SCAN) && mma_able &&
+               ((flags & TAV_FORCE_MMA) || (n_queries >= 16 && ix->size >= 4096));
+    if ((flags & TAV_FORCE_MMA) && !*use_mma) {
+        set_error("%s: TAV_FORCE_MMA needs dim %% 8 == 0, no subset, at most %d queries", fn, kMmaMaxQueries);
+        return TAV_ERR_INVALID;
+    }
+    return TAV_OK;
+}
+
 int tav_range_search(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
                      const int64_t* subset, int64_t subset_len, int64_t item_offset, int64_t expected_hits,
                      int64_t* out_offsets, void* stream) {
@@ -2705,6 +2800,7 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
     if (int rc = enter_stream(ix, s)) return rc;  // (also: a queued tav_range_fetch reads the hits replaced here)
     const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
     ix->range_total = 0;
+    ix->range_grouped = false;
     ix->range_replaced = false;
     std::vector<int64_t> offsets(static_cast<size_t>(n_queries) + 1, 0);
     const uint32_t* d_mask = nullptr;
@@ -2719,15 +2815,8 @@ int tav_range_search(tav_index* ix, const float* queries, int n_queries, float m
         return TAV_ERR_INVALID;
     }
     if (int rc = check_subset_ordinals(ix, subset, subset_len)) return rc;
-    // path choice as in tav_search: tensor cores for batches (no subset), the row scan otherwise
-    const bool mma_able = (mma_supported(ix->dtype, ix->dim) || (ix->dtype == TAV_F32 && mma_split_supported(ix->dim))) &&
-                          !subset && n_queries <= kMmaMaxQueries && ix->size < (1ll << 31);
-    const bool use_mma = !(flags & TAV_FORCE_SCAN) && mma_able &&
-                         ((flags & TAV_FORCE_MMA) || (n_queries >= 16 && ix->size >= 4096));
-    if ((flags & TAV_FORCE_MMA) && !use_mma) {
-        set_error("tav_range_search: TAV_FORCE_MMA needs dim %% 8 == 0, no subset, at most %d queries", kMmaMaxQueries);
-        return TAV_ERR_INVALID;
-    }
+    bool use_mma = false;
+    if (int rc = range_path(ix, "tav_range_search", n_queries, flags, subset != nullptr, &use_mma)) return rc;
     TimedSearch* ts = begin_search(ix, use_mma ? (ix->dtype == TAV_F32 ? 3 : 2) : 1);
     const bool timing = ts != &ix->untimed;
     const float* d_queries = nullptr;
@@ -2773,6 +2862,292 @@ int tav_range_fetch(tav_index* ix, int64_t first, int64_t n, int64_t* out_items,
     return TAV_OK;
 }
 
+// ---- grouped lookups: the k best groups of rows, each scored by its best row ------------------------------
+int tav_set_row_groups(tav_index* ix, const int32_t* groups, int64_t n_rows, int on_device, void* stream) {
+    if (!ix || n_rows < 0 || (n_rows > 0 && !groups)) {
+        set_error("tav_set_row_groups: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(ix->mu);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = enter_stream(ix, s)) return rc;  // queued searches read the old map
+    if (int rc = finish_pending(ix, s, nullptr)) return rc;
+    if (n_rows == 0) {
+        ix->group_rows = 0;
+        return TAV_OK;
+    }
+    if (n_rows != ix->size) {
+        set_error("tav_set_row_groups: %lld groups for an index of %lld rows", (long long)n_rows, (long long)ix->size);
+        return TAV_ERR_INVALID;
+    }
+    // into the stage, checked there: a refused map leaves the current one in place
+    const size_t bytes = static_cast<size_t>(n_rows) * sizeof(int32_t);
+    TAV_CUDA(ix->group_stage.ensure(bytes));
+    TAV_CUDA(ix->group_stat.ensure(2 * sizeof(uint64_t)));
+    TAV_CUDA(cudaMemcpyAsync(ix->group_stage.p, groups, bytes,
+                             on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
+    TAV_CUDA(cudaMemsetAsync(ix->group_stat.p, 0, 2 * sizeof(uint64_t), s));
+    TAV_CUDA(launch_group_check(static_cast<const int32_t*>(ix->group_stage.p), n_rows,
+                                static_cast<uint64_t*>(ix->group_stat.p), s));
+    uint64_t stat[2] = {0, 0};
+    TAV_CUDA(cudaMemcpyAsync(stat, ix->group_stat.p, sizeof(stat), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaStreamSynchronize(s));
+    mark_done(ix);
+    if (stat[0]) {
+        set_error("tav_set_row_groups: a group is negative (groups must lie in [0, 2^31))");
+        return TAV_ERR_INVALID;
+    }
+    std::swap(ix->group_map, ix->group_stage);
+    ix->group_rows = n_rows;
+    ix->group_runs = static_cast<int64_t>(stat[1]);
+    return TAV_OK;
+}
+
+static int check_groups(const tav_index* ix, const char* fn) {
+    if (ix->group_rows == 0 || ix->group_rows != ix->size) {
+        set_error("%s: no current group map (tav_set_row_groups after the last change of the rows)", fn);
+        return TAV_ERR_STATE;
+    }
+    return TAV_OK;
+}
+
+constexpr int kGroupFlags = TAV_QUERIES_ON_DEVICE | TAV_OUTPUTS_ON_DEVICE | TAV_FORCE_SCAN | TAV_FORCE_MMA |
+                            TAV_USE_ROW_MASK | TAV_USE_QUERY_MASKS | TAV_TIES_LOW_FIRST;
+
+// The grouped threshold search of nq device queries: the leaders in ix->range_items (rows) / range_scores and their
+// groups in ix->range_groups, CSR offsets[nq + 1] on the host.
+static int range_groups_core(tav_index* ix, TimedSearch* ts, bool timing, const float* d_queries, int nq, float floor,
+                             const uint32_t* d_mask, const QueryMasks& qm, int ties_low, int64_t expected_hits,
+                             bool use_mma, std::vector<int64_t>& offsets, cudaStream_t s) {
+    if (int rc = range_core(ix, ts, timing, d_queries, nq, floor, nullptr, ix->size, 0, d_mask, ties_low, expected_hits,
+                            use_mma, offsets, s, 0, qm, true))
+        return rc;
+    const int64_t total = offsets[nq];
+    if (int rc = range_alloc(ix->range_groups, static_cast<size_t>(total) * sizeof(int64_t), "the hit groups")) return rc;
+    TAV_CUDA(launch_group_decode(total, static_cast<const int64_t*>(ix->range_items.p),
+                                 static_cast<const int32_t*>(ix->group_map.p), static_cast<int64_t*>(ix->range_groups.p), s));
+    ts->launches += total > 0;
+    return TAV_OK;
+}
+
+int tav_range_search_groups(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
+                            int64_t expected_hits, int64_t* out_offsets, void* stream) {
+    if (!ix || n_queries < 0 || expected_hits < 0 || !out_offsets || (n_queries > 0 && !queries) ||
+        (flags & ~kGroupFlags)) {
+        set_error("tav_range_search_groups: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(ix->mu);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = enter_stream(ix, s)) return rc;  // (also: a queued fetch reads the hits replaced here)
+    const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
+    ix->range_total = 0;
+    ix->range_grouped = false;
+    ix->range_replaced = false;
+    std::vector<int64_t> offsets(static_cast<size_t>(n_queries) + 1, 0);
+    const uint32_t* d_mask = nullptr;
+    QueryMasks qm;
+    if (int rc = resolve_masks(ix, "tav_range_search_groups", n_queries, flags, false, &d_mask, &qm)) return rc;
+    if (ix->size > 0)
+        if (int rc = check_groups(ix, "tav_range_search_groups")) return rc;
+    if (n_queries == 0 || ix->size == 0 || ix->dim == 0 || min_score != min_score)
+        return deliver_offsets(ix, offsets, out_offsets, o_dev, s);
+    if (ix->size > 0xFFFFFFFFll) {
+        set_error("tav_range_search_groups: more than 2^32 rows per index are not supported; shard the corpus");
+        return TAV_ERR_INVALID;
+    }
+    bool use_mma = false;
+    if (int rc = range_path(ix, "tav_range_search_groups", n_queries, flags, false, &use_mma)) return rc;
+    TimedSearch* ts = begin_search(ix, use_mma ? (ix->dtype == TAV_F32 ? 3 : 2) : 1);
+    const bool timing = ts != &ix->untimed;
+    const float* d_queries = nullptr;
+    const int64_t* d_subset = nullptr;
+    if (int rc = stage_inputs(ix, ts, timing, queries, n_queries, q_dev, false, nullptr, 0, &d_queries, &d_subset, s))
+        return rc;
+    if (int rc = range_groups_core(ix, ts, timing, d_queries, n_queries, min_score, d_mask, qm,
+                                   (flags & TAV_TIES_LOW_FIRST) ? 1 : 0, expected_hits, use_mma, offsets, s))
+        return rc;
+    if (int rc = end_search(ix, ts, s)) return rc;
+    ix->range_total = offsets[n_queries];
+    ix->range_grouped = true;
+    return deliver_offsets(ix, offsets, out_offsets, o_dev, s);
+}
+
+int tav_range_fetch_groups(tav_index* ix, int64_t first, int64_t n, int64_t* out_groups, float* out_scores,
+                           int64_t* out_rows, int flags, void* stream) {
+    if (!ix || first < 0 || n < 0 || (n > 0 && (!out_groups || !out_scores || !out_rows)) ||
+        (flags & ~TAV_OUTPUTS_ON_DEVICE)) {
+        set_error("tav_range_fetch_groups: invalid argument");
+        return TAV_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(ix->mu);
+    if (!ix->range_grouped) {
+        set_error("tav_range_fetch_groups: the last threshold search was not a tav_range_search_groups");
+        return TAV_ERR_STATE;
+    }
+    if (first + n > ix->range_total) {
+        set_error("tav_range_fetch_groups: leaders [%lld, %lld) out of range (the last grouped search has %lld)",
+                  (long long)first, (long long)(first + n), (long long)ix->range_total);
+        return TAV_ERR_RANGE;
+    }
+    if (n == 0) return TAV_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = enter_stream(ix, s)) return rc;  // after the search that wrote the leaders
+    const cudaMemcpyKind kind = (flags & TAV_OUTPUTS_ON_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    TAV_CUDA(cudaMemcpyAsync(out_groups, static_cast<const int64_t*>(ix->range_groups.p) + first,
+                             static_cast<size_t>(n) * sizeof(int64_t), kind, s));
+    TAV_CUDA(cudaMemcpyAsync(out_scores, static_cast<const float*>(ix->range_scores.p) + first,
+                             static_cast<size_t>(n) * sizeof(float), kind, s));
+    TAV_CUDA(cudaMemcpyAsync(out_rows, static_cast<const int64_t*>(ix->range_items.p) + first,
+                             static_cast<size_t>(n) * sizeof(int64_t), kind, s));
+    if (flags & TAV_OUTPUTS_ON_DEVICE) return mark_queued(ix, s);
+    TAV_CUDA(cudaStreamSynchronize(s));
+    mark_done(ix);
+    return TAV_OK;
+}
+
+// [nq, k] of grouped results from CSR leaders in ix->range_items / range_scores (host offsets), rows [q0, q0 + nq)
+// of the result arrays: the first min(k, leaders) of each query, then group -1, score 0, row -1
+static int group_layout(tav_index* ix, const std::vector<int64_t>& offsets, int k, int q0, int64_t* groups,
+                        float* scores, int64_t* rows, int32_t* counts, cudaStream_t s) {
+    const int nq = static_cast<int>(offsets.size()) - 1;
+    if (int rc = range_alloc(ix->group_csr, offsets.size() * sizeof(int64_t), "the leader offsets")) return rc;
+    // from pageable memory: consumed when the call returns
+    TAV_CUDA(cudaMemcpyAsync(ix->group_csr.p, offsets.data(), offsets.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    const size_t at = static_cast<size_t>(q0) * k;
+    TAV_CUDA(launch_subset_topk_layout(nq, k, static_cast<const int64_t*>(ix->group_csr.p),
+                                       static_cast<const int64_t*>(ix->range_items.p),
+                                       static_cast<const float*>(ix->range_scores.p), rows + at, scores + at, counts + q0, s));
+    TAV_CUDA(launch_group_decode(static_cast<int64_t>(nq) * k, rows + at, static_cast<const int32_t*>(ix->group_map.p),
+                                 groups + at, s));
+    return TAV_OK;
+}
+
+int tav_search_groups(tav_index* ix, const float* queries, int n_queries, int k, float min_score, int flags,
+                      int64_t* out_groups, float* out_scores, int64_t* out_rows, int32_t* out_counts, void* stream,
+                      int* redone) {
+    if (!ix || n_queries < 0 || k < 1 || (flags & ~kGroupFlags) ||
+        (n_queries > 0 && (!queries || !out_groups || !out_scores || !out_rows || !out_counts))) {
+        set_error("tav_search_groups: invalid argument (k must be >= 1)");
+        return TAV_ERR_INVALID;
+    }
+    if (redone) *redone = 0;
+    if (n_queries == 0) return TAV_OK;
+    std::lock_guard<std::mutex> lock(ix->mu);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = enter_stream(ix, s)) return rc;
+    const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, o_dev = flags & TAV_OUTPUTS_ON_DEVICE;
+    const int ties_low = (flags & TAV_TIES_LOW_FIRST) ? 1 : 0;
+    const uint32_t* d_mask = nullptr;
+    QueryMasks qm;
+    if (int rc = resolve_masks(ix, "tav_search_groups", n_queries, flags, false, &d_mask, &qm)) return rc;
+    if (ix->size > 0)
+        if (int rc = check_groups(ix, "tav_search_groups")) return rc;
+    if (ix->size > 0xFFFFFFFFll) {
+        set_error("tav_search_groups: more than 2^32 rows per index are not supported; shard the corpus");
+        return TAV_ERR_INVALID;
+    }
+    // the results on the device: the caller's arrays, or a staging of [groups | rows | scores | counts]
+    const size_t nk = static_cast<size_t>(n_queries) * k;
+    int64_t *groups = out_groups, *rows = out_rows;
+    float* scores = out_scores;
+    int32_t* counts = out_counts;
+    if (!o_dev) {
+        TAV_CUDA(ix->group_res.ensure(nk * (2 * sizeof(int64_t) + sizeof(float)) + n_queries * sizeof(int32_t)));
+        groups = static_cast<int64_t*>(ix->group_res.p);
+        rows = groups + nk;
+        scores = reinterpret_cast<float*>(rows + nk);
+        counts = reinterpret_cast<int32_t*>(scores + nk);
+    }
+    int n_redone = 0;
+    if (ix->size == 0 || ix->dim == 0 || min_score != min_score) {  // no hits
+        TAV_CUDA(cudaMemsetAsync(groups, 0xFF, nk * sizeof(int64_t), s));
+        TAV_CUDA(cudaMemsetAsync(rows, 0xFF, nk * sizeof(int64_t), s));
+        TAV_CUDA(cudaMemsetAsync(scores, 0, nk * sizeof(float), s));
+        TAV_CUDA(cudaMemsetAsync(counts, 0, n_queries * sizeof(int32_t), s));
+    } else {
+        // The top-kp prefix of the hit list: its groups' first rows are the first leaders of the whole list, so
+        // a query whose prefix is all of its hits, or holds k groups, is answered exactly by the prefix.  kp is k
+        // times the rows per run of equal group ids (the map's mean multiplicity for contiguous groups), at most one
+        // pass of the top-k kernels.  A prefix that covers the rows is the grouped threshold search itself.
+        const int64_t mult = std::max<int64_t>(1, (ix->size + ix->group_runs - 1) / std::max<int64_t>(1, ix->group_runs));
+        const int64_t kp = std::min<int64_t>(ix->size, std::max<int64_t>(k, std::min<int64_t>(kPassK, k * mult)));
+        const bool prefix = kp < ix->size && !((flags & TAV_FORCE_MMA) && kp > kPassK);
+        ix->range_total = 0;  // the leaders pass through the threshold search's buffers
+        ix->range_grouped = false;
+        ix->range_replaced = false;
+        TimedSearch aux;  // the prefix search keeps the timing record; the steps after it are not timed
+        std::vector<int64_t> offsets;
+        std::vector<int> flagged;
+        if (prefix) {
+            const size_t nkp = static_cast<size_t>(n_queries) * kp;
+            TAV_CUDA(ix->group_topk.ensure(nkp * (sizeof(int64_t) + sizeof(float)) + n_queries * sizeof(int32_t)));
+            int64_t* p_rows = static_cast<int64_t*>(ix->group_topk.p);
+            float* p_scores = reinterpret_cast<float*>(p_rows + nkp);
+            int32_t* p_counts = reinterpret_cast<int32_t*>(p_scores + nkp);
+            if (int rc = search_locked(ix, queries, n_queries, static_cast<int>(kp), min_score,
+                                       flags | TAV_OUTPUTS_ON_DEVICE, nullptr, 0, 0,
+                                       p_rows, p_scores, p_counts, stream))
+                return rc;
+            if (int rc = range_alloc(ix->group_keys, nkp * sizeof(uint64_t), "the prefix keys")) return rc;
+            uint64_t* keys = static_cast<uint64_t*>(ix->group_keys.p);
+            TAV_CUDA(launch_topk_keys(n_queries, static_cast<int>(kp), p_rows, p_scores, p_counts, ties_low, keys, s));
+            std::vector<int32_t> cnt(static_cast<size_t>(n_queries));
+            TAV_CUDA(cudaMemcpyAsync(cnt.data(), p_counts, cnt.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+            TAV_CUDA(cudaStreamSynchronize(s));
+            std::vector<SortSeg> segs(static_cast<size_t>(n_queries));
+            for (int q = 0; q < n_queries; ++q) {
+                segs[q].keys = keys + static_cast<size_t>(q) * kp;
+                segs[q].n = cnt[q];
+            }
+            if (int rc = reduce_leaders(ix, &aux, false, segs, offsets, ties_low, s)) return rc;
+            for (int q = 0; q < n_queries; ++q)
+                if (cnt[q] == kp && offsets[q + 1] - offsets[q] < k) flagged.push_back(q);
+            if (int rc = range_sort(ix, &aux, false, segs, offsets[n_queries], nullptr, 0, ties_low, s)) return rc;
+        } else {
+            bool use_mma = false;
+            if (int rc = range_path(ix, "tav_search_groups", n_queries, flags, false, &use_mma)) return rc;
+            TimedSearch* ts = begin_search(ix, use_mma ? (ix->dtype == TAV_F32 ? 3 : 2) : 1);
+            const bool timing = ts != &ix->untimed;
+            const float* d_q = nullptr;
+            const int64_t* d_sub = nullptr;
+            if (int rc = stage_inputs(ix, ts, timing, queries, n_queries, q_dev, false, nullptr, 0, &d_q, &d_sub, s))
+                return rc;
+            if (int rc = range_groups_core(ix, ts, timing, d_q, n_queries, min_score, d_mask, qm, ties_low, 0, use_mma,
+                                           offsets, s))
+                return rc;
+            if (int rc = end_search(ix, ts, s)) return rc;
+        }
+        if (int rc = group_layout(ix, offsets, k, 0, groups, scores, rows, counts, s)) return rc;
+        // a query whose prefix held fewer than k groups: its grouped threshold search, alone (the row scan), cut to k
+        for (int q : flagged) {
+            const float* d_q = nullptr;
+            const int64_t* d_sub = nullptr;
+            if (int rc = stage_inputs(ix, &aux, false, queries + static_cast<size_t>(q) * ix->dim, 1, q_dev, false,
+                                      nullptr, 0, &d_q, &d_sub, s))
+                return rc;
+            const uint32_t* mask = qm.bits ? qm.bits + static_cast<size_t>(q) * qm.stride : d_mask;
+            std::vector<int64_t> off1;
+            if (int rc = range_groups_core(ix, &aux, false, d_q, 1, min_score, mask, QueryMasks{}, ties_low, 0, false,
+                                           off1, s))
+                return rc;
+            if (int rc = group_layout(ix, off1, k, q, groups, scores, rows, counts, s)) return rc;
+        }
+        n_redone = static_cast<int>(flagged.size());
+        ix->range_total = 0;
+        ix->range_grouped = false;
+    }
+    if (redone) *redone = n_redone;
+    if (o_dev) return mark_queued(ix, s);
+    TAV_CUDA(cudaMemcpyAsync(out_groups, groups, nk * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaMemcpyAsync(out_rows, rows, nk * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaMemcpyAsync(out_scores, scores, nk * sizeof(float), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaMemcpyAsync(out_counts, counts, n_queries * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    TAV_CUDA(cudaStreamSynchronize(s));
+    mark_done(ix);
+    return TAV_OK;
+}
+
 int tav_range_search_into(tav_index* ix, const float* queries, int n_queries, float min_score, int flags,
                           const int64_t* subset, int64_t subset_len, int64_t item_offset, int64_t expected_hits,
                           int64_t capacity, int64_t* out_offsets, int64_t* out_items, float* out_scores, void* stream) {
@@ -2789,6 +3164,7 @@ int tav_range_search_into(tav_index* ix, const float* queries, int n_queries, fl
     if (int rc = enter_stream(ix, s)) return rc;
     const bool q_dev = flags & TAV_QUERIES_ON_DEVICE, defer = flags & TAV_DEFER_RETRY;
     ix->range_total = 0;  // the hits of the last tav_range_search are given up (the sort scratch is reused)
+    ix->range_grouped = false;
     ix->range_replaced = true;
     const uint32_t* d_mask = nullptr;
     QueryMasks qm;
@@ -3032,6 +3408,7 @@ static int subsets_into(tav_index* ix, const char* fn, const float* queries, int
         if (int rc = stage_inputs(ix, ts, timing, queries, nq, true, true, nullptr, 0, &d_queries, &no_subset, s, held))
             return rc;
         ix->range_total = 0;  // the hits of the last tav_range_search are given up (the sort scratch is reused)
+        ix->range_grouped = false;
         ix->range_replaced = true;
         // device [work0 | CSR offsets of the top-k form's hits | planned work items]
         const size_t n1 = static_cast<size_t>(nq) + 1;
@@ -3149,6 +3526,7 @@ int tav_search_subsets(tav_index* ix, const float* queries, int n_queries, int k
     const bool timing = ts != &ix->untimed;
     std::vector<int64_t> csr;
     ix->range_total = 0;  // the hits land in the threshold search's buffers
+    ix->range_grouped = false;
     ix->range_replaced = false;
     if (int rc = subsets_core(ix, ts, timing, queries, n_queries, flags, min_score, offsets, ordinals, csr, s))
         return rc;
@@ -3190,6 +3568,7 @@ int tav_range_search_subsets(tav_index* ix, const float* queries, int n_queries,
         if (int rc = check_subset_ordinals(ix, ordinals, total)) return rc;
     std::vector<int64_t> csr(static_cast<size_t>(n_queries) + 1, 0);
     ix->range_total = 0;
+    ix->range_grouped = false;
     ix->range_replaced = false;
     if (!none) {
         TimedSearch* ts = begin_search(ix, 1);

@@ -227,6 +227,33 @@ cudaError_t launch_range_plan_subsets(const RangePlanArgs& a, const int64_t* key
 // counts), and hits at CSR positions >= cap are not written
 cudaError_t launch_segmented_sort_dev(const SortArgs& a, const int* sizes, int64_t cap, cudaStream_t s, int* launches);
 
+// ---- grouped lookups (tav_leaders.cu) ----------------------------------------------------
+// Leader reduction of one query's unsorted keys (n of them at `keys`): its open-addressing table is the slot_mask + 1
+// (a power of two >= 2n, or 0 slots when n == 0) slots from slot0 of the shared table, and its tiles of the flat key
+// (slot) space start at key_tile0 (slot_tile0).  The segments are in ascending tile order.
+constexpr int kLeaderTileKeys = 4096;
+struct LeaderSeg {
+    uint64_t* keys;
+    int64_t n;
+    int64_t slot0;
+    uint32_t slot_mask;
+    int64_t key_tile0;
+    int64_t slot_tile0;
+};
+// every segment's keys -> the keys of its groups' leaders (groups[position of the key]), compacted in place, in no
+// order; counts[q] (zero on entry) = its leaders.  tgroup (-1) and tkey (0) are the table, initialised by the caller.
+cudaError_t launch_leaders(const LeaderSeg* segs, int nq, int64_t key_tiles, int64_t slot_tiles, const int32_t* groups,
+                           int ties_low, int32_t* tgroup, uint64_t* tkey, uint32_t* counts, cudaStream_t s);
+// the group map's check: stat[0] (zero on entry) |= 1 when some value is negative, stat[1] (zero on entry) += the
+// runs of equal consecutive values
+cudaError_t launch_group_check(const int32_t* groups, int64_t n, uint64_t* stat, cudaStream_t s);
+// [nq, k] top-k rows / scores / counts -> the library's keys of each query's hits at keys + q * k
+cudaError_t launch_topk_keys(int nq, int k, const int64_t* rows, const float* scores, const int32_t* counts,
+                             int ties_low, uint64_t* keys, cudaStream_t s);
+// out_groups[i] = groups[rows[i]] for rows[i] >= 0, else -1
+cudaError_t launch_group_decode(int64_t n, const int64_t* rows, const int32_t* groups, int64_t* out_groups,
+                                cudaStream_t s);
+
 struct SelectArgs {
     const uint64_t* cand_keys;   // [nq, cand_stride]
     int cand_stride;

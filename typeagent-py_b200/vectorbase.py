@@ -184,6 +184,9 @@ class VectorBase:
         self._qmask_ref = None               # ... and the mask object itself (so its id() cannot be recycled)
         self._predicate_masks: dict = {}     # (id(predicate), generation, n) -> packed bitmask
         self._range_hint = 0                 # hits of the last search_range: the next one's capacity hint
+        self._groups_key = None              # identity of the group map currently on the device
+        self._groups_ref = None              # ... and the map object itself (so its id() cannot be recycled)
+        self.last_redone = 0                 # queries the last search_groups redid by the grouped threshold search
         self.clear()
 
     # ------------------------------------------------------------------ housekeeping
@@ -375,6 +378,7 @@ class VectorBase:
         self._mask_ref = None
         self._qmask_key = None
         self._qmask_ref = None
+        self._groups_key = None
         self._predicate_masks.clear()
 
     def _replace_rebalanced(self, rows: np.ndarray) -> None:
@@ -392,6 +396,7 @@ class VectorBase:
         self._mask_ref = None
         self._qmask_key = None
         self._qmask_ref = None
+        self._groups_key = None
         self._predicate_masks.clear()
 
     def remove_embedding_at(self, pos: int) -> None:
@@ -476,9 +481,11 @@ class VectorBase:
             self._ix_generation = self._generation
             self._mask_key = None
             self._qmask_key = None
+            self._groups_key = None
         if self._ix_rows < self._count:
             self._mask_key = None
             self._qmask_key = None
+            self._groups_key = None
             fresh = np.ascontiguousarray(self._buf[self._ix_rows : self._count])
             _capi.check(
                 lib.tav_append(self._ix, fresh.ctypes.data_as(C.c_void_p), len(fresh),
@@ -839,6 +846,175 @@ class VectorBase:
         breakdown = [(names.get(kinds[i], "?"), ms[i]) for i in range(min(n.value, 64))]
         return {"scan_ms": scan.value, "total_ms": total.value, "launches": launches.value,
                 "path": {1: "scan", 2: "mma", 3: "mma_split"}.get(path.value, "none"), "kernels": breakdown}
+
+    # ------------------------------------------------------------------ grouped lookups
+    def _check_groups(self, groups):
+        """``groups`` -> what ``tav_set_row_groups`` takes: a contiguous int32 array, or the contiguous int32 CUDA
+        tensor itself (its values are checked on the device).  ValueError for a wrong length, a non-integer dtype,
+        a shape other than 1-D or a value outside [0, 2^31)."""
+        n = len(self)
+        if getattr(groups, "is_cuda", False):
+            import torch
+
+            if not (groups.dtype == torch.int32 and groups.dim() == 1 and groups.is_contiguous()):
+                raise ValueError("device groups must be a contiguous 1-D int32 CUDA tensor")
+            if groups.device.index != self._device:
+                raise ValueError(f"device groups are on cuda:{groups.device.index}, the index on cuda:{self._device}")
+            if groups.shape[0] != n:
+                raise ValueError(f"groups has {groups.shape[0]} entries for {n} rows")
+            return groups
+        a = np.asarray(groups)
+        if a.ndim != 1:
+            raise ValueError(f"groups must be one-dimensional, not of shape {a.shape}")
+        if len(a) != n:
+            raise ValueError(f"groups has {len(a)} entries for {n} rows")
+        if a.size == 0:
+            return np.zeros(0, dtype=np.int32)
+        if not np.issubdtype(a.dtype, np.integer):
+            raise ValueError(f"groups must be integers, not {a.dtype}")
+        if int(a.min()) < 0 or int(a.max()) >= 2**31:
+            raise ValueError("groups must lie in [0, 2^31)")
+        return np.ascontiguousarray(a, dtype=np.int32)
+
+    def _groups_arg(self, groups):
+        """(cache key, checked map or None when it is the map on the device): the checks run before any device work."""
+        key = (id(groups), self._generation, len(self))
+        return key, None if key == self._groups_key else self._check_groups(groups)
+
+    def _use_groups(self, lib, ix, groups, key, checked) -> None:
+        """Upload the group map unless it is the one on the device (identity + row generation + rows, as masks)."""
+        if self._groups_key == key:
+            return
+        self._groups_key = None
+        g = self._check_groups(groups) if checked is None else checked
+        if getattr(g, "is_cuda", False):
+            import torch
+
+            stream = torch.cuda.current_stream(g.device).cuda_stream
+            _capi.check(lib.tav_set_row_groups(ix, C.c_void_p(g.data_ptr()), len(self), 1, C.c_void_p(stream)))
+        else:
+            _capi.check(lib.tav_set_row_groups(ix, g.ctypes.data_as(C.c_void_p), len(self), 0, None))
+        self._groups_key = key
+        self._groups_ref = groups
+
+    def _group_flags(self, lib, ix, allowed, ties_low_first: bool, n_queries: int) -> int:
+        flags = self._flags() & ~_capi.TAV_NO_FUSED_SCAN
+        if self._is_query_masks(allowed):
+            self._use_query_masks(lib, ix, allowed, n_queries)
+            flags |= _capi.TAV_USE_QUERY_MASKS
+        elif allowed is not None:
+            self._use_row_mask(lib, ix, allowed)
+            flags |= _capi.TAV_USE_ROW_MASK
+        if ties_low_first:
+            flags |= _capi.TAV_TIES_LOW_FIRST
+        return flags
+
+    def search_groups(
+        self,
+        queries: np.ndarray,
+        k: int,
+        groups,
+        min_score: float = 0.0,
+        allowed: np.ndarray | None = None,
+        ties_low_first: bool = False,
+    ) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+        """Grouped top-k: the k best groups of rows per query, each scored by its best row (its leader).
+        ``groups`` gives the group of every row (a 1-D integer array or sequence of ``len(self)`` values in
+        [0, 2^31), or a contiguous int32 CUDA tensor on the index's device); it is uploaded once and reused while
+        the same object is passed and the rows do not change.  Row b equals the first occurrence of every group in
+        row b of ``search_range`` (same ``min_score``, ``allowed``, ``ties_low_first``), cut to k.  Returns group ids
+        int64 [B, k], scores float32 [B, k], leader rows int64 [B, k] and counts int32 [B]; padding is group -1,
+        score 0, row -1.  `k` is clamped to the number of rows.  ``last_redone`` holds the number of queries whose
+        top rows held fewer than k groups and were answered by the grouped threshold search."""
+        self._single_device_only("search_groups")
+        q = self._check_queries(queries)
+        b = len(q)
+        if k < 1:
+            raise ValueError("k must be >= 1")
+        key, checked = self._groups_arg(groups)
+        n = len(self)
+        k_eff = max(1, min(k, n))
+        group_ids = np.full((b, k_eff), -1, dtype=np.int64)
+        scores = np.zeros((b, k_eff), dtype=np.float32)
+        rows = np.full((b, k_eff), -1, dtype=np.int64)
+        counts = np.zeros(b, dtype=np.int32)
+        self.last_redone = 0
+        floor = _as_f32_scalar(min_score)
+        if b == 0 or n == 0 or np.isnan(floor):
+            return group_ids, scores, rows, counts
+        redone = C.c_int(0)
+        with self._single_lock:  # the leaders pass through the index's threshold-search buffers
+            lib, ix = self._ensure_device()
+            self._use_groups(lib, ix, groups, key, checked)
+            flags = self._group_flags(lib, ix, allowed, ties_low_first, b)
+            _capi.check(
+                lib.tav_search_groups(
+                    ix, q.ctypes.data_as(C.c_void_p), b, k_eff, C.c_float(float(floor)), flags,
+                    group_ids.ctypes.data_as(C.c_void_p), scores.ctypes.data_as(C.c_void_p),
+                    rows.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), None, C.byref(redone),
+                )
+            )
+        self.last_redone = redone.value
+        return group_ids, scores, rows, counts
+
+    def search_range_groups(
+        self,
+        queries: np.ndarray,
+        groups,
+        min_score: float = 0.0,
+        allowed: np.ndarray | None = None,
+        ties_low_first: bool = False,
+    ) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+        """Grouped threshold search: every group with a row at or above ``min_score``, per query, each once, in
+        the order of its leader (its first row in ``search_range``'s list).  ``groups``, ``allowed`` and
+        ``ties_low_first`` as in ``search_groups``.  Returns CSR arrays offsets int64 [B + 1], group ids int64 [T],
+        scores float32 [T] and leader rows int64 [T]."""
+        self._single_device_only("search_range_groups")
+        q = self._check_queries(queries)
+        b = len(q)
+        key, checked = self._groups_arg(groups)
+        offsets = np.zeros(b + 1, dtype=np.int64)
+        floor = _as_f32_scalar(min_score)
+        if b == 0 or len(self) == 0 or np.isnan(floor):
+            return offsets, np.empty(0, np.int64), np.empty(0, np.float32), np.empty(0, np.int64)
+        with self._single_lock:  # the leaders wait in the index's buffers until they are fetched
+            lib, ix = self._ensure_device()
+            self._use_groups(lib, ix, groups, key, checked)
+            flags = self._group_flags(lib, ix, allowed, ties_low_first, b)
+            _capi.check(
+                lib.tav_range_search_groups(ix, q.ctypes.data_as(C.c_void_p), b, C.c_float(float(floor)), flags,
+                                            self._range_hint, offsets.ctypes.data_as(C.c_void_p), None)
+            )
+            total = int(offsets[-1])
+            group_ids = np.empty(total, dtype=np.int64)
+            scores = np.empty(total, dtype=np.float32)
+            rows = np.empty(total, dtype=np.int64)
+            if total:
+                _capi.check(lib.tav_range_fetch_groups(ix, 0, total, group_ids.ctypes.data_as(C.c_void_p),
+                                                       scores.ctypes.data_as(C.c_void_p),
+                                                       rows.ctypes.data_as(C.c_void_p), 0, None))
+        return offsets, group_ids, scores, rows
+
+    def fuzzy_lookup_embedding_grouped(
+        self,
+        embedding,
+        groups,
+        max_hits: int | None = None,
+        min_score: float | None = None,
+    ) -> list[ScoredInt]:
+        """``fuzzy_lookup_embedding`` over groups of rows (messages made of chunks): the ``max_hits`` best groups,
+        each as ``ScoredInt(group, score of its best row)``, exactly (see ``search_groups``).  The defaults follow
+        ``fuzzy_lookup_embedding``: ``max_hits=None`` means 10, ``0`` every group; ``min_score=None`` means 0."""
+        self._single_device_only("fuzzy_lookup_embedding_grouped")
+        if min_score is None:
+            min_score = 0.0
+        n = len(self)
+        k = self._resolve_k(max_hits, n)
+        if n == 0:
+            self._check_groups(groups)
+            return []
+        group_ids, scores, _, counts = self.search_groups(embedding, k, groups, min_score)
+        return [ScoredInt(int(group_ids[0, i]), float(scores[0, i])) for i in range(int(counts[0]))]
 
     # ------------------------------------------------------------------ lookups
     @staticmethod
